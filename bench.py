@@ -2,10 +2,10 @@
 """Headline benchmark: tokens/sec of one Long-VITA prefill forward (ViT tower + projector + 48-layer
 14B decoder + masked LM head) on synthetic frames, through the HF `forward()` surface.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--frames F]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--frames F] [--dump-outputs DIR]
 
 A "step" is one full prefill of the configured prompt.  N = 1: BASELINE.json configs[1]
-("Long-VITA-16K bf16 single B200, 64 synthetic frames -> 16K tokens").  Launched under torchrun
+("Long-VITA-16K bf16 single H100, 64 synthetic frames -> 16K tokens").  Launched under torchrun
 for N > 1 (one rank per GPU); see DESIGN.md for what each N runs.  Rank 0 prints ONE JSON line.
 
 `--impl reference` times the reference's own CPU implementation of the path - the oracle port
@@ -51,7 +51,8 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:  # noqa: BLE001
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # H100 SXM data sheet (dense bf16, HBM3): an upper bound, not a measured rate
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "fallback"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -215,9 +216,9 @@ def attn_128k_probe(ops, dev, pk, launches: int = 3):
     ach = flops / (ms / 1000.0) / 1e12
     burst, sust = pk["bf16_tflops"], pk.get("bf16_tflops_sustained", pk["bf16_tflops"])
     return {"bound": "tensor", "kernel": "attn_fwd (standalone, S=131072, 40:8x128 causal)", "achieved": ach, "peak": burst,
-            "unit": "TFLOP/s", "frac": ach / burst, "frac_sustained": ach / sust, "frac_of_2250_datasheet": ach / 2250.0,
+            "unit": "TFLOP/s", "frac": ach / burst, "frac_sustained": ach / sust, "frac_of_989_datasheet": ach / 989.0,
             "launches": launches, "avg_launch_ms": ms, "flops_per_launch": flops,
-            "inputs": "2.7 GB Q+O, 0.5 GB K+V per launch (far beyond the 126 MB L2)"}
+            "inputs": "2.7 GB Q+O, 0.5 GB K+V per launch (far beyond the 50 MB L2)"}
 
 
 def cp_parity_probe(model, runner, S, dev, n_rows: int = 64):
@@ -287,18 +288,6 @@ def cp_parity_probe(model, runner, S, dev, n_rows: int = 64):
     return float(worst[0]), float(worst[1]), float(worst[2]), bool(flag.item() > 0.5)
 
 
-def ncu_traffic(kind: str):
-    """DRAM bytes per launch of the dominant kernel from the committed `ncu --set full` capture of this same command
-    (profiles/ncu_traffic.json, written by tools/ncu_summary.py; dram__bytes_read.sum + dram__bytes_write.sum averaged
-    over the captured launches).  None when no capture is committed for that kernel."""
-    try:
-        t = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        e = t.get(kind)
-        return (e["dram_bytes_per_launch"], e["source"]) if e else (None, None)
-    except Exception:  # noqa: BLE001
-        return None, None
-
-
 # ------------------------------------------------------------------------------------------------
 def main():
     ap = argparse.ArgumentParser()
@@ -315,6 +304,9 @@ def main():
                     help="minutes-per-step configs (1M tokens): honour --warmup < 3 and skip the separate e2e pass; "
                          "the printed line is then marked as outside the timing contract")
     ap.add_argument("--layers", type=int, default=None, help="debug: fewer decoder layers (number is then INVALID)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (the kept logits) as "
+                         "DIR/<name>.npy in float32, so that two builds can be compared output for output")
     args = ap.parse_args()
     # stdout carries exactly ONE JSON line: everything libraries print meanwhile (e.g. NCCL's
     # "NCCL version ..." banner, written to fd 1 from C) is routed to stderr until the line is emitted
@@ -345,7 +337,7 @@ def main():
                 f"({args.frames * 256} visual + {2 * args.frames} delimiter tokens) + text, padded to {S} tokens")
     config = {"workload": workload, "frames": args.frames, "tokens": S, "layers": cfg.num_hidden_layers,
               "parallelism": f"cp{cp}" if cp > 1 else "single",
-              "l2": "per-step working set (29.5 GB weights + activations) far exceeds the 126 MB L2"}
+              "l2": "per-step working set (29.5 GB weights + activations) far exceeds the 50 MB L2"}
 
     if args.impl == "reference":
         if rank != 0:
@@ -468,11 +460,23 @@ def main():
     timer = ops.KernelTimer()
     ops.set_kernel_timer(timer)
     n0 = ops.launch_count()
-    ms_resident = timed(lambda: forward_resident(images_d, ids_d, idx_d), args.steps)
+    last_out = {}
+
+    def step_resident():
+        last_out["logits"] = forward_resident(images_d, ids_d, idx_d)
+
+    ms_resident = timed(step_resident, args.steps)
     log(f"timed region done: {ms_resident / args.steps:.1f} ms/step")
     launches = ops.launch_count() - n0
     ops.set_kernel_timer(None)
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in last_out.items():
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.detach().float().cpu().numpy())
+        log(f"outputs of the last timed step written to {args.dump_outputs}: {sorted(last_out)}")
     ksum = timer.summary()
     # e2e: host buffers, H2D + forward + D2H inside the timed region
     if args.long_run:
@@ -503,7 +507,7 @@ def main():
         return {"bound": "tensor", "kernel": kind, "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
                 "peak_source": f"{pk_kind} sustained cuBLAS bf16 (kernel timed inside a long step)",
                 "launches_per_step": d["launches"] / args.steps, "avg_launch_ms": d["ms"] / d["launches"],
-                "share_of_step": d["ms"] / ms_resident, "traffic": ncu_traffic(kind)[0], "traffic_source": ncu_traffic(kind)[1],
+                "share_of_step": d["ms"] / ms_resident,
                 "algorithmic_bytes_or_flops_per_launch": d["flops"] / d["launches"]}
 
     dominant = max(ksum, key=lambda k_: ksum[k_]["ms"]) if ksum else None

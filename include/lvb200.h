@@ -1,5 +1,5 @@
 /*
- * lvb200.h - C ABI of the B200-native Long-VITA hot path (long-context forward / backward).
+ * lvb200.h - C ABI of the H100-native Long-VITA hot path (long-context forward / backward).
  *
  * This is the drop-in boundary (SURVEY.md section 8, row B5).  The reference has no native layer: on
  * GPU it reaches flash-attn 2, TransformerEngine, apex and cuBLAS through Python.  Every entry

@@ -1,8 +1,7 @@
-"""Build liblvb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build liblvb200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 The library has no Python / torch dependency: `nvcc -shared` over long-vita_b200/csrc/*.cu with the
-static CUDA runtime.  The built artefact lives at long-vita_b200/lib/liblvb200.so (git-ignored,
-shipped to the GPU box by gpurun).
+static CUDA runtime.  The built artefact lives at long-vita_b200/lib/liblvb200.so (git-ignored).
 """
 from __future__ import annotations
 
@@ -20,7 +19,7 @@ OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "liblvb200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -30,7 +29,7 @@ NVCC_FLAGS = [
 
 if os.environ.get("LV_WATCHDOG") == "1":      # debug build: stuck waits report themselves and trap (csrc/ptx.cuh)
     NVCC_FLAGS.append("-DLV_WATCHDOG")
-if os.environ.get("LV_EXTRA_DEFINES"):         # experiment builds, e.g. LV_EXTRA_DEFINES="-DLV_ATTN_QBUF64=2"
+if os.environ.get("LV_EXTRA_DEFINES"):         # experiment builds: extra nvcc -D flags, space separated
     NVCC_FLAGS.extend(os.environ["LV_EXTRA_DEFINES"].split())
 
 
@@ -46,8 +45,8 @@ def _sources():
 
 
 def _digest(paths) -> str:
-    """Content hash of the sources (file names, not absolute paths: gpurun runs the snapshot from another
-    directory, and the library built here must be accepted there instead of being rebuilt on GPU time)."""
+    """Content hash of the sources (file names, not absolute paths: a copy of the tree in another directory
+    accepts the library built here instead of rebuilding it)."""
     h = hashlib.sha256()
     for p in sorted(paths, key=os.path.basename):
         with open(p, "rb") as f:

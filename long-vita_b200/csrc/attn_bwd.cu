@@ -1,19 +1,12 @@
-// Attention backward for sm_100a (tcgen05 / TMEM / TMA), deterministic two-pass formulation:
+// Attention backward for sm_90a (wgmma / TMA), deterministic two-pass formulation:
 //
 //   prep   : delta[b,h,i] = sum_d dO[b,i,h,d] * O[b,i,h,d]                         (HBM-bound)
 //   pass A : dK, dV.  One CTA owns a 128-row K/V tile (resident in shared memory) and streams the
-//            Q / dO tiles of every query head of its GQA group that can see it:
-//                S^T  = K Q^T,   dP^T = V dO^T            (SS UMMA, accumulators in TMEM)
-//                P^T  = exp2(S^T * scale_log2 - lse2[q]),  dS^T = P^T * (dP^T - delta[q]) * scale
-//                dV  += P^T dO,  dK += dS^T Q             (TS UMMA: A = P^T / dS^T read from TMEM)
-//   pass B : dQ.  One CTA owns a 128-row Q / dO tile and streams the K / V tiles it can see:
-//                S = Q K^T,  dP = dO V^T,  dS = P * (dP - delta[i]) * scale,  dQ += dS K
+//            Q / dO tiles of every query head of its GQA group that can see it.
+//   pass B : dQ.  One CTA owns a 128-row Q / dO tile and streams the K / V tiles it can see.
 //
 // Recomputing S in both passes costs 7 GEMM-units instead of the minimal 5, but needs no atomics
-// (bit-reproducible dQ), no dQ transposes and fits TMEM (pass A: S^T dP^T dV dK = 512 columns).
-// This first version is synchronous inside a CTA (TMA prefetch of the next streamed tile is the
-// only overlap); it exists for correctness + coverage of the training path and is the kernel to
-// pipeline next (see DESIGN.md).
+// (bit-reproducible dQ) and no dQ transposes.
 //
 // Replaces flash-attn 2's backward, reached in the reference through autograd of
 // flash_attn_func / TE AttnFuncWithCP (dot_product_attention.py:318-326, 374-390).
@@ -40,18 +33,6 @@ struct BwdKParams {
   const float* delta;   // [b, hq, sq]
 };
 
-__device__ __forceinline__ long long q_tile_pos(const BwdKParams& p, int qt) {
-  const int row0 = qt * 128;
-  const int seg = row0 / p.q_seg_len;
-  return (seg == 0 ? p.q_seg_pos0 : p.q_seg_pos1) + (row0 - seg * p.q_seg_len);
-}
-
-// a (q tile, kv tile) pair contributes unless it is entirely above the causal diagonal
-__device__ __forceinline__ bool pair_visible(const BwdKParams& p, int qt, int kt) {
-  if (!p.causal) return true;
-  return p.kv_pos0 + (long long)kt * 128 <= q_tile_pos(p, qt) + 127;
-}
-
 // delta = rowsum(dO * O)
 __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const __nv_bfloat16* __restrict__ o,
                                                             const __nv_bfloat16* __restrict__ d_o, float* __restrict__ delta,
@@ -77,740 +58,330 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const __nv_bfloat16*
   if (lane == 0) delta[((long long)b * hq + h) * sq + i] = acc;
 }
 
-// MODE 0: dK/dV pass (resident = K,V tile; streamed = Q,dO tiles).  MODE 1: dQ pass.
-template <int D, int MODE>
-__global__ void __launch_bounds__(128, 1)
-    attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                    const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                    const __grid_constant__ CUtensorMap tmOut0, const __grid_constant__ CUtensorMap tmOut1,
-                    const BwdKParams p) {
-  constexpr int TILE = 128 * D * 2;
-  constexpr int BOXES = D / 64;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sR0 = smem;                 // resident operand 0 (K or Q)
-  uint8_t* sR1 = sR0 + TILE;           // resident operand 1 (V or dO)
-  uint8_t* sS0 = sR1 + TILE;           // streamed operand 0, 2 stages (Q or K)
-  uint8_t* sS1 = sS0 + 2 * TILE;       // streamed operand 1, 2 stages (dO or V)
-  float* s_lse = reinterpret_cast<float*>(sS1 + 2 * TILE);   // [2][128]  (MODE 0 only)
-  float* s_dlt = s_lse + 256;                               // [2][128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_dlt + 256);
-  uint64_t* res_full = bars;        // resident tiles landed
-  uint64_t* str_full = bars + 1;    // [2]
-  uint64_t* mma1 = bars + 3;
-  uint64_t* mma2 = bars + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
+// MODE 0: dK/dV pass (resident = 128-row K, V tile; streamed = 64-row Q, dO tiles of every query head of the group).
+// MODE 1: dQ pass (resident = 128-row Q, dO tile; streamed = 64-row K, V tiles).
+// One persistent CTA per SM, 3 warpgroups: warp 0 is the TMA producer (resident tiles per item, streamed tiles in a
+// BW_STAGES ring); warpgroups 1-2 own 64 rows each of the resident tile and run, per streamed tile,
+//   MODE 0:  S^T = K Q^T, dP^T = V dO^T (wgmma, both operands in shared memory),
+//            P^T = exp2(S^T * scale_log2 - lse2[q]), dS^T = P^T * (dP^T - delta[q]) * scale,
+//            dV += P^T dO, dK += dS^T Q (wgmma with P^T / dS^T from registers, dO / Q as MN-major operands)
+//   MODE 1:  S = Q K^T, dP = dO V^T, dS = P * (dP - delta[i]) * scale, dQ += dS K
+// with the accumulators in registers; the epilogue stages the bf16 result in the warpgroup's half of the resident
+// tile and stores it with TMA.
+constexpr int BW_THREADS = 384;
+constexpr int BW_STAGES = 3;
 
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  const uint32_t lane_base = uint32_t(warp * 32) << 16;
+template <int D>
+struct BwdCfg {
+  static constexpr int RES_TILE = 128 * D * 2;   // resident 128-row tile (64-column boxes of 16 KB)
+  static constexpr int STR_TILE = 64 * D * 2;    // streamed 64-row tile (64-column boxes of 8 KB)
+  // + barriers (128 B) + per-warpgroup column statistics of pass A (2 x 2 x 128 floats) + align slack
+  static constexpr int SMEM = 2 * RES_TILE + 2 * BW_STAGES * STR_TILE + 128 + 2048 + 1024;
+};
 
-  if (tid == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    tma_prefetch_desc(&tmdO);
-    mbar_init(res_full, 1);
-    mbar_init(&str_full[0], 1);
-    mbar_init(&str_full[1], 1);
-    mbar_init(mma1, 1);
-    mbar_init(mma2, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tA = tmem_base;             // S^T / S     (P^T packed over its first 64 columns)
-  const uint32_t tB = tmem_base + 128;       // dP^T / dP   (dS^T / dS packed over its first 64 columns)
-  const uint32_t tAcc0 = tmem_base + 256;    // dV  | dQ
-  const uint32_t tAcc1 = tmem_base + 256 + D;  // dK
-
-  constexpr uint32_t idesc_ss = make_idesc_bf16(128, 128, 0, 0);
-  constexpr uint32_t idesc_ts = make_idesc_bf16(128, D, 0, 1);
-  const int G = p.hq / p.hkv;
-
-  uint32_t n_res = 0, n_str[2] = {0, 0}, n_mma1 = 0, n_mma2 = 0;   // completed phases per barrier
-
-  for (int item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-    // ---- decode ----
-    int b, kvh, h_fixed = 0, rt;     // rt: resident tile index (kv tile for MODE 0, q tile for MODE 1)
-    if (MODE == 0) {
-      rt = item % p.n_kt;
-      kvh = (item / p.n_kt) % p.hkv;
-      b = item / (p.n_kt * p.hkv);
-    } else {
-      const int r = item % p.n_qt;
-      rt = p.causal ? (p.n_qt - 1 - r) : r;
-      h_fixed = (item / p.n_qt) % p.hq;
-      kvh = h_fixed / G;
-      b = item / (p.n_qt * p.hq);
-    }
-    // streamed iteration space: MODE 0: (g, qt) pairs; MODE 1: kt
-    const int n_inner = (MODE == 0) ? G * p.n_qt : p.n_kt;
-    auto visible = [&](int it) -> bool {
-      if (MODE == 0) return pair_visible(p, it % p.n_qt, rt);
-      return pair_visible(p, rt, it);
-    };
-    auto next_visible = [&](int it) -> int {
-      while (it < n_inner && !visible(it)) ++it;
-      return it;
-    };
-    auto load_streamed = [&](int it, int stage) {   // thread 0 only
-      mbar_arrive_expect_tx(&str_full[stage], 2 * TILE);
-      if (MODE == 0) {
-        const int qt = it % p.n_qt, h = kvh * G + it / p.n_qt;
-        for (int bx = 0; bx < BOXES; ++bx) {
-          tma_load_4d(sS0 + stage * TILE + bx * 16384, &tmQ, &str_full[stage], bx * 64, qt * 128, h, b, kEvictNormal);
-          tma_load_4d(sS1 + stage * TILE + bx * 16384, &tmdO, &str_full[stage], bx * 64, qt * 128, h, b, kEvictNormal);
-        }
-      } else {
-        for (int bx = 0; bx < BOXES; ++bx) {
-          tma_load_4d(sS0 + stage * TILE + bx * 16384, &tmK, &str_full[stage], bx * 64, it * 128, kvh, b, kEvictLast);
-          tma_load_4d(sS1 + stage * TILE + bx * 16384, &tmV, &str_full[stage], bx * 64, it * 128, kvh, b, kEvictLast);
-        }
-      }
-    };
-    auto load_col_stats = [&](int it, int stage) {   // MODE 0: every thread loads one q column's lse2 / delta
-      const int qt = it % p.n_qt, h = kvh * G + it / p.n_qt;
-      const int qi = qt * 128 + tid;
-      float l2 = INFINITY, dl = 0.f;
-      if (qi < p.sq) {
-        const long long o = ((long long)b * p.hq + h) * p.sq + qi;
-        l2 = p.lse[o] * 1.4426950408889634f;
-        dl = p.delta[o];
-      }
-      s_lse[stage * 128 + tid] = l2;
-      s_dlt[stage * 128 + tid] = dl;
-    };
-
-    // ---- resident tiles ----
-    if (tid == 0) {
-      mbar_arrive_expect_tx(res_full, 2 * TILE);
-      for (int bx = 0; bx < BOXES; ++bx) {
-        if (MODE == 0) {
-          tma_load_4d(sR0 + bx * 16384, &tmK, res_full, bx * 64, rt * 128, kvh, b, kEvictFirst);
-          tma_load_4d(sR1 + bx * 16384, &tmV, res_full, bx * 64, rt * 128, kvh, b, kEvictFirst);
-        } else {
-          tma_load_4d(sR0 + bx * 16384, &tmQ, res_full, bx * 64, rt * 128, h_fixed, b, kEvictFirst);
-          tma_load_4d(sR1 + bx * 16384, &tmdO, res_full, bx * 64, rt * 128, h_fixed, b, kEvictFirst);
-        }
-      }
-    }
-    // row statistics for MODE 1 (thread = query row)
-    float row_lse2 = INFINITY, row_delta = 0.f;
-    long long row_pos = 0;      // global position of this thread's row (kv row in MODE 0, q row in MODE 1)
-    if (MODE == 1) {
-      const int qi = rt * 128 + tid;
-      if (qi < p.sq) {
-        const long long o = ((long long)b * p.hq + h_fixed) * p.sq + qi;
-        row_lse2 = p.lse[o] * 1.4426950408889634f;
-        row_delta = p.delta[o];
-      }
-      row_pos = q_tile_pos(p, rt) + tid;
-    } else {
-      row_pos = p.kv_pos0 + (long long)rt * 128 + tid;
-    }
-
-    int it = next_visible(0);
-    int stage = 0;
-    bool first = true;
-    if (it < n_inner) {
-      if (tid == 0) load_streamed(it, 0);
-      if (MODE == 0) load_col_stats(it, 0);
-    }
-    mbar_wait(res_full, n_res & 1);
-    ++n_res;
-
-    while (it < n_inner) {
-      const int nxt = next_visible(it + 1);
-      // prefetch the next streamed tile into the other stage (its last readers were MMA2 of the
-      // previous iteration, which thread 0 has waited for below)
-      if (nxt < n_inner) {
-        if (tid == 0) load_streamed(nxt, stage ^ 1);
-        if (MODE == 0) load_col_stats(nxt, stage ^ 1);
-      }
-      mbar_wait(&str_full[stage], n_str[stage] & 1);
-      ++n_str[stage];
-      __syncthreads();   // column statistics of this stage are visible to every thread
-      // ---- MMA phase 1: the two SS GEMMs (warp 0, warp-uniform; one elected lane issues) ----
-      if (warp == 0) {
-        tc_fence_after();
-        const uint64_t r0 = make_smem_desc(smem_u32(sR0), 16, 1024), r1 = make_smem_desc(smem_u32(sR1), 16, 1024);
-        const uint64_t s0 = make_smem_desc(smem_u32(sS0 + stage * TILE), 16, 1024);
-        const uint64_t s1 = make_smem_desc(smem_u32(sS1 + stage * TILE), 16, 1024);
-        if (elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = ((kk / 4) * 16384 + (kk % 4) * 32) >> 4;
-            umma_ss(tA, r0 + off, s0 + off, idesc_ss, kk != 0);
-          }
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = ((kk / 4) * 16384 + (kk % 4) * 32) >> 4;
-            umma_ss(tB, r1 + off, s1 + off, idesc_ss, kk != 0);
-          }
-          umma_commit(mma1);
-        }
-        __syncwarp();
-      }
-      mbar_wait(mma1, n_mma1 & 1);
-      ++n_mma1;
-      tc_fence_after();
-
-      // ---- element-wise phase: P and dS, packed to bf16 over the fp32 tiles ----
-      long long col_pos0;      // global position of column 0 of the streamed tile
-      int col_valid;           // columns of the streamed tile that exist
-      if (MODE == 0) {
-        const int qt = it % p.n_qt;
-        col_pos0 = q_tile_pos(p, qt);
-        col_valid = p.sq - qt * 128;
-      } else {
-        col_pos0 = p.kv_pos0 + (long long)it * 128;
-        col_valid = p.sk - it * 128;
-      }
-      const bool need_mask = p.causal && (MODE == 0 ? (row_pos - tid + 127 > col_pos0) : (col_pos0 + 127 > row_pos - tid));
-#pragma unroll 1
-      for (int c4 = 0; c4 < 4; ++c4) {
-        uint32_t sv[32], dv[32];
-        tmem_ld32(tA + lane_base + c4 * 32, sv);
-        tmem_ld32(tB + lane_base + c4 * 32, dv);
-        tmem_wait_ld();
-        uint32_t pp[16], ds[16];
-#pragma unroll
-        for (int k = 0; k < 32; k += 2) {
-          float pv[2], dsv[2];
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = c4 * 32 + k + e;
-            const float l2 = (MODE == 0) ? s_lse[stage * 128 + c] : row_lse2;
-            const float dl = (MODE == 0) ? s_dlt[stage * 128 + c] : row_delta;
-            float pe = ex2(fmaf(__uint_as_float(sv[k + e]), p.scale_log2, -l2));
-            bool keep = c < col_valid;
-            if (need_mask) keep = keep && (MODE == 0 ? (row_pos <= col_pos0 + c) : (col_pos0 + c <= row_pos));
-            pe = keep ? pe : 0.f;
-            pv[e] = pe;
-            dsv[e] = pe * (__uint_as_float(dv[k + e]) - dl) * p.scale;
-          }
-          pp[k / 2] = pack_bf16(pv[0], pv[1]);
-          ds[k / 2] = pack_bf16(dsv[0], dsv[1]);
-        }
-        if (MODE == 0) tmem_st16(tA + lane_base + c4 * 16, pp);
-        tmem_st16(tB + lane_base + c4 * 16, ds);
-      }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncthreads();
-
-      // ---- MMA phase 2: TS GEMMs into the accumulators (warp 0, one elected lane issues) ----
-      if (warp == 0) {
-        tc_fence_after();
-        const uint64_t s0 = make_smem_desc(smem_u32(sS0 + stage * TILE), 16384, 1024);
-        const uint64_t s1 = make_smem_desc(smem_u32(sS1 + stage * TILE), 16384, 1024);
-        const uint32_t acc = first ? 0u : 1u;
-        if (elect_one()) {
-          if (MODE == 0) {
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk)   // dV += P^T dO
-              umma_ts(tAcc0, tA + kk * 8, s1 + (uint64_t)(kk * 128), idesc_ts, (acc | (kk != 0)) ? 1u : 0u);
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk)   // dK += dS^T Q
-              umma_ts(tAcc1, tB + kk * 8, s0 + (uint64_t)(kk * 128), idesc_ts, (acc | (kk != 0)) ? 1u : 0u);
-          } else {
-#pragma unroll
-            for (int kk = 0; kk < 8; ++kk)   // dQ += dS K
-              umma_ts(tAcc0, tB + kk * 8, s0 + (uint64_t)(kk * 128), idesc_ts, (acc | (kk != 0)) ? 1u : 0u);
-          }
-          umma_commit(mma2);
-        }
-        __syncwarp();
-        // the streamed stage (and, for the next item, the resident tiles) may be overwritten only
-        // after these MMAs have read them
-        mbar_wait(mma2, n_mma2 & 1);
-      }
-      ++n_mma2;
-      first = false;
-      it = nxt;
-      stage ^= 1;
-    }
-
-    // ---- epilogue: accumulators -> bf16 -> swizzled staging -> TMA store ----
-    __syncthreads();      // thread 0 has seen the last MMA2 retire
-    tc_fence_after();
-    constexpr int NACC = (MODE == 0) ? 2 : 1;
-#pragma unroll 1
-    for (int a = 0; a < NACC; ++a) {
-      uint8_t* stg = (a == 0 ? sS0 : sS1);     // stage 0 of a streamed buffer; no load is in flight
-      const uint32_t tacc = (a == 0 ? tAcc0 : tAcc1) + lane_base;
-#pragma unroll 1
-      for (int c = 0; c < D / 32; ++c) {
-        uint32_t o[32];
-        if (!first) {
-          tmem_ld32(tacc + c * 32, o);
-          tmem_wait_ld();
-        } else {
-#pragma unroll
-          for (int k = 0; k < 32; ++k) o[k] = 0u;
-        }
-        uint8_t* box = stg + (c >> 1) * 16384 + tid * 128;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 v;
-          v.x = pack_bf16(__uint_as_float(o[8 * q + 0]), __uint_as_float(o[8 * q + 1]));
-          v.y = pack_bf16(__uint_as_float(o[8 * q + 2]), __uint_as_float(o[8 * q + 3]));
-          v.z = pack_bf16(__uint_as_float(o[8 * q + 4]), __uint_as_float(o[8 * q + 5]));
-          v.w = pack_bf16(__uint_as_float(o[8 * q + 6]), __uint_as_float(o[8 * q + 7]));
-          const int chunk = (c & 1) * 4 + q;
-          *reinterpret_cast<uint4*>(box + ((chunk ^ (tid & 7)) << 4)) = v;
-        }
-      }
-    }
-    tc_fence_before();
-    fence_proxy_async_smem();
-    __syncthreads();
-    if (tid == 0) {
-      for (int bx = 0; bx < BOXES; ++bx) {
-        if (MODE == 0) {
-          tma_store_4d(&tmOut0, sS0 + bx * 16384, bx * 64, rt * 128, kvh, b);   // dV
-          tma_store_4d(&tmOut1, sS1 + bx * 16384, bx * 64, rt * 128, kvh, b);   // dK
-        } else {
-          tma_store_4d(&tmOut0, sS0 + bx * 16384, bx * 64, rt * 128, h_fixed, b);   // dQ
-        }
-      }
-      tma_store_commit();
-      tma_store_wait_read0();
-    }
-    __syncthreads();
-  }
-  if (tid == 0) tma_store_wait_all0();
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tmem_base, 512);
+__device__ __forceinline__ long long q_row_pos(const BwdKParams& p, int row0) {
+  const int seg = row0 / p.q_seg_len;
+  return (seg == 0 ? p.q_seg_pos0 : p.q_seg_pos1) + (row0 - seg * p.q_seg_len);
 }
 
-// ================================================================================================
-// Version 2 of the backward kernel (LV_BWD_VERSION=2): the same two passes, warp-specialised and pipelined like
-// the forward v2 kernel.  Version 1 runs TMA wait -> MMA1 -> element-wise -> MMA2 strictly one after the other on
-// one warpgroup, so the tensor pipe idles through the whole element-wise phase (and vice versa).  Here
-//   warp 0      TMA producer (resident tiles per item, 128-row streamed tiles in a 2-stage ring, column statistics)
-//   warp 1      tcgen05 issuer
-//   warps 4-7   element-wise warpgroup 0 \  each streamed 128-row tile is consumed as two 64-row halves;
-//   warps 8-11  element-wise warpgroup 1 /  warpgroup b owns half b and the TMEM buffer pair b
-// TMEM: [S^T_0 | dP^T_0 | S^T_1 | dP^T_1] = 4 x 64 fp32 columns, accumulators at column 256 (D) and 256 + D (D).
-// The issuer queues MMA1 of half j+1 before it waits for the probabilities of half j, so S(j+1) is computed while
-// warpgroup j&1 is still in its exponentials, and MMA2(j) runs while warpgroup (j+1)&1 works.  Buffer reuse needs
-// no extra barrier: MMA1(j+2) is issued after MMA2(j) by the same thread, and tcgen05 operations of one thread
-// execute in order.  Arithmetic (masking, bf16 packing, MMA shapes of the TS products) is that of version 1.
-// ================================================================================================
-constexpr int B2_THREADS = 384;
+// MODE 0: does the 64-row query tile qt see any key of [key0, key0 + nkeys)?  (64-row tiles never straddle segments)
+__device__ __forceinline__ bool q_sees(const BwdKParams& p, int qt, long long key0) {
+  return !p.causal || p.kv_pos0 + key0 <= q_row_pos(p, qt * 64) + 63;
+}
+
+// X[64 x 64] = A[64 rows of a resident tile] . B[64-row streamed tile]^T over the head dimension
+template <int D>
+__device__ __forceinline__ void mma_rows(float (&x)[32], uint64_t adesc, uint64_t bdesc) {
+#pragma unroll
+  for (int kk = 0; kk < D / 16; ++kk)
+    wgmma_ss_n64(x, adesc + (((kk / 4) * 16384 + (kk % 4) * 32) >> 4), bdesc + (((kk / 4) * 8192 + (kk % 4) * 32) >> 4),
+                 kk != 0 ? 1u : 0u);
+}
+
+// acc[64 x D] += X[64 x 64] (bf16 pairs in the accumulator layout) . B[64-row streamed tile] (MN-major)
+template <int D>
+__device__ __forceinline__ void mma_acc(float (&acc)[D / 2], const uint32_t (&xk)[16], uint64_t bdesc) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const uint32_t a[4] = {xk[4 * kk], xk[4 * kk + 1], xk[4 * kk + 2], xk[4 * kk + 3]};
+    if constexpr (D == 128)
+      wgmma_rs_n128(acc, a, bdesc + (uint64_t)(kk * 128), 1u);
+    else
+      wgmma_rs_n64(acc, a, bdesc + (uint64_t)(kk * 128), 1u);
+  }
+}
+
+// Stage a 64 x D fp32 accumulator as bf16 into 64 rows of a 128-row resident tile (128-byte swizzle).
+template <int D>
+__device__ __forceinline__ void stage_rows(uint8_t* half, const float (&acc)[D / 2], int r_lo, int cq) {
+#pragma unroll
+  for (int jj = 0; jj < D / 8; ++jj) {
+    uint8_t* box = half + (jj >> 3) * 16384;
+    const int ch = jj & 7;
+    const int r1 = r_lo + 8;
+    *reinterpret_cast<uint32_t*>(box + r_lo * 128 + ((ch ^ (r_lo & 7)) << 4) + cq * 2) = pack_bf16(acc[4 * jj], acc[4 * jj + 1]);
+    *reinterpret_cast<uint32_t*>(box + r1 * 128 + ((ch ^ (r1 & 7)) << 4) + cq * 2) = pack_bf16(acc[4 * jj + 2], acc[4 * jj + 3]);
+  }
+}
+
+// Resident tile of a work item.  Causal dQ items run longest-first (the last query tiles see the most keys), which
+// balances the static round-robin over the CTAs.
+template <int MODE>
+__device__ __forceinline__ int item_tile(const BwdKParams& p, int item) {
+  const int n = MODE == 0 ? p.n_kt : p.n_qt;
+  const int r = item % n;
+  return (MODE == 1 && p.causal) ? n - 1 - r : r;
+}
 
 template <int D, int MODE>
-__global__ void __launch_bounds__(B2_THREADS, 1)
-    attn_bwd2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
-                     const __grid_constant__ CUtensorMap tmOut0, const __grid_constant__ CUtensorMap tmOut1,
-                     const BwdKParams p) {
-  constexpr int TILE = 128 * D * 2;
+__global__ void __launch_bounds__(BW_THREADS, 1)
+    attn_bwd_kernel(const __grid_constant__ CUtensorMap tmR0, const __grid_constant__ CUtensorMap tmR1,
+                    const __grid_constant__ CUtensorMap tmS0, const __grid_constant__ CUtensorMap tmS1,
+                    const __grid_constant__ CUtensorMap tmOut0, const __grid_constant__ CUtensorMap tmOut1,
+                    const BwdKParams p) {
+  using Cfg = BwdCfg<D>;
+  constexpr int NS = BW_STAGES;
   constexpr int BOXES = D / 64;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sR0 = smem;                 // resident operand 0 (K or Q); staging of accumulator 0 in the epilogue
-  uint8_t* sR1 = sR0 + TILE;           // resident operand 1 (V or dO); staging of accumulator 1
-  uint8_t* sS0 = sR1 + TILE;           // streamed operand 0, 2 stages (Q or K)
-  uint8_t* sS1 = sS0 + 2 * TILE;       // streamed operand 1, 2 stages (dO or V)
-  float* s_lse = reinterpret_cast<float*>(sS1 + 2 * TILE);   // [2][128]  (MODE 0 only)
-  float* s_dlt = s_lse + 256;                               // [2][128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_dlt + 256);
-  uint64_t* res_full = bars;          // resident tiles landed                 (tx, 1 arrival)
-  uint64_t* res_empty = bars + 1;     // both warpgroups' TMA stores have read the staging tiles (2 arrivals)
-  uint64_t* str_full = bars + 2;      // [2] streamed stage landed              (tx, 1 arrival)
-  uint64_t* str_empty = bars + 4;     // [2] both halves' MMA2 have read it     (tcgen05.commit)
-  uint64_t* s_full = bars + 6;        // [2] MMA1 of a half done                (tcgen05.commit)
-  uint64_t* p_full = bars + 8;        // [2] P^T / dS^T of a half written       (128 arrivals)
-  uint64_t* acc_full = bars + 10;     // all MMA2 of the item done              (tcgen05.commit / plain arrive)
-  uint64_t* acc_empty = bars + 11;    // accumulators read by the epilogue      (256 arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
+  uint8_t* sR0 = smem;                        // resident operand 0 (K or Q); later the staging tile of output 1
+  uint8_t* sR1 = sR0 + Cfg::RES_TILE;         // resident operand 1 (V or dO); later the staging tile of output 0
+  uint8_t* sS0 = sR1 + Cfg::RES_TILE;         // streamed operand 0 (Q or K), NS stages
+  uint8_t* sS1 = sS0 + NS * Cfg::STR_TILE;    // streamed operand 1 (dO or V), NS stages
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sS1 + NS * Cfg::STR_TILE);
+  uint64_t* res_full = bars;
+  uint64_t* res_empty = bars + 1;             // both warpgroups have stored their outputs out of the resident tiles
+  uint64_t* str_full = bars + 2;              // [NS]
+  uint64_t* str_empty = bars + 2 + NS;        // [NS]
+  float* s_stat = reinterpret_cast<float*>(bars + 16);   // MODE 0: [warpgroup][2 buffers][lse2 x 64 | delta x 64]
 
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5;
-  const int lane = tid & 31;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int G = p.hq / p.hkv;
+  const int n_q64 = (p.sq + 63) / 64;
+  const int n_k64 = (p.sk + 63) / 64;
 
-  if (tid == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    tma_prefetch_desc(&tmdO);
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmR0);
+    tma_prefetch_desc(&tmR1);
+    tma_prefetch_desc(&tmS0);
+    tma_prefetch_desc(&tmS1);
     mbar_init(res_full, 1);
     mbar_init(res_empty, 2);
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < NS; ++i) {
       mbar_init(&str_full[i], 1);
-      mbar_init(&str_empty[i], 1);
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 128);
+      mbar_init(&str_empty[i], 2);
     }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 256);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tAcc0 = tmem_base + 256;        // dV | dQ
-  const uint32_t tAcc1 = tmem_base + 256 + D;    // dK
-  const int G = p.hq / p.hkv;
 
-  // ---- the item / streamed-tile enumeration every role walks identically ----
-  struct Item {
-    int b, kvh, h_fixed, rt;
-  };
-  auto decode = [&](int item) {
-    Item w;
-    w.h_fixed = 0;
-    if (MODE == 0) {
-      w.rt = item % p.n_kt;
-      w.kvh = (item / p.n_kt) % p.hkv;
-      w.b = item / (p.n_kt * p.hkv);
-    } else {
-      const int r = item % p.n_qt;
-      w.rt = p.causal ? (p.n_qt - 1 - r) : r;
-      w.h_fixed = (item / p.n_qt) % p.hq;
-      w.kvh = w.h_fixed / G;
-      w.b = item / (p.n_qt * p.hq);
-    }
-    return w;
-  };
-  const int n_inner = (MODE == 0) ? G * p.n_qt : p.n_kt;
-  auto visible = [&](const Item& w, int it) -> bool {
-    if (MODE == 0) return pair_visible(p, it % p.n_qt, w.rt);
-    return pair_visible(p, w.rt, it);
-  };
-  auto next_visible = [&](const Item& w, int it) -> int {
-    while (it < n_inner && !visible(w, it)) ++it;
-    return it;
+  // Item decoding shared by all roles.  MODE 0: (b, kv head, 128-key tile); MODE 1: (b, head, 128-row query tile).
+  // Streamed step list: MODE 0 - every (head of the group, 64-row query tile) that sees the key tile; MODE 1 - the
+  // 64-key tiles [0, n) the query tile sees.
+  auto n_k_steps = [&](int t) -> int {   // MODE 1: 64-key tiles visible to 128-row query tile t
+    if (!p.causal) return n_k64;
+    const long long hi = q_row_pos(p, t * 128) + 127 - p.kv_pos0;
+    if (hi < 0) return 0;
+    return (int)min((long long)n_k64, hi / 64 + 1);
   };
 
-  if (warp == 0) {
-    // =========================== TMA producer ===========================
-    uint32_t item_cnt = 0, n_stream = 0;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++item_cnt) {
-      const Item w = decode(item);
-      mbar_wait(res_empty, (item_cnt & 1) ^ 1);           // previous item's epilogue has left the staging tiles
-      if (elect_one()) {
-        mbar_arrive_expect_tx(res_full, 2 * TILE);
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      // =========================== TMA producer ===========================
+      uint32_t item_cnt = 0, scnt = 0;
+      auto load_str = [&](int row64, int head, int b) {
+        const int st = scnt % NS;
+        mbar_wait(&str_empty[st], ((scnt / NS) & 1) ^ 1);
+        mbar_arrive_expect_tx(&str_full[st], 2 * Cfg::STR_TILE);
         for (int bx = 0; bx < BOXES; ++bx) {
-          if (MODE == 0) {
-            tma_load_4d(sR0 + bx * 16384, &tmK, res_full, bx * 64, w.rt * 128, w.kvh, w.b, kEvictFirst);
-            tma_load_4d(sR1 + bx * 16384, &tmV, res_full, bx * 64, w.rt * 128, w.kvh, w.b, kEvictFirst);
-          } else {
-            tma_load_4d(sR0 + bx * 16384, &tmQ, res_full, bx * 64, w.rt * 128, w.h_fixed, w.b, kEvictFirst);
-            tma_load_4d(sR1 + bx * 16384, &tmdO, res_full, bx * 64, w.rt * 128, w.h_fixed, w.b, kEvictFirst);
-          }
+          tma_load_4d(sS0 + st * Cfg::STR_TILE + bx * 8192, &tmS0, &str_full[st], bx * 64, row64 * 64, head, b, kEvictLast);
+          tma_load_4d(sS1 + st * Cfg::STR_TILE + bx * 8192, &tmS1, &str_full[st], bx * 64, row64 * 64, head, b, kEvictLast);
         }
-      }
-      __syncwarp();
-      for (int it = next_visible(w, 0); it < n_inner; it = next_visible(w, it + 1), ++n_stream) {
-        const int st = n_stream & 1;
-        mbar_wait(&str_empty[st], ((n_stream >> 1) & 1) ^ 1);
-        if (MODE == 0) {
-          // column statistics of the 128 query rows of this tile (visible to the warpgroups through str_full)
-          const int qt = it % p.n_qt, h = w.kvh * G + it / p.n_qt;
-          for (int c = lane; c < 128; c += 32) {
-            const int qi = qt * 128 + c;
-            float l2 = INFINITY, dl = 0.f;
-            if (qi < p.sq) {
-              const long long o = ((long long)w.b * p.hq + h) * p.sq + qi;
-              l2 = p.lse[o] * 1.4426950408889634f;
-              dl = p.delta[o];
-            }
-            s_lse[st * 128 + c] = -l2;      // stored NEGATED: the consumers add them inside packed FFMA2 / FADD2
-            s_dlt[st * 128 + c] = -dl;
-          }
-          __syncwarp();
-        }
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&str_full[st], 2 * TILE);
-          if (MODE == 0) {
-            const int qt = it % p.n_qt, h = w.kvh * G + it / p.n_qt;
-            for (int bx = 0; bx < BOXES; ++bx) {
-              tma_load_4d(sS0 + st * TILE + bx * 16384, &tmQ, &str_full[st], bx * 64, qt * 128, h, w.b, kEvictNormal);
-              tma_load_4d(sS1 + st * TILE + bx * 16384, &tmdO, &str_full[st], bx * 64, qt * 128, h, w.b, kEvictNormal);
-            }
-          } else {
-            for (int bx = 0; bx < BOXES; ++bx) {
-              tma_load_4d(sS0 + st * TILE + bx * 16384, &tmK, &str_full[st], bx * 64, it * 128, w.kvh, w.b, kEvictLast);
-              tma_load_4d(sS1 + st * TILE + bx * 16384, &tmV, &str_full[st], bx * 64, it * 128, w.kvh, w.b, kEvictLast);
-            }
-          }
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    constexpr uint32_t idesc_ss = make_idesc_bf16(128, 64, 0, 0);
-    constexpr uint32_t idesc_ts = make_idesc_bf16(128, D, 0, 1);
-    const uint64_t r0 = make_smem_desc(smem_u32(sR0), 16, 1024), r1 = make_smem_desc(smem_u32(sR1), 16, 1024);
-    uint32_t item_cnt = 0, n_stream = 0;
-    uint32_t pcnt[2] = {0, 0};
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++item_cnt) {
-      const Item w = decode(item);
-      int nvis = 0;
-      for (int it = next_visible(w, 0); it < n_inner; it = next_visible(w, it + 1)) ++nvis;
-      const int J = 2 * nvis;                               // 64-row halves
-      mbar_wait(res_full, item_cnt & 1);
-      tc_fence_after();
-      auto stage_of = [&](int j) { return (int)((n_stream + (uint32_t)(j >> 1)) & 1); };
-      auto issue_mma1 = [&](int j) {
-        const int st = stage_of(j), h = j & 1;
-        if (h == 0) {
-          const uint32_t n = n_stream + (uint32_t)(j >> 1);
-          mbar_wait(&str_full[st], (n >> 1) & 1);
-          tc_fence_after();
-        }
-        const uint64_t s0 = make_smem_desc(smem_u32(sS0 + st * TILE) + h * 8192, 16, 1024);
-        const uint64_t s1 = make_smem_desc(smem_u32(sS1 + st * TILE) + h * 8192, 16, 1024);
-        const uint32_t tA = tmem_base + h * 128, tB = tmem_base + h * 128 + 64;
-        if (elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = ((kk / 4) * 16384 + (kk % 4) * 32) >> 4;
-            umma_ss(tA, r0 + off, s0 + off, idesc_ss, kk != 0);
-          }
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = ((kk / 4) * 16384 + (kk % 4) * 32) >> 4;
-            umma_ss(tB, r1 + off, s1 + off, idesc_ss, kk != 0);
-          }
-          umma_commit(&s_full[h]);
-        }
-        __syncwarp();
-      };
-      if (J == 0) {
-        if (elect_one()) mbar_arrive(acc_full);             // nothing to accumulate: the epilogue writes zeros
-        __syncwarp();
-        continue;
-      }
-      issue_mma1(0);
-      for (int j = 0; j < J; ++j) {
-        if (j + 1 < J) issue_mma1(j + 1);
-        const int st = stage_of(j), h = j & 1;
-        mbar_wait(&p_full[h], pcnt[h] & 1);
-        ++pcnt[h];
-        if (j == 0) mbar_wait(acc_empty, (item_cnt & 1) ^ 1);   // previous item's accumulators have been read
-        tc_fence_after();
-        const uint64_t s0 = make_smem_desc(smem_u32(sS0 + st * TILE) + h * 8192, 16384, 1024);
-        const uint64_t s1 = make_smem_desc(smem_u32(sS1 + st * TILE) + h * 8192, 16384, 1024);
-        const uint32_t tA = tmem_base + h * 128, tB = tmem_base + h * 128 + 64;
-        const uint32_t acc = j > 0 ? 1u : 0u;
-        if (elect_one()) {
-          if (MODE == 0) {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)   // dV += P^T dO      (K = 64 streamed rows)
-              umma_ts(tAcc0, tA + kk * 8, s1 + (uint64_t)(kk * 128), idesc_ts, (acc | (kk != 0)) ? 1u : 0u);
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)   // dK += dS^T Q
-              umma_ts(tAcc1, tB + kk * 8, s0 + (uint64_t)(kk * 128), idesc_ts, (acc | (kk != 0)) ? 1u : 0u);
-          } else {
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk)   // dQ += dS K
-              umma_ts(tAcc0, tB + kk * 8, s0 + (uint64_t)(kk * 128), idesc_ts, (acc | (kk != 0)) ? 1u : 0u);
-          }
-          if (h == 1) umma_commit(&str_empty[st]);          // both halves of this stage have been consumed
-          if (j == J - 1) umma_commit(acc_full);
-        }
-        __syncwarp();
-      }
-      n_stream += (uint32_t)nvis;
-    }
-  } else if (warp >= 4) {
-    // =========================== element-wise warpgroups + epilogue ===========================
-    const int b = (warp - 4) >> 2;                     // warpgroup = half index = TMEM buffer pair
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;                  // resident-tile row of this thread = TMEM lane
-    const uint32_t lane_base = uint32_t(quad * 32) << 16;
-    const uint32_t tA = tmem_base + lane_base + b * 128;
-    const uint32_t tB = tmem_base + lane_base + b * 128 + 64;
-    uint32_t item_cnt = 0, n_stream = 0, scnt = 0;
-    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++item_cnt) {
-      const Item w = decode(item);
-      float row_lse2 = INFINITY, row_delta = 0.f;
-      long long row_pos;
-      if (MODE == 1) {
-        const int qi = w.rt * 128 + row;
-        if (qi < p.sq) {
-          const long long o = ((long long)w.b * p.hq + w.h_fixed) * p.sq + qi;
-          row_lse2 = p.lse[o] * 1.4426950408889634f;
-          row_delta = p.delta[o];
-        }
-        row_pos = q_tile_pos(p, w.rt) + row;
-      } else {
-        row_pos = p.kv_pos0 + (long long)w.rt * 128 + row;
-      }
-      int nvis = 0;
-      for (int it = next_visible(w, 0); it < n_inner; it = next_visible(w, it + 1), ++nvis) {
-        const uint32_t n = n_stream + (uint32_t)nvis;
-        const int st = (int)(n & 1);
-        mbar_wait(&str_full[st], (n >> 1) & 1);        // acquires the column statistics the producer wrote
-        mbar_wait(&s_full[b], scnt & 1);
         ++scnt;
-        tc_fence_after();
-        long long col_pos0;
-        int col_valid;
+      };
+      for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++item_cnt) {
+        const int t = item_tile<MODE>(p, item);
+        const int bh = item / (MODE == 0 ? p.n_kt : p.n_qt);   // b * heads + head
+        const int heads = MODE == 0 ? p.hkv : p.hq;
+        const int b = bh / heads, head = bh % heads;
+        mbar_wait(res_empty, (item_cnt & 1) ^ 1);
+        mbar_arrive_expect_tx(res_full, 2 * Cfg::RES_TILE);
+        for (int bx = 0; bx < BOXES; ++bx) {
+          tma_load_4d(sR0 + bx * 16384, &tmR0, res_full, bx * 64, t * 128, head, b, kEvictFirst);
+          tma_load_4d(sR1 + bx * 16384, &tmR1, res_full, bx * 64, t * 128, head, b, kEvictFirst);
+        }
         if (MODE == 0) {
-          const int qt = it % p.n_qt;
-          col_pos0 = q_tile_pos(p, qt) + b * 64;
-          col_valid = p.sq - qt * 128 - b * 64;
+          for (int g = 0; g < G; ++g)
+            for (int qt = 0; qt < n_q64; ++qt)
+              if (q_sees(p, qt, (long long)t * 128)) load_str(qt, head * G + g, b);
         } else {
-          col_pos0 = p.kv_pos0 + (long long)it * 128 + b * 64;
-          col_valid = p.sk - it * 128 - b * 64;
+          const int n = n_k_steps(t);
+          for (int kt = 0; kt < n; ++kt) load_str(kt, head / G, b);
         }
-        const long long row0_pos = row_pos - row;
-        const bool need_mask = p.causal && (MODE == 0 ? (row0_pos + 127 > col_pos0) : (col_pos0 + 63 > row0_pos));
-        // Columns this thread keeps: [c_lo, c_hi) of the 64 of this half.  Interior tiles (no causal boundary, no
-        // ragged edge) keep everything and take the branch-free path below - the round-2 ncu source view showed a
-        // third of the element-wise samples on per-element 64-bit compares and selects that only diagonal tiles need.
-        int c_lo = 0, c_hi = col_valid < 64 ? (col_valid < 0 ? 0 : col_valid) : 64;
-        if (need_mask) {
-          const long long dlt = row_pos - col_pos0;                      // MODE 0: keep c >= dlt; MODE 1: keep c <= dlt
+      }
+    }
+  } else {
+    // =========================== consumer warpgroups ===========================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int c = (warp >> 2) - 1;                         // 64-row half of the resident tile
+    const int wg_tid = threadIdx.x & 127;
+    const int r_lo = ((wg_tid >> 5) << 4) + (lane >> 2);   // this thread's rows: r_lo and r_lo + 8 (of 64)
+    const int cq = 2 * (lane & 3);                         // its first column in every 8-column group
+    const uint64_t r0desc = make_smem_desc(smem_u32(sR0) + c * 8192, 16, 1024);
+    const uint64_t r1desc = make_smem_desc(smem_u32(sR1) + c * 8192, 16, 1024);
+    const uint64_t s0desc = make_smem_desc(smem_u32(sS0), 16, 1024);
+    const uint64_t s1desc = make_smem_desc(smem_u32(sS1), 16, 1024);
+    const uint64_t s0mn = make_smem_desc(smem_u32(sS0), 8192, 1024);   // streamed operand 0 as an MN-major B
+    const uint64_t s1mn = make_smem_desc(smem_u32(sS1), 8192, 1024);
+    const float scale = p.scale, scale_log2 = p.scale_log2;
+    constexpr float LOG2E = 1.4426950408889634f;
+    uint32_t item_cnt = 0, scnt = 0, act_cnt = 0;
+    for (int item = blockIdx.x; item < p.n_items; item += gridDim.x, ++item_cnt) {
+      const int t = item_tile<MODE>(p, item);
+      const int bh = item / (MODE == 0 ? p.n_kt : p.n_qt);
+      const int heads = MODE == 0 ? p.hkv : p.hq;
+      const int b = bh / heads, head = bh % heads;
+      float acc0[D / 2], acc1[D / 2];    // MODE 0: dV, dK;  MODE 1: dQ, (unused)
+#pragma unroll
+      for (int i = 0; i < D / 2; ++i) acc0[i] = acc1[i] = 0.f;
+      const int rrow0 = t * 128 + c * 64;                  // first resident row of this warpgroup
+      mbar_wait(res_full, item_cnt & 1);
+
+      // one streamed tile: rows / columns -> masking, P, dS, the two accumulating products
+      auto step = [&](int row64, int hq_idx, bool active) {
+        const int st = scnt % NS;
+        mbar_wait(&str_full[st], (scnt / NS) & 1);
+        ++scnt;
+        if (active) {
+          const uint64_t so = (uint64_t)((st * Cfg::STR_TILE) >> 4);
+          float x[32], dp[32];
+          wgmma_fence();
+          mma_rows<D>(x, r0desc, s0desc + so);      // S^T = K Q^T  |  S = Q K^T
+          mma_rows<D>(dp, r1desc, s1desc + so);     // dP^T = V dO^T  |  dP = dO V^T
+          wgmma_commit();
+          const long long stat = ((long long)b * p.hq + hq_idx) * p.sq;
+          // MODE 0: the 64 query columns' lse2 and delta, loaded once per tile by the warpgroup while the MMAs run.
+          // Two buffers alternate, so a buffer is rewritten only after every thread passed the next step's barrier.
+          const float* st_buf = s_stat + (c * 2 + (act_cnt & 1)) * 128;
           if (MODE == 0) {
-            c_lo = dlt <= 0 ? 0 : (dlt > 64 ? 64 : (int)dlt);
-          } else {
-            const int hi = dlt < 0 ? 0 : (dlt >= 64 ? 64 : (int)dlt + 1);
-            c_hi = hi < c_hi ? hi : c_hi;
+            const int qi = row64 * 64 + (wg_tid & 63);
+            float v = 0.f;
+            if (qi < p.sq) v = wg_tid < 64 ? p.lse[stat + qi] * LOG2E : p.delta[stat + qi];
+            const_cast<float*>(st_buf)[wg_tid] = v;
+            named_bar_sync(1 + c, 128);
           }
-        }
-        const bool masked_tile = need_mask || col_valid < 64;           // warp-uniform (tile-level quantities)
-        const float sc_log2 = p.scale_log2, sc = p.scale;
-#pragma unroll 1
-        for (int c2 = 0; c2 < 2; ++c2) {
-          uint32_t sv[32], dv[32];
-          tmem_ld32(tA + c2 * 32, sv);
-          tmem_ld32(tB + c2 * 32, dv);
-          tmem_wait_ld();
-          uint32_t pp[16], ds[16];
-          if (!masked_tile) {
-            // interior tile: packed fp32 pairs throughout (x = s * scale - lse, dP - delta, p * (dP - delta) * scale: the
-            // same roundings as the scalar forms), column statistics as 8-byte shared-memory loads
+          ++act_cnt;
+          wgmma_wait<0>();
+          wgmma_keep(x);
+          wgmma_keep(dp);
+          uint32_t pk[16], dsk[16];
+          if (MODE == 0) {
+            // rows = keys rrow0 + r, columns = queries row64 * 64 + col
+            const long long kpos0 = p.kv_pos0 + rrow0 + r_lo, kpos1 = kpos0 + 8;
+            const bool kv0 = rrow0 + r_lo < p.sk, kv1 = rrow0 + r_lo + 8 < p.sk;
+            const long long qp = q_row_pos(p, row64 * 64);
 #pragma unroll
-            for (int k = 0; k < 32; k += 2) {
-              const int c = c2 * 32 + k;
-              float nl0, nl1, nd0, nd1;
-              if (MODE == 0) {
-                const float2 nl = *reinterpret_cast<const float2*>(&s_lse[st * 128 + b * 64 + c]);
-                const float2 nd = *reinterpret_cast<const float2*>(&s_dlt[st * 128 + b * 64 + c]);
-                nl0 = nl.x, nl1 = nl.y, nd0 = nd.x, nd1 = nd.y;
-              } else {
-                nl0 = nl1 = -row_lse2;
-                nd0 = nd1 = -row_delta;
-              }
-              float x0, x1;
-              ffma2v(x0, x1, __uint_as_float(sv[k]), __uint_as_float(sv[k + 1]), sc_log2, sc_log2, nl0, nl1);
-              const float p0 = ex2(x0);
-              const float p1 = ex2(x1);
-              float d0, d1;
-              fadd2(d0, d1, __uint_as_float(dv[k]), __uint_as_float(dv[k + 1]), nd0, nd1);
-              fmul2(d0, d1, p0, p1, d0, d1);
-              fmul2(d0, d1, d0, d1, sc, sc);
-              pp[k / 2] = pack_bf16(p0, p1);
-              ds[k / 2] = pack_bf16(d0, d1);
-            }
-          } else {
-#pragma unroll
-            for (int k = 0; k < 32; k += 2) {
-              float pv[2], dsv[2];
+            for (int jj = 0; jj < 8; ++jj) {
+              float pr[4], ds[4];
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
-                const int c = c2 * 32 + k + e;
-                const float nl2 = (MODE == 0) ? s_lse[st * 128 + b * 64 + c] : -row_lse2;
-                const float ndl = (MODE == 0) ? s_dlt[st * 128 + b * 64 + c] : -row_delta;
-                float pe = ex2(fmaf(__uint_as_float(sv[k + e]), sc_log2, nl2));
-                pe = (c >= c_lo && c < c_hi) ? pe : 0.f;
-                pv[e] = pe;
-                dsv[e] = pe * (__uint_as_float(dv[k + e]) + ndl) * sc;
+                const int qi = row64 * 64 + 8 * jj + cq + e;
+                const bool qv = qi < p.sq;
+                const float lse2 = st_buf[8 * jj + cq + e];
+                const float dl = st_buf[64 + 8 * jj + cq + e];
+                const long long qpos = qp + 8 * jj + cq + e;
+                const bool vis0 = qv && kv0 && (!p.causal || kpos0 <= qpos);
+                const bool vis1 = qv && kv1 && (!p.causal || kpos1 <= qpos);
+                pr[e] = vis0 ? ex2(fmaf(x[4 * jj + e], scale_log2, -lse2)) : 0.f;
+                pr[2 + e] = vis1 ? ex2(fmaf(x[4 * jj + 2 + e], scale_log2, -lse2)) : 0.f;
+                ds[e] = pr[e] * (dp[4 * jj + e] - dl) * scale;
+                ds[2 + e] = pr[2 + e] * (dp[4 * jj + 2 + e] - dl) * scale;
               }
-              pp[k / 2] = pack_bf16(pv[0], pv[1]);
-              ds[k / 2] = pack_bf16(dsv[0], dsv[1]);
+              pk[2 * jj] = pack_bf16(pr[0], pr[1]);
+              pk[2 * jj + 1] = pack_bf16(pr[2], pr[3]);
+              dsk[2 * jj] = pack_bf16(ds[0], ds[1]);
+              dsk[2 * jj + 1] = pack_bf16(ds[2], ds[3]);
             }
-          }
-          if (MODE == 0) tmem_st16(tA + c2 * 16, pp);
-          tmem_st16(tB + c2 * 16, ds);
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        mbar_arrive(&p_full[b]);
-      }
-      n_stream += (uint32_t)nvis;
-
-      // ---- epilogue: accumulator -> bf16 -> swizzled staging (the resident tile) -> TMA store ----
-      mbar_wait(acc_full, item_cnt & 1);
-      tc_fence_after();
-      const bool mine = (MODE == 0) || (b == 0);       // MODE 0: warpgroup b stores accumulator b; MODE 1: warpgroup 0
-      if (mine) {
-        uint8_t* stg = (b == 0 ? sR0 : sR1);
-        const uint32_t tacc = (b == 0 ? tAcc0 : tAcc1) + lane_base;
-#pragma unroll 1
-        for (int c = 0; c < D / 32; ++c) {
-          uint32_t o[32];
-          if (nvis > 0) {
-            tmem_ld32(tacc + c * 32, o);
-            tmem_wait_ld();
           } else {
+            // rows = queries rrow0 + r, columns = keys row64 * 64 + col
+            const int qi0 = rrow0 + r_lo, qi1 = qi0 + 8;
+            const bool qv0 = qi0 < p.sq, qv1 = qi1 < p.sq;
+            const float lse0 = qv0 ? p.lse[stat + qi0] * LOG2E : 0.f, lse1 = qv1 ? p.lse[stat + qi1] * LOG2E : 0.f;
+            const float dl0 = qv0 ? p.delta[stat + qi0] : 0.f, dl1 = qv1 ? p.delta[stat + qi1] : 0.f;
+            const long long qpos0 = q_row_pos(p, rrow0) + r_lo, qpos1 = qpos0 + 8;
 #pragma unroll
-            for (int k = 0; k < 32; ++k) o[k] = 0u;
-          }
-          uint8_t* box = stg + (c >> 1) * 16384 + row * 128;
+            for (int jj = 0; jj < 8; ++jj) {
+              float pr[4], ds[4];
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 v;
-            v.x = pack_bf16(__uint_as_float(o[8 * q + 0]), __uint_as_float(o[8 * q + 1]));
-            v.y = pack_bf16(__uint_as_float(o[8 * q + 2]), __uint_as_float(o[8 * q + 3]));
-            v.z = pack_bf16(__uint_as_float(o[8 * q + 4]), __uint_as_float(o[8 * q + 5]));
-            v.w = pack_bf16(__uint_as_float(o[8 * q + 6]), __uint_as_float(o[8 * q + 7]));
-            const int chunk = (c & 1) * 4 + q;
-            *reinterpret_cast<uint4*>(box + ((chunk ^ (row & 7)) << 4)) = v;
-          }
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(acc_empty);                          // every warpgroup thread, also the idle warpgroup of MODE 1
-      if (mine) {
-        fence_proxy_async_smem();
-        named_bar_sync(1 + b, 128);
-        if (quad == 0 && lane == 0) {
-          for (int bx = 0; bx < BOXES; ++bx) {
-            if (MODE == 0) {
-              if (b == 0) tma_store_4d(&tmOut0, sR0 + bx * 16384, bx * 64, w.rt * 128, w.kvh, w.b);   // dV
-              else tma_store_4d(&tmOut1, sR1 + bx * 16384, bx * 64, w.rt * 128, w.kvh, w.b);         // dK
-            } else {
-              tma_store_4d(&tmOut0, sR0 + bx * 16384, bx * 64, w.rt * 128, w.h_fixed, w.b);           // dQ
+              for (int e = 0; e < 2; ++e) {
+                const int ki = row64 * 64 + 8 * jj + cq + e;
+                const long long kpos = p.kv_pos0 + ki;
+                const bool kv = ki < p.sk;
+                const bool vis0 = qv0 && kv && (!p.causal || kpos <= qpos0);
+                const bool vis1 = qv1 && kv && (!p.causal || kpos <= qpos1);
+                pr[e] = vis0 ? ex2(fmaf(x[4 * jj + e], scale_log2, -lse0)) : 0.f;
+                pr[2 + e] = vis1 ? ex2(fmaf(x[4 * jj + 2 + e], scale_log2, -lse1)) : 0.f;
+                ds[e] = pr[e] * (dp[4 * jj + e] - dl0) * scale;
+                ds[2 + e] = pr[2 + e] * (dp[4 * jj + 2 + e] - dl1) * scale;
+              }
+              dsk[2 * jj] = pack_bf16(ds[0], ds[1]);
+              dsk[2 * jj + 1] = pack_bf16(ds[2], ds[3]);
+              pk[2 * jj] = pk[2 * jj + 1] = 0u;
             }
+          }
+          wgmma_fence();
+          if (MODE == 0) {
+            mma_acc<D>(acc0, pk, s1mn + so);         // dV += P^T dO
+            mma_acc<D>(acc1, dsk, s0mn + so);        // dK += dS^T Q
+          } else {
+            mma_acc<D>(acc0, dsk, s0mn + so);        // dQ += dS K
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+          wgmma_keep(acc0);
+          wgmma_keep(acc1);
+        }
+        if (wg_tid == 0) mbar_arrive(&str_empty[st]);
+      };
+
+      if (MODE == 0) {
+        for (int g = 0; g < G; ++g)
+          for (int qt = 0; qt < n_q64; ++qt)
+            if (q_sees(p, qt, (long long)t * 128)) step(qt, head * G + g, q_sees(p, qt, (long long)rrow0));
+      } else {
+        const int n = n_k_steps(t);
+        const long long my_last = q_row_pos(p, rrow0) + 63 - p.kv_pos0;   // last key index this half sees
+        for (int kt = 0; kt < n; ++kt) step(kt, head, !p.causal || (long long)kt * 64 <= my_last);
+      }
+
+      // ---------------- epilogue: bf16 outputs staged in this warpgroup's half of the resident tiles -> TMA ----------
+      named_bar_sync(1 + c, 128);    // every MMA of this warpgroup that read the resident rows has completed
+      stage_rows<D>(sR1 + c * 8192, acc0, r_lo, cq);                  // dV | dQ
+      if (MODE == 0) stage_rows<D>(sR0 + c * 8192, acc1, r_lo, cq);   // dK
+      fence_proxy_async_smem();
+      named_bar_sync(1 + c, 128);
+      if (wg_tid == 0) {
+        const int nrow = MODE == 0 ? p.sk : p.sq;
+        if (rrow0 < nrow) {
+          for (int bx = 0; bx < BOXES; ++bx) {
+            tma_store_4d(&tmOut0, sR1 + c * 8192 + bx * 16384, bx * 64, rrow0, head, b);
+            if (MODE == 0) tma_store_4d(&tmOut1, sR0 + c * 8192 + bx * 16384, bx * 64, rrow0, head, b);
           }
           tma_store_commit();
           tma_store_wait_read0();
-          mbar_arrive(res_empty);
         }
-      } else if (quad == 0 && lane == 0) {
         mbar_arrive(res_empty);
       }
     }
-    if (quad == 0 && lane == 0) tma_store_wait_all0();
+    if (wg_tid == 0) tma_store_wait_all0();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
-static int make_map(CUtensorMap* m, const void* ptr, int64_t D, int64_t s, int64_t h, int64_t b, const int64_t* str) {
-  const uint32_t box[4] = {64, 128, 1, 1};
+static int make_map(CUtensorMap* m, const void* ptr, int64_t D, int64_t s, int64_t h, int64_t b, const int64_t* str,
+                    uint32_t rows) {
+  const uint32_t box[4] = {64, rows, 1, 1};
   const uint64_t dims[4] = {(uint64_t)D, (uint64_t)s, (uint64_t)h, (uint64_t)b};
   const uint64_t st[4] = {2, (uint64_t)str[1] * 2, (uint64_t)str[2] * 2, (uint64_t)str[0] * 2};
   return encode_tmap_bf16(m, ptr, 4, dims, st, box, true);
@@ -819,16 +390,21 @@ static int make_map(CUtensorMap* m, const void* ptr, int64_t D, int64_t s, int64
 template <int D>
 static int launch_bwd(const lv_attn_bwd_params* a, cudaStream_t s) {
   const lv_attn_params* f = &a->fwd;
-  constexpr int SMEM = 6 * 128 * D * 2 + 2 * 256 * 4 + 128 + 1024;
-  CUtensorMap tmQ, tmK, tmV, tmdO, tmdQ, tmdK, tmdV;
+  constexpr int SMEM = BwdCfg<D>::SMEM;
+  // resident operands: 128-row boxes; streamed operands and outputs: 64-row boxes
+  CUtensorMap tmQr, tmdOr, tmKr, tmVr, tmQs, tmdOs, tmKs, tmVs, tmdQ, tmdK, tmdV;
   int r;
-  if ((r = make_map(&tmQ, f->q, D, f->sq, f->hq, f->batch, f->q_strides))) return r;
-  if ((r = make_map(&tmK, f->k, D, f->sk, f->hkv, f->batch, f->k_strides))) return r;
-  if ((r = make_map(&tmV, f->v, D, f->sk, f->hkv, f->batch, f->v_strides))) return r;
-  if ((r = make_map(&tmdO, a->d_out, D, f->sq, f->hq, f->batch, a->do_strides))) return r;
-  if ((r = make_map(&tmdQ, a->dq, D, f->sq, f->hq, f->batch, a->dq_strides))) return r;
-  if ((r = make_map(&tmdK, a->dk, D, f->sk, f->hkv, f->batch, a->dk_strides))) return r;
-  if ((r = make_map(&tmdV, a->dv, D, f->sk, f->hkv, f->batch, a->dv_strides))) return r;
+  if ((r = make_map(&tmQr, f->q, D, f->sq, f->hq, f->batch, f->q_strides, 128))) return r;
+  if ((r = make_map(&tmdOr, a->d_out, D, f->sq, f->hq, f->batch, a->do_strides, 128))) return r;
+  if ((r = make_map(&tmKr, f->k, D, f->sk, f->hkv, f->batch, f->k_strides, 128))) return r;
+  if ((r = make_map(&tmVr, f->v, D, f->sk, f->hkv, f->batch, f->v_strides, 128))) return r;
+  if ((r = make_map(&tmQs, f->q, D, f->sq, f->hq, f->batch, f->q_strides, 64))) return r;
+  if ((r = make_map(&tmdOs, a->d_out, D, f->sq, f->hq, f->batch, a->do_strides, 64))) return r;
+  if ((r = make_map(&tmKs, f->k, D, f->sk, f->hkv, f->batch, f->k_strides, 64))) return r;
+  if ((r = make_map(&tmVs, f->v, D, f->sk, f->hkv, f->batch, f->v_strides, 64))) return r;
+  if ((r = make_map(&tmdQ, a->dq, D, f->sq, f->hq, f->batch, a->dq_strides, 64))) return r;
+  if ((r = make_map(&tmdK, a->dk, D, f->sk, f->hkv, f->batch, a->dk_strides, 64))) return r;
+  if ((r = make_map(&tmdV, a->dv, D, f->sk, f->hkv, f->batch, a->dv_strides, 64))) return r;
   // delta = rowsum(dO * O)
   {
     const long long warps = (long long)f->batch * f->sq * f->hq;
@@ -861,32 +437,18 @@ static int launch_bwd(const lv_attn_bwd_params* a, cudaStream_t s) {
   if (attr_once.needed(&attr_dev)) {
     LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<D, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<D, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd2_kernel<D, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd2_kernel<D, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr_once.done(attr_dev);
   }
-  // Default: the warp-specialised, pipelined kernel (attn_bwd2_kernel; 449 vs 370 TFLOP/s at 16K, GPU-validated
-  // round 2).  LV_BWD_VERSION=1 selects the synchronous first version (same arithmetic) for A/B runs.
-  static const int version = [] {
-    const char* e = getenv("LV_BWD_VERSION");
-    return (e != nullptr && e[0] == '1') ? 1 : 2;
-  }();
   {
     p.n_items = p.batch * p.hkv * p.n_kt;
     const int grid = p.n_items < sm_count() ? p.n_items : sm_count();
-    if (version == 2)
-      attn_bwd2_kernel<D, 0><<<grid, B2_THREADS, SMEM, s>>>(tmQ, tmK, tmV, tmdO, tmdV, tmdK, p);
-    else
-      attn_bwd_kernel<D, 0><<<grid, 128, SMEM, s>>>(tmQ, tmK, tmV, tmdO, tmdV, tmdK, p);
+    attn_bwd_kernel<D, 0><<<grid, BW_THREADS, SMEM, s>>>(tmKr, tmVr, tmQs, tmdOs, tmdV, tmdK, p);
     LV_CHECK_LAUNCH("attn_bwd_kernel<dKdV>");
   }
   {
     p.n_items = p.batch * p.hq * p.n_qt;
     const int grid = p.n_items < sm_count() ? p.n_items : sm_count();
-    if (version == 2)
-      attn_bwd2_kernel<D, 1><<<grid, B2_THREADS, SMEM, s>>>(tmQ, tmK, tmV, tmdO, tmdQ, tmdQ, p);
-    else
-      attn_bwd_kernel<D, 1><<<grid, 128, SMEM, s>>>(tmQ, tmK, tmV, tmdO, tmdQ, tmdQ, p);
+    attn_bwd_kernel<D, 1><<<grid, BW_THREADS, SMEM, s>>>(tmQr, tmdOr, tmKs, tmVs, tmdQ, tmdQ, p);
     LV_CHECK_LAUNCH("attn_bwd_kernel<dQ>");
   }
   return LV_OK;

@@ -1,23 +1,17 @@
-// Fused attention forward for sm_100a: softmax(scale * Q K^T + mask) V with online softmax, GQA,
+// Fused attention forward for sm_90a: softmax(scale * Q K^T + mask) V with online softmax, GQA,
 // causal / zig-zag-causal / no mask, LSE output.
 //
-// One persistent CTA per SM, 12 warps, warp-specialised:
-//   warp 0      TMA producer: Q tiles (2 x 128 rows per work item) and a K ring + V ring of
-//               128-row tiles, 128-byte swizzle, mbarrier completion
-//   warp 1      tcgen05.mma issuer (one elected thread).  S_t = Q_t K^T (SS form, both operands
-//               from shared memory) into TMEM; O_t += P_t V (TS form: P read from TMEM, V from
-//               shared memory as an MN-major operand).  Two query tiles are ping-ponged so the
-//               tensor pipe works on tile 1-t while the softmax warps work on tile t:
-//               QK0(j) PV1(j-1) QK1(j) PV0(j) ...
-//   warps 2-3   idle in this kernel (the context-parallel variant uses them to pull remote K/V)
-//   warps 4-7   softmax warpgroup for query tile 0 (one thread per query row)
-//   warps 8-11  softmax warpgroup for query tile 1
-// A softmax thread reads its row of S from TMEM (tcgen05.ld), keeps a running max in the log2
-// domain, rescales O only when the max grew by more than 2^8 (lazy rescale: P <= 256 stays well
-// inside bf16/fp32 range), writes P (bf16) back over S in TMEM (tcgen05.st) and at the end
-// normalises O, stages it in the (now free) Q shared-memory tile and stores it with TMA.
-//
-// TMEM map (512 columns): S0/P0 @0, S1/P1 @128, O0 @256, O1 @256 + D.
+// One persistent CTA per SM, 3 warpgroups, warp-specialised:
+//   warp 0          TMA producer: one 128-row Q tile per work item and a K ring + V ring of 128-row
+//                   tiles, 128-byte swizzle, mbarrier completion
+//   warps 2-3       idle in this kernel (the context-parallel variant uses them to pull remote K/V)
+//   warpgroups 1-2  consumers, 64 query rows each: S = Q K^T with wgmma (both operands from shared memory,
+//                   accumulators in registers), online softmax in registers, then O += P V with P fed to
+//                   wgmma from registers (the S accumulator layout is the A-operand layout) and V read from
+//                   shared memory as an MN-major operand.  The two warpgroups share the K/V tiles but are
+//                   not synchronised with each other beyond the ring barriers, so the warp schedulers can
+//                   overlap one's softmax with the other's MMAs; nothing enforces that order.  At the end O is
+//                   normalised, staged in the warpgroup's half of the (now free) Q tile and stored with TMA.
 //
 // Reference call sites replaced: flash_attn_func / _flash_attention_forward in
 // long_vita_megatron/core/transformer/dot_product_attention.py:318-326, 374-390 and
@@ -42,12 +36,10 @@ struct AttnKParams {
   float scale_log2;
   int q_seg_len;
   long long q_seg_pos0, q_seg_pos1, kv_pos0;
-  int n_qblk;      // ceil(sq / 256)
+  int n_qblk;      // ceil(sq / 128)
   int n_items;     // batch * hq * n_qblk
   int block_major; // 1: order work items (q-block, kv-head, head) - global longest-first; 0: (kv-head, q-block, head)
   int serpentine;  // 1: odd rounds sweep the item list backwards (default); LV_ATTN_SCHED=0 turns it off for A/B runs
-  int poly_exp;    // 1: every 4th exponential of the softmax runs on the FMA pipe (polynomial), the rest on MUFU
-  int mufu_turns;  // 1: the two softmax warps of an SM sub-partition take turns on its MUFU unit (LV_ATTN_TURNS=0: off)
   float* lse;
 };
 
@@ -80,31 +72,21 @@ struct CpKParams {
 // tiles of a query row arrive, so every rank starts on the K/V rows it owns (no waiting at all) and then walks the
 // peers in ring order - rank r reads from r-1 first, r-2 next ... - which staggers the ranks over the NVSwitch ports
 // instead of all of them pulling chunk 0 from rank 0 at once (the "ring" schedule of TE / ring-flash-attn, SURVEY.md
-// 8e).  The two query tiles of a work item share the K/V tiles, and tile t must take part in a PREFIX of the steps
-// (steps j < n[t]): the tiles [0, lo) that both see come first, then [lo, hi), each range in chunk-priority order.
+// 8e).  A query tile sees the key tiles [0, n); they are visited in chunk-priority order.
 struct KvWalk {
-  int lo, hi, a, b, li, g, gend;
-  __device__ __forceinline__ void begin(int n0, int n1) {
-    lo = min(n0, n1);
-    hi = max(n0, n1);
-    a = 0;
-    b = lo;
+  int n, li, g, gend;
+  __device__ __forceinline__ void begin(int n_tiles) {
+    n = n_tiles;
     li = -1;
     g = gend = 0;
   }
-  // global index of the next key tile (call exactly hi times per item)
+  // global index of the next key tile (call exactly n times per item)
   __device__ __forceinline__ int next(const CpKParams& c) {
     for (;;) {
       if (g < gend) return g++;
-      if (++li >= 2 * c.cp) {       // first range done: the tiles only the longer query tile sees
-        a = lo;
-        b = hi;
-        li = -1;
-        continue;
-      }
-      const int ch = (int)((c.order >> (4 * li)) & 15ull);
-      g = max(a, ch * c.tiles_per_chunk);
-      gend = min(b, (ch + 1) * c.tiles_per_chunk);
+      const int ch = (int)((c.order >> (4 * ++li)) & 15ull);
+      g = ch * c.tiles_per_chunk;
+      gend = min(n, (ch + 1) * c.tiles_per_chunk);
     }
   }
 };
@@ -164,89 +146,6 @@ __device__ __forceinline__ uint4 ld_peer_v4(const void* p) {
                : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
                : "l"(p)
                : "memory");
-  return v;
-}
-
-// 2^x on the FMA pipe (no MUFU): round-to-nearest split x = n + f, f in [-0.5, 0.5], cubic minimax for 2^f
-// (max relative error 7.5e-5, tools/exp2_poly.py - 50x below the bf16 rounding P gets anyway), exponent
-// add through the low mantissa bits of the magic-number sum.  x is clamped to >= -125 so the result
-// stays a normal number (a masked -inf score becomes 2^-125 ~ 2e-38 instead of 0: invisible in l and P V).
-__device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -125.f);
-  const float t = x + 12582912.f;            // 1.5 * 2^23: the integer part of x lands in the low mantissa bits
-  const float f = x - (t - 12582912.f);
-  float p = fmaf(0.055171321f, f, 0.24261054f);
-  p = fmaf(p, f, 0.69326099f);
-  p = fmaf(p, f, 0.99992811f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(t) << 23));
-}
-
-// One 32-column chunk of a score row: P = 2^(S * scale_log2 - m), four partial row sums, bf16 pack.
-// POLY: every 4th exponential is evaluated on the FMA pipe (ex2_poly), relieving the MUFU pipe that both
-// softmax warpgroups share (16 ex2 / clk / SM = as many cycles as the two MMAs of a step at d = 128).
-// Two exponentials at once on the FMA / ALU pipes with packed fp32 arithmetic (ex2_poly for a pair): 2 FMNMX (clamp),
-// 3 FADD2 (magic-number split x = n + f), 3 FFMA2 (cubic), 2 LEA (exponent insert) = 5 issue slots per element and no
-// MUFU slot, against 8 MUFU cycles per element otherwise.
-__device__ __forceinline__ void ex2_poly_pair(float x0, float x1, float& p0, float& p1) {
-  x0 = fmaxf(x0, -125.f);
-  x1 = fmaxf(x1, -125.f);
-  float t0, t1, n0, n1, f0, f1;
-  fadd2(t0, t1, x0, x1, 12582912.f, 12582912.f);
-  fadd2(n0, n1, t0, t1, -12582912.f, -12582912.f);
-  fadd2(f0, f1, x0, x1, -n0, -n1);
-  float q0, q1;
-  ffma2v(q0, q1, f0, f1, 0.055171321f, 0.055171321f, 0.24261054f, 0.24261054f);
-  ffma2v(q0, q1, q0, q1, f0, f1, 0.69326099f, 0.69326099f);
-  ffma2v(q0, q1, q0, q1, f0, f1, 0.99992811f, 0.99992811f);
-  p0 = __int_as_float(__float_as_int(q0) + (__float_as_int(t0) << 23));
-  p1 = __int_as_float(__float_as_int(q1) + (__float_as_int(t1) << 23));
-}
-
-// One 32-column chunk of a score row: P = 2^(S * scale_log2 - m), four partial row sums, bf16 pack.
-// POLY = number of element PAIRS per 8 (16 elements) whose exponentials run on the FMA pipe instead of the MUFU:
-// 0 (none), 2 (25 %), 3 (37.5 %), 4 (50 %).  The MUFU unit delivers 4 results per cycle per SM sub-partition - a 128 x
-// 128 tile keeps it busy 1024 cycles, as long as the tile's two MMAs - and is the softmax's bottleneck; the packed
-// fp32 forms (2.5 issue slots per MUFU element, 6.5 per polynomial one) leave room to move part of the work over.
-template <int POLY>
-__device__ __forceinline__ void softmax_exp_chunk(const uint32_t (&sc)[32], float scale_log2, float neg_m, float& l0,
-                                                  float& l1, float& l2, float& l3, uint32_t (&pk)[16]) {
-#pragma unroll
-  for (int i = 0; i < 32; i += 4) {
-    float x0, x1, x2, x3;
-    ffma2(x0, x1, __uint_as_float(sc[i + 0]), __uint_as_float(sc[i + 1]), scale_log2, neg_m);
-    ffma2(x2, x3, __uint_as_float(sc[i + 2]), __uint_as_float(sc[i + 3]), scale_log2, neg_m);
-    // pairs are numbered 0..7 inside a 16-element window; which of them take the polynomial is a compile-time pattern
-    const int pair_a = (i / 2) & 7, pair_b = (i / 2 + 1) & 7;
-    constexpr unsigned pattern = POLY == 2 ? 0x44u : (POLY == 3 ? 0x54u : (POLY == 4 ? 0xAAu : 0u));
-    float p0, p1, p2, p3;
-    if ((pattern >> pair_a) & 1u) {
-      ex2_poly_pair(x0, x1, p0, p1);
-    } else {
-      p0 = ex2(x0);
-      p1 = ex2(x1);
-    }
-    if ((pattern >> pair_b) & 1u) {
-      ex2_poly_pair(x2, x3, p2, p3);
-    } else {
-      p2 = ex2(x2);
-      p3 = ex2(x3);
-    }
-    fadd2(l0, l1, l0, l1, p0, p1);
-    fadd2(l2, l3, l2, l3, p2, p3);
-    pk[i / 2] = pack_bf16(p0, p1);
-    pk[i / 2 + 1] = pack_bf16(p2, p3);
-  }
-}
-
-// Exponentials on the FMA pipe, in element pairs per 8 pairs: LV_ATTN_POLY = 0 | 2 | 3 | 4 (default ATTN_POLY_DEFAULT).
-constexpr int ATTN_POLY_DEFAULT = 2;   // measured round 2: 25 % is the best share at both head dims (profiles/README.md)
-static int attn_poly_exp() {
-  static const int v = [] {
-    const char* e = getenv("LV_ATTN_POLY");
-    if (e == nullptr) return ATTN_POLY_DEFAULT;
-    const int x = atoi(e);
-    return (x == 0 || x == 2 || x == 3 || x == 4) ? x : (x == 1 ? 2 : ATTN_POLY_DEFAULT);
-  }();
   return v;
 }
 
@@ -381,20 +280,11 @@ struct AttnCfg {
   static constexpr int KV_STAGES = (D == 128) ? 2 : 4;
   static constexpr int TILE_BYTES = 128 * D * 2;           // one 128-row tile of Q / K / V
   static constexpr int BOXES = D / 64;                     // 64-column (128-byte) TMA boxes per row
-  // Q tiles of two work items in flight when they fit (head_dim 64: 4 x 16 KB): the next item's Q lands while this
-  // one computes, and its first Q.K^T does not wait for this item's epilogue.  Short items - the ViT's 9 key tiles per
-  // (frame, head, 256 rows) - otherwise pay an exposed TMA round trip (~1.5 us) per item.
-  // (compile-time switch while the two-item path is being validated: -DLV_ATTN_QBUF64=2)
-#ifndef LV_ATTN_QBUF64
-#define LV_ATTN_QBUF64 1
-#endif
-  static constexpr int QBUF = (D == 64) ? LV_ATTN_QBUF64 : 1;
-  static constexpr int SMEM_Q = QBUF * 2 * TILE_BYTES;
+  static constexpr int SMEM_Q = TILE_BYTES;
   static constexpr int SMEM_K = KV_STAGES * TILE_BYTES;
   static constexpr int SMEM_V = KV_STAGES * TILE_BYTES;
-  static constexpr int SMEM_BAR = 512;
+  static constexpr int SMEM_BAR = 256;
   static constexpr int SMEM_TOTAL = SMEM_Q + SMEM_K + SMEM_V + SMEM_BAR + 1024;
-  static constexpr uint32_t TM_S0 = 0, TM_S1 = 128, TM_O0 = 256, TM_O1 = 256 + D;
 };
 
 // Static work assignment: the item list is sorted longest-first; CTAs sweep it boustrophedon (round r
@@ -427,10 +317,10 @@ __device__ __forceinline__ void split_item(const AttnKParams& p, int item, int& 
 }
 
 struct WorkItem {
-  int b, h, kvh, qblk;
-  int n[2];          // kv tiles each query tile attends to (0: nothing to do)
-  long long qpos[2]; // global position of row 0 of each query tile
-  int row0[2];       // local row index of row 0 of each query tile
+  int b, h, kvh;
+  int n;             // kv tiles the query tile attends to (0: nothing to do)
+  long long qpos;    // global position of row 0 of the query tile
+  int row0;          // local row index of row 0 of the query tile
 };
 
 __device__ __forceinline__ WorkItem decode_item(const AttnKParams& p, int item) {
@@ -439,38 +329,51 @@ __device__ __forceinline__ WorkItem decode_item(const AttnKParams& p, int item) 
   int g, rank;
   split_item(p, item, w.b, w.kvh, rank, g);
   w.h = w.kvh * G + g;
-  w.qblk = p.causal ? (p.n_qblk - 1 - rank) : rank;   // heaviest causal blocks first
+  const int qblk = p.causal ? (p.n_qblk - 1 - rank) : rank;   // heaviest causal blocks first
   const int n_kv_tiles = (p.sk + A_BN - 1) / A_BN;
-#pragma unroll
-  for (int t = 0; t < 2; ++t) {
-    const int row0 = w.qblk * 256 + t * A_BM;
-    w.row0[t] = row0;
-    const int seg = row0 / p.q_seg_len;
-    w.qpos[t] = (seg == 0 ? p.q_seg_pos0 : p.q_seg_pos1) + (row0 - seg * p.q_seg_len);
-    int n = 0;
-    if (row0 < p.sq) {
-      n = n_kv_tiles;
-      if (p.causal) {
-        const long long hi = w.qpos[t] + (A_BM - 1) - p.kv_pos0;  // last visible key index for the tile
-        if (hi < 0)
-          n = 0;
-        else {
-          const long long lim = hi / A_BN + 1;
-          if (lim < n) n = (int)lim;
-        }
-      }
+  w.row0 = qblk * A_BM;
+  const int seg = w.row0 / p.q_seg_len;
+  w.qpos = (seg == 0 ? p.q_seg_pos0 : p.q_seg_pos1) + (w.row0 - seg * p.q_seg_len);
+  int n = n_kv_tiles;
+  if (p.causal) {
+    const long long hi = w.qpos + (A_BM - 1) - p.kv_pos0;  // last visible key index for the tile
+    if (hi < 0)
+      n = 0;
+    else {
+      const long long lim = hi / A_BN + 1;
+      if (lim < n) n = (int)lim;
     }
-    w.n[t] = n;
   }
+  w.n = n;
   return w;
 }
 
-// POLY: every 4th exponential on the FMA pipe (ex2_poly).  TURNS: MUFU turn-taking of the two softmax warps of an
-// SM sub-partition (see the softmax section).  Both are compile-time so the per-step loop carries no flag tests.
-// HALF: the softmax warps publish P in two 64-key halves and the issuer starts the P.V k-steps of the first half while
-// the exponentials of the second half are still running - it takes 256 of the 512 P.V cycles off the serial chain
-// QK -> softmax -> PV of a query tile.
-template <int D, bool CP, int POLY, bool TURNS, bool HALF>
+// S = Q K^T for one 64-row half of the query tile against one 128-key tile (fp32 accumulators, m64n128k16 steps).
+template <int D>
+__device__ __forceinline__ void mma_qk(float (&s)[64], uint64_t qdesc, uint64_t kdesc) {
+#pragma unroll
+  for (int kk = 0; kk < D / 16; ++kk) {
+    // K-steps of 16 columns: four per 128-byte row, the next 64 head-dim columns one 16 KB box further
+    const uint32_t qoff = ((kk / 4) * 16384 + (kk % 4) * 32) >> 4;
+    wgmma_ss_n128(s, qdesc + qoff, kdesc + qoff, kk != 0 ? 1u : 0u);
+  }
+}
+
+// O += P V: P (bf16, packed in the accumulator layout of S) from registers, V tile MN-major from shared memory,
+// 16 key rows (2 KB) per k-step.
+template <int D>
+__device__ __forceinline__ void mma_pv(float (&o)[D / 2], const uint32_t (&pk)[32], uint64_t vdesc) {
+#pragma unroll
+  for (int kk = 0; kk < A_BN / 16; ++kk) {
+    const uint32_t a[4] = {pk[4 * kk], pk[4 * kk + 1], pk[4 * kk + 2], pk[4 * kk + 3]};
+    if constexpr (D == 128)
+      wgmma_rs_n128(o, a, vdesc + (uint64_t)(kk * 128), 1u);
+    else
+      wgmma_rs_n64(o, a, vdesc + (uint64_t)(kk * 128), 1u);
+  }
+}
+
+template <int D, bool CP>
 __global__ void __launch_bounds__(A_THREADS, 1)
     attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO,
@@ -483,20 +386,12 @@ __global__ void __launch_bounds__(A_THREADS, 1)
   uint8_t* sK = sQ + Cfg::SMEM_Q;
   uint8_t* sV = sK + Cfg::SMEM_K;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + Cfg::SMEM_V);
-  constexpr int QB = Cfg::QBUF;
-  uint64_t* q_full = bars;            // [QB][2]
-  uint64_t* q_empty = bars + 4;       // [QB][2]
-  uint64_t* k_full = bars + 8;        // [NS]
-  uint64_t* k_empty = bars + 8 + NS;  // [NS]
-  uint64_t* v_full = bars + 8 + 2 * NS;
-  uint64_t* v_empty = bars + 8 + 3 * NS;
-  uint64_t* s_full = bars + 8 + 4 * NS;   // [2]
-  uint64_t* p_full = s_full + 2;          // [2]
-  uint64_t* o_full = p_full + 2;          // [2]
-  uint64_t* o_free = o_full + 2;          // [2]: the epilogue has read O_t out of TMEM (the next item's first P.V overwrites it)
-  uint64_t* tok = o_free + 2;             // [2 tiles][4 SM sub-partitions]: MUFU turn-taking, see the softmax warps
-  uint64_t* p_half = tok + 8;             // [2]: the first 64 keys of P_t are in TMEM (HALF: P.V starts on them early)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(p_half + 2);
+  uint64_t* q_full = bars;            // [1]
+  uint64_t* q_empty = bars + 1;       // [1]: both consumer warpgroups have stored their O half out of the Q tile
+  uint64_t* k_full = bars + 2;        // [NS]
+  uint64_t* k_empty = bars + 2 + NS;  // [NS]
+  uint64_t* v_full = bars + 2 + 2 * NS;
+  uint64_t* v_empty = bars + 2 + 3 * NS;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -506,881 +401,249 @@ __global__ void __launch_bounds__(A_THREADS, 1)
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     tma_prefetch_desc(&tmO);
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&q_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 4);
-      mbar_init(&o_full[i], 1);
-      mbar_init(&o_free[i], 4);
-      mbar_init(&p_half[i], 4);
-    }
-    for (int i = 0; i < 8; ++i) mbar_init(&tok[i], 1);
+    mbar_init(q_full, 1);
+    mbar_init(q_empty, 2);
     for (int i = 0; i < NS; ++i) {
       mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
+      mbar_init(&k_empty[i], 2);
       mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
+      mbar_init(&v_empty[i], 2);
     }
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // =========================== TMA producer ===========================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
-    if (lane == 0) {
-      uint32_t item_cnt = 0, kcnt = 0, vcnt = 0;
-      KvWalk walk;
-      for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
-        const WorkItem w = decode_item(p, item);
-        const int nmax = max(w.n[0], w.n[1]);
-        if (CP) walk.begin(w.n[0], w.n[1]);
-        const int qb = (int)(item_cnt % QB);
-        const uint32_t qpar = (item_cnt / QB) & 1;
-        auto load_kv = [&](int j) {
-          int g = j;            // global key tile visited in step j
-          if (CP) {
-            g = walk.next(cpp);
-            // staged by the copier warps of this GPU (any CTA)?  One L2 poll per tile; the K / V rings keep the
-            // producer a step ahead of the tensor pipe, so the poll latency is off the critical path.
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
+    if (warp == 0) {
+      // =========================== TMA producer ===========================
+      if (lane == 0) {
+        uint32_t item_cnt = 0, kcnt = 0, vcnt = 0;
+        KvWalk walk;
+        for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
+          const WorkItem w = decode_item(p, item);
+          if (CP) walk.begin(w.n);
+          const int pre = min(NS, w.n);
+          auto load_tile = [&](int j) {
+            int g = j;            // global key tile visited in step j
+            if (CP) {
+              g = walk.next(cpp);
+              // staged by the copier warps of this GPU (any CTA)?  One L2 poll per tile; the K / V rings keep the
+              // producer a step ahead of the tensor cores, so the poll latency is off the critical path.
+              {
+                [[maybe_unused]] uint32_t spins = 0;
+                PeerWait pw;
+                while (ld_acquire_gpu(cpp.blk_flags + g) < cpp.epoch1 * CP_SUB) {
+                  LV_SPIN_GUARD(spins, "staged block flag", cpp.blk_flags + g, cpp.epoch1 * CP_SUB)
+                  if (pw.expired(cpp, CP_FAULT_BLOCK)) break;
+                }
+              }
+              fence_proxy_async_all();   // copier warps wrote the staging rows through the generic proxy
+            }
             {
-              [[maybe_unused]] uint32_t spins = 0;
-              PeerWait pw;
-              while (ld_acquire_gpu(cpp.blk_flags + g) < cpp.epoch1 * CP_SUB) {
-                LV_SPIN_GUARD(spins, "staged block flag", cpp.blk_flags + g, cpp.epoch1 * CP_SUB)
-                if (pw.expired(cpp, CP_FAULT_BLOCK)) break;
-              }
+              const int st = kcnt % NS;
+              mbar_wait(&k_empty[st], ((kcnt / NS) & 1) ^ 1);
+              mbar_arrive_expect_tx(&k_full[st], Cfg::TILE_BYTES);
+              for (int bx = 0; bx < Cfg::BOXES; ++bx)
+                tma_load_4d(sK + st * Cfg::TILE_BYTES + bx * 16384, &tmK, &k_full[st], bx * 64, g * A_BN, w.kvh, w.b,
+                            kEvictLast);
+              ++kcnt;
             }
-            fence_proxy_async_all();   // copier warps wrote the staging rows through the generic proxy
-          }
-          {
-            const int st = kcnt % NS;
-            mbar_wait(&k_empty[st], ((kcnt / NS) & 1) ^ 1);
-            mbar_arrive_expect_tx(&k_full[st], Cfg::TILE_BYTES);
-            for (int bx = 0; bx < Cfg::BOXES; ++bx)
-              tma_load_4d(sK + st * Cfg::TILE_BYTES + bx * 16384, &tmK, &k_full[st], bx * 64, g * A_BN, w.kvh, w.b,
-                          kEvictLast);
-            ++kcnt;
-          }
-          {
-            const int st = vcnt % NS;
-            mbar_wait(&v_empty[st], ((vcnt / NS) & 1) ^ 1);
-            mbar_arrive_expect_tx(&v_full[st], Cfg::TILE_BYTES);
-            for (int bx = 0; bx < Cfg::BOXES; ++bx)
-              tma_load_4d(sV + st * Cfg::TILE_BYTES + bx * 16384, &tmV, &v_full[st], bx * 64, g * A_BN, w.kvh, w.b,
-                          kEvictLast);
-            ++vcnt;
-          }
-        };
-        // With a single Q buffer the Q loads of this item wait for the previous item's epilogue; its first key tiles
-        // do not (their ring slots free up as the previous item's last MMAs retire), so they are requested first.
-        const int pre = (QB == 1) ? min(NS, nmax) : 0;
-        for (int j = 0; j < pre; ++j) load_kv(j);
-        for (int t = 0; t < 2; ++t) {
-          mbar_wait(&q_empty[qb * 2 + t], qpar ^ 1);
-          mbar_arrive_expect_tx(&q_full[qb * 2 + t], Cfg::TILE_BYTES);
+            {
+              const int st = vcnt % NS;
+              mbar_wait(&v_empty[st], ((vcnt / NS) & 1) ^ 1);
+              mbar_arrive_expect_tx(&v_full[st], Cfg::TILE_BYTES);
+              for (int bx = 0; bx < Cfg::BOXES; ++bx)
+                tma_load_4d(sV + st * Cfg::TILE_BYTES + bx * 16384, &tmV, &v_full[st], bx * 64, g * A_BN, w.kvh, w.b,
+                            kEvictLast);
+              ++vcnt;
+            }
+          };
+          // The Q load of this item waits for the previous item's epilogue (O is staged in the Q tile); its first key
+          // tiles do not (their ring slots free up as the previous item's last MMAs retire), so they are requested first.
+          for (int j = 0; j < pre; ++j) load_tile(j);
+          mbar_wait(q_empty, (item_cnt & 1) ^ 1);
+          mbar_arrive_expect_tx(q_full, Cfg::TILE_BYTES);
           for (int bx = 0; bx < Cfg::BOXES; ++bx)
-            tma_load_4d(sQ + (qb * 2 + t) * Cfg::TILE_BYTES + bx * 16384, &tmQ, &q_full[qb * 2 + t], bx * 64, w.row0[t], w.h, w.b,
-                        kEvictFirst);
+            tma_load_4d(sQ + bx * 16384, &tmQ, q_full, bx * 64, w.row0, w.h, w.b, kEvictFirst);
+          for (int j = pre; j < w.n; ++j) load_tile(j);
         }
-        for (int j = pre; j < nmax; ++j) load_kv(j);
       }
+    } else if (warp >= 2) {
+      // =========================== warps 2-3: context-parallel K/V copier ===========================
+      if (CP) cp_copier(cpp, warp, lane);
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
-    {
-      // The whole warp executes this warp-uniform control flow and ONE elected lane issues the
-      // tcgen05 instructions: descriptor arithmetic then lives in uniform registers.  (With the issue
-      // loop under `if (lane == 0)` the compiler wrapped every MMA in an ELECT / R2UR.BROADCAST /
-      // BRA.U.ANY sequence: ~73 issue cycles per 64-cycle MMA - the issuer was 64 % busy and bounded the
-      // kernel, profiles/README.md.)
-      constexpr uint32_t idesc_qk = make_idesc_bf16(A_BM, A_BN, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(A_BM, D, 0, 1);
-      const uint32_t tS[2] = {tmem_base + Cfg::TM_S0, tmem_base + Cfg::TM_S1};
-      const uint32_t tO[2] = {tmem_base + Cfg::TM_O0, tmem_base + Cfg::TM_O1};
-      uint32_t item_cnt = 0, kcnt = 0, vcnt_wait = 0, vcnt_rel = 0;
-      uint32_t pcnt[2] = {0, 0};
-      uint32_t of_cnt[2] = {0, 0};     // items so far in which tile t had key tiles (= completed o_free[t] phases)
-
-      // tiles are 1024-byte aligned, so stepping a descriptor is a plain add on its 14-bit address field
-      const uint64_t qdesc0 = make_smem_desc(smem_u32(sQ), 16, 1024);
-      uint64_t qdesc[2] = {qdesc0, qdesc0};
-      const uint64_t kdesc0 = make_smem_desc(smem_u32(sK), 16, 1024);
-      const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), 16384, 1024);
-      auto issue_qk = [&](int t, int kst) {
-        const uint64_t qd = qdesc[t];
-        const uint64_t kd = kdesc0 + (uint64_t)((kst * Cfg::TILE_BYTES) >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (int kk = 0; kk < D / 16; ++kk) {
-            const uint32_t off = ((kk / 4) * 16384 + (kk % 4) * 32) >> 4;
-            umma_ss(tS[t], qd + off, kd + off, idesc_qk, kk != 0 ? 1u : 0u);
-          }
-        }
-        __syncwarp();
-      };
-      auto issue_pv = [&](int t, int vst, bool accumulate) {
-        const uint64_t vd = vdesc0 + (uint64_t)((vst * Cfg::TILE_BYTES) >> 4);
-        const bool leader = elect_one();
-#pragma unroll
-        for (int kk = 0; kk < A_BN / 16; ++kk) {
-          if (HALF && kk == A_BN / 32) {
-            // second half of P_t: pcnt[t] was advanced by the caller, so this step's phase is pcnt[t] - 1
-            mbar_wait(&p_full[t], (pcnt[t] - 1) & 1);
-            tc_fence_after();
-          }
-          // A: P_t rows in TMEM, 16 bf16 (= 8 columns) per k-step.  B: V tile, MN-major: 16 key rows
-          // (2 KB) per k-step, the second 64 head-dim columns live one 16 KB box further.
-          if (leader) umma_ts(tO[t], tS[t] + kk * 8, vd + (uint64_t)(kk * 128), idesc_pv, (accumulate || kk != 0) ? 1u : 0u);
-        }
-        __syncwarp();
-      };
-      auto commit = [&](uint64_t* bar) {
-        if (elect_one()) umma_commit(bar);
-        __syncwarp();
-      };
-
-      for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
-        const WorkItem w = decode_item(p, item);
-        const int n0 = w.n[0], n1 = w.n[1];
-        const int nmax = max(n0, n1);
-        const int qb = (int)(item_cnt % QB);
-        const uint32_t qpar = (item_cnt / QB) & 1;
-        qdesc[0] = qdesc0 + (uint64_t)(((qb * 2 + 0) * Cfg::TILE_BYTES) >> 4);
-        qdesc[1] = qdesc0 + (uint64_t)(((qb * 2 + 1) * Cfg::TILE_BYTES) >> 4);
-        mbar_wait(&q_full[qb * 2 + 0], qpar);
-        mbar_wait(&q_full[qb * 2 + 1], qpar);
-        tc_fence_after();
-        // O_t of the previous item with key tiles read out by its epilogue?  o_free[t] completes one phase per item in
-        // which tile t HAS key tiles (n[t] > 0) - both sides count those items the same way.  (Counting every item
-        // let the epilogue warps of a tile without key tiles - the empty second tile of the ViT's last query block -
-        // arrive for two consecutive items before the issuer looked: a parity wait cannot tell two phases from none.)
-        bool o_waited[2] = {false, false};
-        const uint32_t vbase = vcnt_wait;   // V tile j of this item has ring counter vbase + j
-        for (int j = 0; j <= nmax; ++j) {
-          int kst = 0;
-          if (j < nmax) {
-            kst = kcnt % NS;
-            mbar_wait(&k_full[kst], (kcnt / NS) & 1);
-            tc_fence_after();
-          }
-          if (j < n0) {
-            issue_qk(0, kst);
-            commit(&s_full[0]);
-          }
-          if (j >= 1) {
-            if (j - 1 < n1) {
-              const uint32_t vc = vbase + (j - 1);
-              if (vc == vcnt_wait) {
-                mbar_wait(&v_full[vc % NS], (vc / NS) & 1);
-                ++vcnt_wait;
-              }
-              mbar_wait(HALF ? &p_half[1] : &p_full[1], pcnt[1] & 1);
-              ++pcnt[1];
-              if (!o_waited[1]) {
-                if (of_cnt[1] > 0) mbar_wait(&o_free[1], (of_cnt[1] - 1) & 1);
-                o_waited[1] = true;
-              }
-              tc_fence_after();
-              issue_pv(1, vc % NS, j - 1 > 0);
-              if (j - 1 == n1 - 1) commit(&o_full[1]);
-            }
-            // V(j-1) has now been consumed by every PV that needs it
-            commit(&v_empty[vcnt_rel % NS]);
-            ++vcnt_rel;
-          }
-          if (j < n1) {
-            issue_qk(1, kst);
-            commit(&s_full[1]);
-          }
-          if (j < nmax) {
-            commit(&k_empty[kst]);
-            ++kcnt;
-          }
-          if (j < n0) {
-            const uint32_t vc = vbase + j;
-            if (vc == vcnt_wait) {
-              mbar_wait(&v_full[vc % NS], (vc / NS) & 1);
-              ++vcnt_wait;
-            }
-            mbar_wait(HALF ? &p_half[0] : &p_full[0], pcnt[0] & 1);
-            ++pcnt[0];
-            if (!o_waited[0]) {
-              if (of_cnt[0] > 0) mbar_wait(&o_free[0], (of_cnt[0] - 1) & 1);
-              o_waited[0] = true;
-            }
-            tc_fence_after();
-            issue_pv(0, vc % NS, j > 0);
-            if (j == n0 - 1) commit(&o_full[0]);
-          }
-        }
-        if (n0 > 0) ++of_cnt[0];
-        if (n1 > 0) ++of_cnt[1];
-      }
-    }
-  } else if (warp >= 4) {
-    // =========================== softmax / epilogue warpgroups ===========================
+  } else {
+    // =========================== consumer warpgroups ===========================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int t = (warp - 4) >> 2;                // query tile handled by this warpgroup
-    const int quad = warp & 3;                    // TMEM lane quadrant of this warp
-    const int row = quad * 32 + lane;             // row inside the 128-row tile
-    const int wg_tid = (warp - 4 - 4 * t) * 32 + lane;
-    const uint32_t lane_base = uint32_t(quad * 32) << 16;
-    const uint32_t tS = keep_u32(tmem_base + lane_base + (t == 0 ? Cfg::TM_S0 : Cfg::TM_S1));
-    const uint32_t tO = keep_u32(tmem_base + lane_base + (t == 0 ? Cfg::TM_O0 : Cfg::TM_O1));
-    uint32_t item_cnt = 0, scnt = 0, ocnt = 0;
-    // Everything the per-step loop touches is resolved ONCE here: 32-bit shared-window addresses of its barriers
-    // (a generic pointer costs an S2UR + uniform ALU chain per use), the scale, and per item the first step that
-    // needs a mask.  The ncu source view of round 2 showed ~900 of the ~3800 cycles of a (2 x 128 rows) x 128 keys
-    // step going to such scalar set-up on the softmax warps' critical path (profiles/README.md).
-    const uint32_t a_sfull = keep_u32(smem_u32(&s_full[t])), a_pfull = keep_u32(smem_u32(&p_full[t]));
-    const uint32_t a_ofull = keep_u32(smem_u32(&o_full[t])), a_ofree = keep_u32(smem_u32(&o_free[t]));
-    const uint32_t a_phalf = keep_u32(smem_u32(&p_half[t]));
-    // MUFU turn-taking (TURNS): the exponentials of one 128 x 128 score tile keep the MUFU unit of an SM sub-partition
-    // busy for ~1050 cycles.  The two softmax warps of a sub-partition (one per query tile) take turns on it - tile
-    // 0's warp runs exp(j), then tile 1's exp(j), then tile 0's exp(j+1) ... - so that the load / max / store /
-    // hand-off parts of one warp overlap the exp phase of the other instead of both exp phases colliding.
-    // tok[t][quad] is arrived by the OTHER tile's warp when its exp phase ends; waits and arrivals are paired exactly
-    // (both sides know n[0], n[1] of the item).
-    const uint32_t a_tok_mine = keep_u32(smem_u32(&tok[t * 4 + quad])), a_tok_other = keep_u32(smem_u32(&tok[(1 - t) * 4 + quad]));
-    uint32_t tok_cnt = 0;
+    const int c = (warp >> 2) - 1;                // 64-row half of the query tile
+    const int wg_tid = threadIdx.x & 127;
+    const int r_lo = ((wg_tid >> 5) << 4) + (lane >> 2);   // this thread's rows: r_lo and r_lo + 8 (of 64)
+    const int cq = 2 * (lane & 3);                         // its first column in every 8-column group
+    const uint64_t qdesc = make_smem_desc(smem_u32(sQ) + c * 8192, 16, 1024);
+    const uint64_t kdesc0 = make_smem_desc(smem_u32(sK), 16, 1024);
+    const uint64_t vdesc0 = make_smem_desc(smem_u32(sV), 16384, 1024);
     const float scale_log2 = p.scale_log2;
     const int n_kv_tiles = (p.sk + A_BN - 1) / A_BN;
     const int j_ragged = (p.sk % A_BN) ? n_kv_tiles - 1 : 0x7fffffff;
+    uint32_t item_cnt = 0, kcnt = 0, vcnt = 0;
 
     for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
       const WorkItem w = decode_item(p, item);
-      const int n = w.n[t];
-      const int n_other = w.n[1 - t];
-      const int qb = (int)(item_cnt % QB);
-      uint8_t* stage = sQ + (qb * 2 + t) * Cfg::TILE_BYTES;    // this item's Q_t tile doubles as the staging tile of O_t
-      const long long qpos = w.qpos[t] + row;           // global position of this thread's query row
-      // first key tile (GLOBAL index) that needs a mask: the diagonal ones (kv_pos0 + 128 g + 127 > position of the
-      // tile's row 0) and the ragged last one
+      const int n = w.n;
+      // global positions of this thread's two query rows
+      const long long qpos0 = w.qpos + c * 64 + r_lo, qpos1 = qpos0 + 8;
       KvWalk walk;
-      if (CP) walk.begin(w.n[0], w.n[1]);
+      if (CP) walk.begin(n);
+      // first key tile (GLOBAL index) that needs a mask: the diagonal ones and the ragged last one
       int j_mask = j_ragged;
       if (p.causal) {
-        const long long dd = w.qpos[t] - p.kv_pos0 - (A_BN - 1);
+        const long long dd = w.qpos + c * 64 - p.kv_pos0 - (A_BN - 1);
         const long long jd = dd < 0 ? 0 : dd / A_BN + 1;
         if (jd < j_mask) j_mask = (int)jd;
       }
-      float m_used = 0.f, l = 0.f;
+      float o[D / 2];
+#pragma unroll
+      for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+      float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running max (log2 domain) and sum per row
+      mbar_wait(q_full, item_cnt & 1);
       for (int j = 0; j < n; ++j) {
         int g = j;         // global key tile of this step (context parallelism visits them out of order)
         if (CP) g = walk.next(cpp);
-        mbar_wait_a(a_sfull, scnt & 1);
-        ++scnt;
-        tc_fence_after();
-        uint32_t s[128];
-        tmem_ld128(tS, s);
-        tmem_wait_ld();
+        const int kst = kcnt % NS;
+        mbar_wait(&k_full[kst], (kcnt / NS) & 1);
+        ++kcnt;
+        float s[64];
+        wgmma_fence();
+        mma_qk<D>(s, qdesc, kdesc0 + (uint64_t)((kst * Cfg::TILE_BYTES) >> 4));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_keep(s);
+        if (wg_tid == 0) mbar_arrive(&k_empty[kst]);
 
         // ---- mask (only diagonal tiles and the ragged last key tile) ----
-        // 32-column chunks with at least one visible key for some row of this warp (warp-uniform).  Only tracked at
-        // head_dim 64 (the ViT's ragged 1025-key rows: 1 live chunk of 4 in every 9th tile); at head_dim 128 the test
-        // per chunk costs more on every step than the skipped exponentials save on the rare diagonal tile.
-        constexpr bool SKIP_DEAD = (D == 64);
-        int live = 4;
         if (g >= j_mask) {
           const long long kidx0 = (long long)g * A_BN;
-          long long lim = p.sk - kidx0;                               // first invalid column (ragged)
-          long long lim_warp = lim;                                   // the same bound for the warp's LAST row
+          long long lim0 = p.sk - kidx0, lim1 = lim0;                 // first invalid column of each row
           if (p.causal) {
-            const long long c = qpos - p.kv_pos0 - kidx0 + 1;         // first masked column (causal)
-            if (c < lim) lim = c;
-            const long long cw = c + (31 - lane);
-            if (cw < lim_warp) lim_warp = cw;
+            lim0 = min(lim0, qpos0 - p.kv_pos0 - kidx0 + 1);
+            lim1 = min(lim1, qpos1 - p.kv_pos0 - kidx0 + 1);
           }
-          const int ilim = lim < 0 ? 0 : (lim > A_BN ? A_BN : (int)lim);
 #pragma unroll
-          for (int i = 0; i < 128; ++i)
-            if (i >= ilim) s[i] = 0xff800000u;  // -inf
-          // chunks beyond the warp's last visible column hold only masked scores: their exponentials are skipped
-          // (P = 0).  The ragged last key tile of the ViT (1025 = 8 x 128 + 1 keys) costs 1 chunk instead of 4.
-          if (SKIP_DEAD) {
-            const int lw = __shfl_sync(0xffffffffu, lim_warp < 0 ? 0 : (lim_warp > A_BN ? A_BN : (int)lim_warp), 0);
-            live = (lw + 31) >> 5;
-          }
-        }
-
-        // ---- row max: 8 independent chains ----
-        float mx[8];
+          for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-        for (int c = 0; c < 8; ++c) mx[c] = fmax3(__uint_as_float(s[c * 16]), __uint_as_float(s[c * 16 + 1]), __uint_as_float(s[c * 16 + 2]));
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-#pragma unroll
-          for (int i = 3; i < 15; i += 2) mx[c] = fmax3(mx[c], __uint_as_float(s[c * 16 + i]), __uint_as_float(s[c * 16 + i + 1]));
-          mx[c] = fmaxf(mx[c], __uint_as_float(s[c * 16 + 15]));
-        }
-        const float mx_all = fmax3(fmax3(mx[0], mx[1], mx[2]), fmax3(mx[3], mx[4], mx[5]), fmaxf(mx[6], mx[7])) * scale_log2;
-
-        // ---- lazy rescale ----
-        if (j == 0) {
-          m_used = (mx_all == -INFINITY) ? 0.f : mx_all;
-        } else {
-          const bool grow = mx_all > m_used + 8.f;
-          if (__any_sync(0xffffffffu, grow)) {
-            const float m_new = fmaxf(m_used, mx_all);
-            const float alpha = ex2(m_used - m_new);
-            m_used = m_new;
-            l *= alpha;
-#pragma unroll 1
-            for (int c = 0; c < D / 32; ++c) {
-              uint32_t o[32];
-              tmem_ld32(tO + c * 32, o);
-              tmem_wait_ld();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-              tmem_st32(tO + c * 32, o);
+            for (int e = 0; e < 2; ++e) {
+              const int col = 8 * jj + cq + e;
+              if (col >= lim0) s[4 * jj + e] = -INFINITY;
+              if (col >= lim1) s[4 * jj + 2 + e] = -INFINITY;
             }
           }
         }
 
-        // ---- P = exp2(S * scale_log2 - m), row sum, bf16 pack, store over S in TMEM ----
-        const float neg_m = -m_used;
-        float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-        if (TURNS) {
-          // my turn on this sub-partition's MUFU?  tile 0 goes first in every step: it waits for tile 1's step j-1,
-          // tile 1 waits for tile 0's step j (only where the other tile has that step at all)
-          const bool need = (t == 0) ? (j >= 1 && j - 1 < n_other) : (j < n_other);
-          if (need) {
-            mbar_wait_a(a_tok_mine, tok_cnt & 1);
-            ++tok_cnt;
-          }
+        // ---- online softmax: row max over the quad of threads that holds a row ----
+        float mx0 = s[0], mx1 = s[2];
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          mx0 = fmaxf(mx0, fmaxf(s[4 * jj], s[4 * jj + 1]));
+          mx1 = fmaxf(mx1, fmaxf(s[4 * jj + 2], s[4 * jj + 3]));
         }
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t pk[32];
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            if (!SKIP_DEAD || 2 * h + c < live) {
-              softmax_exp_chunk<POLY>(reinterpret_cast<const uint32_t(&)[32]>(s[(2 * h + c) * 32]), scale_log2, neg_m, l0, l1, l2, l3,
-                                      reinterpret_cast<uint32_t(&)[16]>(pk[c * 16]));
-            } else {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) pk[c * 16 + i] = 0u;
-            }
-          }
-          if (h == 1 && TURNS) {
-            // the exponentials of this step are issued: hand the MUFU turn over (tile 0 -> tile 1's step j,
-            // tile 1 -> tile 0's step j + 1) before the store / fence / hand-off tail of this step
-            const bool give = (t == 0) ? (j < n_other) : (j + 1 < n_other);
-            __syncwarp();
-            if (give && lane == 0) mbar_arrive_a(a_tok_other);
-          }
-          tmem_st32(tS + h * 32, pk);
-          if (HALF && h == 0) {
-            tmem_wait_st();          // (also covers the lazy O rescale above)
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_a(a_phalf);
-          }
+        for (int off = 1; off <= 2; off <<= 1) {
+          mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off));
+          mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
         }
-        l += (l0 + l1) + (l2 + l3);
-        tmem_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_a(a_pfull);
+        const float mn0 = fmaxf(m0, mx0 * scale_log2), mn1 = fmaxf(m1, mx1 * scale_log2);
+        // a row that has seen only masked keys keeps max -inf: subtract 0 instead (its P and alpha are 0)
+        const float ms0 = mn0 == -INFINITY ? 0.f : mn0, ms1 = mn1 == -INFINITY ? 0.f : mn1;
+        const float alpha0 = ex2(m0 - ms0), alpha1 = ex2(m1 - ms1);
+        m0 = mn0;
+        m1 = mn1;
+        l0 *= alpha0;
+        l1 *= alpha1;
+#pragma unroll
+        for (int jj = 0; jj < D / 8; ++jj) {
+          o[4 * jj] *= alpha0;
+          o[4 * jj + 1] *= alpha0;
+          o[4 * jj + 2] *= alpha1;
+          o[4 * jj + 3] *= alpha1;
+        }
+        uint32_t pk[32];
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+          const float p0 = ex2(fmaf(s[4 * jj], scale_log2, -ms0)), p1 = ex2(fmaf(s[4 * jj + 1], scale_log2, -ms0));
+          const float p2 = ex2(fmaf(s[4 * jj + 2], scale_log2, -ms1)), p3 = ex2(fmaf(s[4 * jj + 3], scale_log2, -ms1));
+          l0 += p0 + p1;
+          l1 += p2 + p3;
+          pk[2 * jj] = pack_bf16(p0, p1);
+          pk[2 * jj + 1] = pack_bf16(p2, p3);
+        }
+
+        // ---- O += P V ----
+        const int vst = vcnt % NS;
+        mbar_wait(&v_full[vst], (vcnt / NS) & 1);
+        ++vcnt;
+        wgmma_fence();
+        mma_pv<D>(o, pk, vdesc0 + (uint64_t)((vst * Cfg::TILE_BYTES) >> 4));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_keep(o);
+        if (wg_tid == 0) mbar_arrive(&v_empty[vst]);
       }
 
-      // ---------------- epilogue: O / l -> bf16 -> smem (swizzled) -> TMA store; LSE ----------------
-      const float inv_l = (n > 0 && l > 0.f) ? 1.f / l : 0.f;
-      if (n > 0) {
-        mbar_wait_a(a_ofull, ocnt & 1);
-        ++ocnt;
-        tc_fence_after();
-      } else {
-        mbar_wait(&q_full[qb * 2 + t], (item_cnt / QB) & 1);   // the Q load into the staging tile must have landed
-      }
-#pragma unroll 1
-      for (int c = 0; c < D / 32; ++c) {
-        uint32_t o[32];
-        if (n > 0) {
-          tmem_ld32(tO + c * 32, o);
-          tmem_wait_ld();
-          if (c == D / 32 - 1) {
-            // O_t is in registers: the next item's first P.V may overwrite the accumulator
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_a(a_ofree);
-          }
-        } else {
+      // ---------------- epilogue: O / l -> bf16 -> smem (swizzled, this half of the Q tile) -> TMA store; LSE -------
 #pragma unroll
-          for (int i = 0; i < 32; ++i) o[i] = 0u;
-        }
-        uint8_t* box = stage + (c >> 1) * 16384 + row * 128;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 v;
-          v.x = pack_bf16(__uint_as_float(o[8 * q + 0]) * inv_l, __uint_as_float(o[8 * q + 1]) * inv_l);
-          v.y = pack_bf16(__uint_as_float(o[8 * q + 2]) * inv_l, __uint_as_float(o[8 * q + 3]) * inv_l);
-          v.z = pack_bf16(__uint_as_float(o[8 * q + 4]) * inv_l, __uint_as_float(o[8 * q + 5]) * inv_l);
-          v.w = pack_bf16(__uint_as_float(o[8 * q + 6]) * inv_l, __uint_as_float(o[8 * q + 7]) * inv_l);
-          const int chunk = (c & 1) * 4 + q;
-          *reinterpret_cast<uint4*>(box + ((chunk ^ (row & 7)) << 4)) = v;
-        }
+      for (int off = 1; off <= 2; off <<= 1) {
+        l0 += __shfl_xor_sync(0xffffffffu, l0, off);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, off);
       }
-      tc_fence_before();
-      if (p.lse != nullptr && w.row0[t] + row < p.sq) {
-        const float lse = (n > 0 && l > 0.f) ? (m_used + log2f(l)) * 0.69314718055994530942f : -INFINITY;
-        p.lse[((long long)w.b * p.hq + w.h) * p.sq + w.row0[t] + row] = lse;
+      const float inv0 = l0 > 0.f ? 1.f / l0 : 0.f, inv1 = l1 > 0.f ? 1.f / l1 : 0.f;
+      uint8_t* stage = sQ + c * 8192;
+      named_bar_sync(1 + c, 128);    // every thread of this warpgroup is done reading its Q rows
+#pragma unroll
+      for (int jj = 0; jj < D / 8; ++jj) {
+        uint8_t* box = stage + (jj >> 3) * 16384;
+        const int ch = jj & 7;       // 16-byte chunk of the 128-byte row
+        *reinterpret_cast<uint32_t*>(box + r_lo * 128 + ((ch ^ (r_lo & 7)) << 4) + cq * 2) =
+            pack_bf16(o[4 * jj] * inv0, o[4 * jj + 1] * inv0);
+        const int r1 = r_lo + 8;
+        *reinterpret_cast<uint32_t*>(box + r1 * 128 + ((ch ^ (r1 & 7)) << 4) + cq * 2) =
+            pack_bf16(o[4 * jj + 2] * inv1, o[4 * jj + 3] * inv1);
+      }
+      if (p.lse != nullptr && (lane & 3) == 0) {
+        const int row = w.row0 + c * 64 + r_lo;
+        float* dst = p.lse + ((long long)w.b * p.hq + w.h) * p.sq;
+        if (row < p.sq) dst[row] = l0 > 0.f ? (m0 + log2f(l0)) * 0.69314718055994530942f : -INFINITY;
+        if (row + 8 < p.sq) dst[row + 8] = l1 > 0.f ? (m1 + log2f(l1)) * 0.69314718055994530942f : -INFINITY;
       }
       fence_proxy_async_smem();
-      named_bar_sync(1 + t, 128);
+      named_bar_sync(1 + c, 128);
       if (wg_tid == 0) {
-        if (w.row0[t] < p.sq) {
-          for (int bx = 0; bx < Cfg::BOXES; ++bx) tma_store_4d(&tmO, stage + bx * 16384, bx * 64, w.row0[t], w.h, w.b);
+        if (w.row0 + c * 64 < p.sq) {
+          for (int bx = 0; bx < Cfg::BOXES; ++bx)
+            tma_store_4d(&tmO, stage + bx * 16384, bx * 64, w.row0 + c * 64, w.h, w.b);
           tma_store_commit();
           tma_store_wait_read0();
         }
-        mbar_arrive(&q_empty[qb * 2 + t]);   // this Q_t / staging tile may be overwritten by a later item's Q load
+        mbar_arrive(q_empty);   // this half of the Q / staging tile may be overwritten by a later item's Q load
       }
     }
     if (wg_tid == 0) tma_store_wait_all0();
-  } else {
-    // =========================== warps 2-3: context-parallel K/V copier ===========================
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
-    if (CP) cp_copier(cpp, warp, lane);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
-}
-
-// ================================================================================================
-// Version 2 of the forward kernel: 64-key softmax steps with DOUBLE-BUFFERED S.
-//
-// v1 aliases P over the only S buffer of a query tile, so QK(j+1) cannot be issued before PV(j) and
-// every iteration pays softmax latency + two mbarrier round trips on the tensor pipe's critical
-// path (measured: 55 % tensor-pipe activity, softmax warps idle 47 % of the time waiting for S).
-// Here each query tile owns two 64-column S buffers (TMEM: S0a S0b S1a S1b O0 O1 = 512 columns);
-// the issuer runs one step ahead - QK_t(i+1) is queued before PV_t(i) - so S(i+1) is ready when
-// softmax(i) retires and the chain becomes throughput- (MUFU / tensor) instead of latency-bound.
-// Work per step and query tile: QK 128x64x128, PV 128x128x64.  Causal skipping is also 64-granular.
-// ================================================================================================
-constexpr int A_BH = 64;
-
-struct WorkItem2 {
-  int b, h, kvh;
-  int n[2];           // 64-key steps per query tile
-  long long qpos[2];
-  int row0[2];
-};
-
-__device__ __forceinline__ WorkItem2 decode_item2(const AttnKParams& p, int item) {
-  WorkItem2 w;
-  const int G = p.hq / p.hkv;
-  int g, rank;
-  split_item(p, item, w.b, w.kvh, rank, g);
-  w.h = w.kvh * G + g;
-  const int qblk = p.causal ? (p.n_qblk - 1 - rank) : rank;
-  const int n_steps = (p.sk + A_BH - 1) / A_BH;
-#pragma unroll
-  for (int t = 0; t < 2; ++t) {
-    const int row0 = qblk * 256 + t * A_BM;
-    w.row0[t] = row0;
-    const int seg = row0 / p.q_seg_len;
-    w.qpos[t] = (seg == 0 ? p.q_seg_pos0 : p.q_seg_pos1) + (row0 - seg * p.q_seg_len);
-    int n = 0;
-    if (row0 < p.sq) {
-      n = n_steps;
-      if (p.causal) {
-        const long long hi = w.qpos[t] + (A_BM - 1) - p.kv_pos0;
-        if (hi < 0)
-          n = 0;
-        else {
-          const long long lim = hi / A_BH + 1;
-          if (lim < n) n = (int)lim;
-        }
-      }
-    }
-    w.n[t] = n;
-  }
-  return w;
 }
 
 template <int D, bool CP>
-__global__ void __launch_bounds__(A_THREADS, 1)
-    attn_fwd2_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO,
-                     const AttnKParams p, const CpKParams cpp) {
-  using Cfg = AttnCfg<D>;
-  constexpr int NS = Cfg::KV_STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sK = sQ + Cfg::SMEM_Q;
-  uint8_t* sV = sK + Cfg::SMEM_K;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + Cfg::SMEM_V);
-  uint64_t* q_full = bars;            // [2]
-  uint64_t* q_empty = bars + 2;       // [2]
-  uint64_t* k_full = bars + 4;        // [NS]
-  uint64_t* k_empty = bars + 4 + NS;
-  uint64_t* v_full = bars + 4 + 2 * NS;
-  uint64_t* v_empty = bars + 4 + 3 * NS;
-  uint64_t* s_full = bars + 4 + 4 * NS;   // [2 tiles][2 buffers]
-  uint64_t* p_full = s_full + 4;          // [2][2]
-  uint64_t* o_done = p_full + 4;          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(o_done + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    tma_prefetch_desc(&tmO);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&q_full[i], 1);
-      mbar_init(&q_empty[i], 1);
-      mbar_init(&o_done[i], 1);
-    }
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_full[i], 4);
-    }
-    for (int i = 0; i < NS; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&k_empty[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&v_empty[i], 1);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // TMEM columns: S_t[b] at t*128 + b*64; O_t at 256 + t*D
-
-  if (warp == 0) {
-    // =========================== TMA producer ===========================
-    if (lane == 0) {
-      uint32_t item_cnt = 0, kcnt = 0, vcnt = 0;
-      int ready_upto = 0;
-      for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
-        const WorkItem2 w = decode_item2(p, item);
-        const int ntile = (max(w.n[0], w.n[1]) + 1) / 2;   // 128-row K/V tiles
-        for (int t = 0; t < 2; ++t) {
-          mbar_wait(&q_empty[t], (item_cnt & 1) ^ 1);
-          mbar_arrive_expect_tx(&q_full[t], Cfg::TILE_BYTES);
-          for (int bx = 0; bx < Cfg::BOXES; ++bx)
-            tma_load_4d(sQ + t * Cfg::TILE_BYTES + bx * 16384, &tmQ, &q_full[t], bx * 64, w.row0[t], w.h, w.b,
-                        kEvictFirst);
-        }
-        for (int j = 0; j < ntile; ++j) {
-          if (CP && j >= ready_upto) {
-            {
-              [[maybe_unused]] uint32_t spins = 0;
-              PeerWait pw;
-              while (ld_acquire_gpu(cpp.blk_flags + j) < cpp.epoch1 * CP_SUB) {
-                LV_SPIN_GUARD(spins, "staged block flag", cpp.blk_flags + j, cpp.epoch1 * CP_SUB)
-                if (pw.expired(cpp, CP_FAULT_BLOCK)) break;
-              }
-            }
-            ready_upto = j + 1;
-            fence_proxy_async_all();
-          }
-          {
-            const int st = kcnt % NS;
-            mbar_wait(&k_empty[st], ((kcnt / NS) & 1) ^ 1);
-            mbar_arrive_expect_tx(&k_full[st], Cfg::TILE_BYTES);
-            for (int bx = 0; bx < Cfg::BOXES; ++bx)
-              tma_load_4d(sK + st * Cfg::TILE_BYTES + bx * 16384, &tmK, &k_full[st], bx * 64, j * A_BN, w.kvh, w.b,
-                          kEvictLast);
-            ++kcnt;
-          }
-          {
-            const int st = vcnt % NS;
-            mbar_wait(&v_empty[st], ((vcnt / NS) & 1) ^ 1);
-            mbar_arrive_expect_tx(&v_full[st], Cfg::TILE_BYTES);
-            for (int bx = 0; bx < Cfg::BOXES; ++bx)
-              tma_load_4d(sV + st * Cfg::TILE_BYTES + bx * 16384, &tmV, &v_full[st], bx * 64, j * A_BN, w.kvh, w.b,
-                          kEvictLast);
-            ++vcnt;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    {   // warp-uniform control flow; one elected lane issues (see the v1 kernel)
-      constexpr uint32_t idesc_qk = make_idesc_bf16(A_BM, A_BH, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(A_BM, D, 0, 1);
-      uint32_t item_cnt = 0;
-      uint32_t kbase = 0, vbase = 0;            // ring counters of this item's tile 0
-      uint32_t scnt[2][2] = {{0, 0}, {0, 0}};   // completed uses of s_full / p_full [tile][buffer]
-      for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
-        const WorkItem2 w = decode_item2(p, item);
-        const int nmax = max(w.n[0], w.n[1]);
-        const int ntile = (nmax + 1) / 2;
-        int k_waited = 0, v_waited = 0;
-        mbar_wait(&q_full[0], item_cnt & 1);
-        mbar_wait(&q_full[1], item_cnt & 1);
-        tc_fence_after();
-
-        auto issue_qk = [&](int t, int i) {
-          const int m = i >> 1;
-          while (k_waited <= m) {
-            const uint32_t c = kbase + k_waited;
-            mbar_wait(&k_full[c % NS], (c / NS) & 1);
-            ++k_waited;
-          }
-          tc_fence_after();
-          const int b = i & 1;
-          const uint64_t qd = make_smem_desc(smem_u32(sQ + t * Cfg::TILE_BYTES), 16, 1024);
-          const uint64_t kd = make_smem_desc(smem_u32(sK + ((kbase + m) % NS) * Cfg::TILE_BYTES) + (i & 1) * 8192, 16, 1024);
-          const uint32_t d_tmem = tmem_base + t * 128 + b * 64;
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < D / 16; ++kk) {
-              const uint32_t off = ((kk / 4) * 16384 + (kk % 4) * 32) >> 4;
-              umma_ss(d_tmem, qd + off, kd + off, idesc_qk, kk != 0 ? 1u : 0u);
-            }
-            umma_commit(&s_full[t * 2 + b]);
-          }
-          __syncwarp();
-        };
-        auto issue_pv = [&](int t, int i) {
-          const int m = i >> 1;
-          while (v_waited <= m) {
-            const uint32_t c = vbase + v_waited;
-            mbar_wait(&v_full[c % NS], (c / NS) & 1);
-            ++v_waited;
-          }
-          const int b = i & 1;
-          mbar_wait(&p_full[t * 2 + b], scnt[t][b] & 1);
-          ++scnt[t][b];
-          tc_fence_after();
-          const uint64_t vd = make_smem_desc(smem_u32(sV + ((vbase + m) % NS) * Cfg::TILE_BYTES) + (i & 1) * 8192, 16384, 1024);
-          const uint32_t a_tmem = tmem_base + t * 128 + b * 64;
-          const uint32_t d_tmem = tmem_base + 256 + t * D;
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < A_BH / 16; ++kk)
-              umma_ts(d_tmem, a_tmem + kk * 8, vd + (uint64_t)(kk * 128), idesc_pv, (i > 0 || kk != 0) ? 1u : 0u);
-            umma_commit(&o_done[t]);
-          }
-          __syncwarp();
-        };
-
-        for (int t = 0; t < 2; ++t)
-          if (w.n[t] > 0) issue_qk(t, 0);
-        auto commit = [&](uint64_t* bar) {
-          if (elect_one()) umma_commit(bar);
-          __syncwarp();
-        };
-        if (nmax == 1) commit(&k_empty[kbase % NS]);
-        for (int i = 0; i < nmax; ++i) {
-          const int s = i + 1;
-          // queue the next step's QK^T of both tiles first (they need no softmax result), so the
-          // tensor pipe has work while this step's probabilities are still being produced
-          if (s < w.n[0]) issue_qk(0, s);
-          if (s < w.n[1]) issue_qk(1, s);
-          if (s < nmax && ((s & 1) == 1 || s == nmax - 1))
-            commit(&k_empty[(kbase + (s >> 1)) % NS]);   // last QK on this K tile has been issued
-          if (i < w.n[0]) issue_pv(0, i);
-          if (i < w.n[1]) issue_pv(1, i);
-          if ((i & 1) == 1 || i == nmax - 1) commit(&v_empty[(vbase + (i >> 1)) % NS]);
-        }
-        kbase += ntile;
-        vbase += ntile;
-      }
-    }
-  } else if (warp >= 4) {
-    // =========================== softmax / epilogue warpgroups ===========================
-    const int t = (warp - 4) >> 2;
-    const int quad = warp & 3;
-    const int row = quad * 32 + lane;
-    const int wg_tid = (warp - 4 - 4 * t) * 32 + lane;
-    const uint32_t lane_base = uint32_t(quad * 32) << 16;
-    const uint32_t tS = tmem_base + lane_base + t * 128;
-    const uint32_t tO = tmem_base + lane_base + 256 + t * D;
-    uint8_t* stage = sQ + t * Cfg::TILE_BYTES;
-    uint32_t item_cnt = 0;
-    uint32_t scnt[2] = {0, 0};   // uses of s_full[t][b]
-    uint32_t pv_base = 0;        // PV commits on o_done[t] before this item
-
-    for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
-      const WorkItem2 w = decode_item2(p, item);
-      const int n = w.n[t];
-      const long long qpos = w.qpos[t] + row;
-      float m_used = 0.f, l = 0.f;
-      for (int i = 0; i < n; ++i) {
-        const int b = i & 1;
-        mbar_wait(&s_full[t * 2 + b], scnt[b] & 1);
-        ++scnt[b];
-        tc_fence_after();
-        uint32_t s[2][32];
-        tmem_ld32(tS + b * 64, s[0]);
-        tmem_ld32(tS + b * 64 + 32, s[1]);
-        tmem_wait_ld();
-
-        const long long kidx0 = (long long)i * A_BH;
-        const bool ragged = kidx0 + A_BH > p.sk;
-        const bool diag = p.causal && (p.kv_pos0 + kidx0 + A_BH - 1 > w.qpos[t]);
-        if (ragged || diag) {
-          long long lim = p.sk - kidx0;
-          if (p.causal) {
-            const long long c = qpos - p.kv_pos0 - kidx0 + 1;
-            if (c < lim) lim = c;
-          }
-#pragma unroll
-          for (int c = 0; c < 2; ++c)
-#pragma unroll
-            for (int k = 0; k < 32; ++k)
-              if (c * 32 + k >= lim) s[c][k] = 0xff800000u;
-        }
-
-        float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-        for (int k = 0; k < 32; k += 4) {
-          mx0 = fmax3(mx0, __uint_as_float(s[0][k]), __uint_as_float(s[0][k + 1]));
-          mx1 = fmax3(mx1, __uint_as_float(s[0][k + 2]), __uint_as_float(s[0][k + 3]));
-          mx2 = fmax3(mx2, __uint_as_float(s[1][k]), __uint_as_float(s[1][k + 1]));
-          mx3 = fmax3(mx3, __uint_as_float(s[1][k + 2]), __uint_as_float(s[1][k + 3]));
-        }
-        const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * p.scale_log2;
-
-        float alpha = 1.f;
-        bool rescale = false;
-        if (i == 0) {
-          m_used = (mx == -INFINITY) ? 0.f : mx;
-        } else {
-          const bool grow = mx > m_used + 8.f;
-          rescale = __any_sync(0xffffffffu, grow);
-          if (rescale) {
-            const float m_new = fmaxf(m_used, mx);
-            alpha = ex2(m_used - m_new);
-            m_used = m_new;
-            l *= alpha;
-          }
-        }
-
-        const float neg_m = -m_used;
-        float l0 = 0.f, l1 = 0.f, l2 = 0.f, l3 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          uint32_t pk[16];
-          if (p.poly_exp)
-            softmax_exp_chunk<2>(s[c], p.scale_log2, neg_m, l0, l1, l2, l3, pk);
-          else
-            softmax_exp_chunk<0>(s[c], p.scale_log2, neg_m, l0, l1, l2, l3, pk);
-          tmem_st16(tS + b * 64 + c * 16, pk);
-        }
-        l += (l0 + l1) + (l2 + l3);
-        if (i > 0) {
-          // PV_t(i-1) has normally retired long ago (QK_t(i) was queued before it, a whole softmax step
-          // has passed).  Its phase is consumed here, every step and in order, so this thread can never
-          // fall two phases behind o_done; O_t is rescaled (lazily) only after it.
-          mbar_wait(&o_done[t], (pv_base + i - 1) & 1);
-          if (rescale) {
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < D / 32; ++c) {
-              uint32_t o[32];
-              tmem_ld32(tO + c * 32, o);
-              tmem_wait_ld();
-#pragma unroll
-              for (int k = 0; k < 32; ++k) o[k] = __float_as_uint(__uint_as_float(o[k]) * alpha);
-              tmem_st32(tO + c * 32, o);
-            }
-          }
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[t * 2 + b]);
-      }
-
-      // ---------------- epilogue ----------------
-      const float inv_l = (n > 0 && l > 0.f) ? 1.f / l : 0.f;
-      if (n > 0) {
-        mbar_wait(&o_done[t], (pv_base + n - 1) & 1);
-        pv_base += n;
-        tc_fence_after();
-      } else {
-        mbar_wait(&q_full[t], item_cnt & 1);
-      }
-#pragma unroll 1
-      for (int c = 0; c < D / 32; ++c) {
-        uint32_t o[32];
-        if (n > 0) {
-          tmem_ld32(tO + c * 32, o);
-          tmem_wait_ld();
-        } else {
-#pragma unroll
-          for (int k = 0; k < 32; ++k) o[k] = 0u;
-        }
-        uint8_t* box = stage + (c >> 1) * 16384 + row * 128;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          uint4 v;
-          v.x = pack_bf16(__uint_as_float(o[8 * q + 0]) * inv_l, __uint_as_float(o[8 * q + 1]) * inv_l);
-          v.y = pack_bf16(__uint_as_float(o[8 * q + 2]) * inv_l, __uint_as_float(o[8 * q + 3]) * inv_l);
-          v.z = pack_bf16(__uint_as_float(o[8 * q + 4]) * inv_l, __uint_as_float(o[8 * q + 5]) * inv_l);
-          v.w = pack_bf16(__uint_as_float(o[8 * q + 6]) * inv_l, __uint_as_float(o[8 * q + 7]) * inv_l);
-          const int chunk = (c & 1) * 4 + q;
-          *reinterpret_cast<uint4*>(box + ((chunk ^ (row & 7)) << 4)) = v;
-        }
-      }
-      tc_fence_before();
-      if (p.lse != nullptr && w.row0[t] + row < p.sq) {
-        const float lse = (n > 0 && l > 0.f) ? (m_used + log2f(l)) * 0.69314718055994530942f : -INFINITY;
-        p.lse[((long long)w.b * p.hq + w.h) * p.sq + w.row0[t] + row] = lse;
-      }
-      fence_proxy_async_smem();
-      named_bar_sync(1 + t, 128);
-      if (wg_tid == 0) {
-        if (w.row0[t] < p.sq) {
-          for (int bx = 0; bx < Cfg::BOXES; ++bx) tma_store_4d(&tmO, stage + bx * 16384, bx * 64, w.row0[t], w.h, w.b);
-          tma_store_commit();
-          tma_store_wait_read0();
-        }
-        mbar_arrive(&q_empty[t]);
-      }
-    }
-    if (wg_tid == 0) tma_store_wait_all0();
-  } else {
-    if (CP) cp_copier(cpp, warp, lane);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_base, 512);
-}
-
-template <int D, bool CP, int VER, int POLY = 0, bool TURNS = false, bool HALF = true>
-static int launch_attn_t(const lv_attn_params* a, const CpKParams* cp, cudaStream_t s) {
+static int launch_attn(const lv_attn_params* a, const CpKParams* cp, cudaStream_t s) {
   using Cfg = AttnCfg<D>;
   CUtensorMap tmQ, tmK, tmV, tmO;
   const uint32_t box[4] = {64, 128, 1, 1};
+  const uint32_t obox[4] = {64, 64, 1, 1};    // each consumer warpgroup stores its own 64 rows
   {
     const uint64_t dims[4] = {(uint64_t)D, (uint64_t)a->sq, (uint64_t)a->hq, (uint64_t)a->batch};
     const uint64_t str[4] = {2, (uint64_t)a->q_strides[1] * 2, (uint64_t)a->q_strides[2] * 2, (uint64_t)a->q_strides[0] * 2};
     int r = encode_tmap_bf16(&tmQ, a->q, 4, dims, str, box, true);
     if (r) return r;
     const uint64_t ostr[4] = {2, (uint64_t)a->o_strides[1] * 2, (uint64_t)a->o_strides[2] * 2, (uint64_t)a->o_strides[0] * 2};
-    r = encode_tmap_bf16(&tmO, a->out, 4, dims, ostr, box, true);
+    r = encode_tmap_bf16(&tmO, a->out, 4, dims, ostr, obox, true);
     if (r) return r;
   }
   {
@@ -1404,18 +667,16 @@ static int launch_attn_t(const lv_attn_params* a, const CpKParams* cp, cudaStrea
   p.q_seg_pos0 = a->q_seg_pos[0];
   p.q_seg_pos1 = a->q_seg_pos[1];
   p.kv_pos0 = a->kv_pos0;
-  p.n_qblk = (int)((a->sq + 255) / 256);
+  p.n_qblk = (int)((a->sq + A_BM - 1) / A_BM);
   p.n_items = (int)(a->batch * a->hq * p.n_qblk);
-  // all kv heads' K and V fit comfortably in the 126 MB L2 -> global longest-first order
-  p.block_major = (a->causal && a->sk * a->hkv * a->d * 4 <= (64ll << 20)) ? 1 : 0;
+  // all kv heads' K and V fit comfortably in the 50 MB L2 -> global longest-first order
+  p.block_major = (a->causal && a->sk * a->hkv * a->d * 4 <= (24ll << 20)) ? 1 : 0;
   static const int order_env = [] {   // LV_ATTN_ORDER=0 / 1 forces head-major / block-major order (A/B runs)
     const char* e = getenv("LV_ATTN_ORDER");
     return (e != nullptr && (e[0] == '0' || e[0] == '1')) ? (e[0] - '0') : -1;
   }();
   if (order_env >= 0 && a->causal) p.block_major = order_env;
   p.lse = a->lse;
-  p.poly_exp = attn_poly_exp();      // read by the v2 kernel only (v1: template parameter)
-  p.mufu_turns = TURNS ? 1 : 0;
   static const int serp = [] {
     const char* e = getenv("LV_ATTN_SCHED");
     return (e != nullptr && e[0] == '0') ? 0 : 1;
@@ -1424,11 +685,7 @@ static int launch_attn_t(const lv_attn_params* a, const CpKParams* cp, cudaStrea
   static PerDeviceOnce attr_once;   // one per template instantiation
   int attr_dev;
   if (attr_once.needed(&attr_dev)) {
-    if constexpr (VER == 2) {
-      LV_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd2_kernel<D, CP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_TOTAL));
-    } else {
-      LV_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, CP, POLY, TURNS, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_TOTAL));
-    }
+    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, CP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_TOTAL));
     attr_once.done(attr_dev);
   }
   int grid = p.n_items < sm_count() ? p.n_items : sm_count();
@@ -1438,61 +695,14 @@ static int launch_attn_t(const lv_attn_params* a, const CpKParams* cp, cudaStrea
     cpp = *cp;
     grid = sm_count();   // every copier warp takes part, also when there are fewer work items than SMs
   }
-  if constexpr (VER == 2)
-    attn_fwd2_kernel<D, CP><<<grid, A_THREADS, Cfg::SMEM_TOTAL, s>>>(tmQ, tmK, tmV, tmO, p, cpp);
-  else
-    attn_fwd_kernel<D, CP, POLY, TURNS, HALF><<<grid, A_THREADS, Cfg::SMEM_TOTAL, s>>>(tmQ, tmK, tmV, tmO, p, cpp);
+  attn_fwd_kernel<D, CP><<<grid, A_THREADS, Cfg::SMEM_TOTAL, s>>>(tmQ, tmK, tmV, tmO, p, cpp);
   LV_CHECK_LAUNCH("attn_fwd_kernel");
   return LV_OK;
-}
-
-// LV_ATTN_TURNS=1 switches the MUFU turn-taking of the softmax warps on (default off: with two warps per sub-partition
-// interleaving on the MUFU, 128K causal measured 1137 TFLOP/s without turns and 1076 with).  LV_ATTN_POLY=1: every
-// 4th exponential on the FMA pipe.
-static int attn_turns_env() {
-  static const int v = [] {
-    const char* e = getenv("LV_ATTN_TURNS");
-    return (e != nullptr && (e[0] == '0' || e[0] == '1')) ? (e[0] - '0') : -1;
-  }();
-  return v;
-}
-
-template <int D, bool CP, int VER>
-static int launch_attn(const lv_attn_params* a, const CpKParams* cp, cudaStream_t s) {
-  if constexpr (VER == 2) {
-    return launch_attn_t<D, CP, 2>(a, cp, s);
-  } else {
-    const bool turns = attn_turns_env() == 1;      // measured round 2: off is faster at both head dims (profiles/README.md)
-    const int poly = attn_poly_exp();              // pairs per 8 on the FMA pipe: LV_ATTN_POLY = 0 | 2 | 3 | 4
-    static const int half_env = [] {      // LV_ATTN_HALF=0: whole-tile P hand-off (A/B runs)
-      const char* e = getenv("LV_ATTN_HALF");
-      return (e != nullptr && e[0] == '0') ? 0 : 1;
-    }();
-    if constexpr (CP) {     // context-parallel launches: the default only (fewer instantiations of the big kernel)
-      return launch_attn_t<D, CP, 1, ATTN_POLY_DEFAULT, false, true>(a, cp, s);
-    } else {
-      if (turns) return launch_attn_t<D, CP, 1, ATTN_POLY_DEFAULT, true, false>(a, cp, s);
-      if (!half_env) return launch_attn_t<D, CP, 1, ATTN_POLY_DEFAULT, false, false>(a, cp, s);
-      if (poly == 0) return launch_attn_t<D, CP, 1, 0, false, true>(a, cp, s);
-      if (poly == 2) return launch_attn_t<D, CP, 1, 2, false, true>(a, cp, s);
-      if (poly == 3) return launch_attn_t<D, CP, 1, 3, false, true>(a, cp, s);
-      return launch_attn_t<D, CP, 1, 4, false, true>(a, cp, s);
-    }
-  }
 }
 
 }  // namespace lv
 
 using namespace lv;
-
-// LV_ATTN_VERSION: 1 = single-S-buffer kernel (default), 2 = double-buffered-S kernel (correct, slower).
-static int attn_version() {
-  static const int v = [] {
-    const char* e = getenv("LV_ATTN_VERSION");
-    return (e != nullptr && e[0] >= '1' && e[0] <= '2') ? (e[0] - '0') : 1;
-  }();
-  return v;
-}
 
 static int check_attn_params(const lv_attn_params* a) {
   LV_CHECK_ARG(a != nullptr, "lv_attn_fwd: null params");
@@ -1501,7 +711,7 @@ static int check_attn_params(const lv_attn_params* a) {
   LV_CHECK_ARG(a->batch > 0 && a->sq > 0 && a->sk > 0 && a->hq > 0 && a->hkv > 0, "lv_attn_fwd: empty shape");
   LV_CHECK_ARG(a->hq % a->hkv == 0, "lv_attn_fwd: hq=%lld is not a multiple of hkv=%lld", (long long)a->hq, (long long)a->hkv);
   LV_CHECK_ARG(a->sq < (1ll << 30) && a->sk < (1ll << 30), "lv_attn_fwd: sequence too long");
-  LV_CHECK_ARG(a->batch * a->hq * ((a->sq + 255) / 256) < (1ll << 31), "lv_attn_fwd: too many work items");
+  LV_CHECK_ARG(a->batch * a->hq * ((a->sq + 127) / 128) < (1ll << 31), "lv_attn_fwd: too many work items");
   LV_CHECK_ARG(a->q_seg_len > 0 && a->q_seg_len <= a->sq, "lv_attn_fwd: q_seg_len=%lld out of range", (long long)a->q_seg_len);
   if (a->q_seg_len < a->sq) {
     LV_CHECK_ARG(a->q_seg_len % 128 == 0 && a->sq <= 2 * a->q_seg_len, "lv_attn_fwd: segmented queries need q_seg_len %% 128 == 0 (a 128-row query tile never straddles segments) and at most two segments");
@@ -1517,14 +727,8 @@ extern "C" int lv_attn_fwd(const lv_attn_params* a, lv_stream_t stream) {
   if (rc) return rc;
   LV_BIND_DEVICE(a->q);
   cudaStream_t s = (cudaStream_t)stream;
-  // P is bf16 like V: tcgen05 kind::f16 faults on an fp16 A operand against a bf16 B operand
-  // (measured on B200), so the fp16-P instantiation is never launched.
-  if (attn_version() == 2) {
-    if (a->d == 128) return launch_attn<128, false, 2>(a, nullptr, s);
-    return launch_attn<64, false, 2>(a, nullptr, s);
-  }
-  if (a->d == 128) return launch_attn<128, false, 1>(a, nullptr, s);
-  return launch_attn<64, false, 1>(a, nullptr, s);
+  if (a->d == 128) return launch_attn<128, false>(a, nullptr, s);
+  return launch_attn<64, false>(a, nullptr, s);
 }
 
 extern "C" int lv_attn_cp_fwd(const lv_attn_params* a, const lv_cp_params* c, lv_stream_t stream) {
@@ -1591,8 +795,7 @@ extern "C" int lv_attn_cp_fwd(const lv_attn_params* a, const lv_cp_params* c, lv
     k.order |= first << (4 * (2 * i));
     k.order |= second << (4 * (2 * i + 1));
   }
-  if (attn_version() == 2) return launch_attn<128, true, 2>(a, &k, (cudaStream_t)stream);
-  return launch_attn<128, true, 1>(a, &k, (cudaStream_t)stream);
+  return launch_attn<128, true>(a, &k, (cudaStream_t)stream);
 }
 
 // Peer-mappable ("symmetric") allocations for the context-parallel K/V exchange: plain cudaMalloc

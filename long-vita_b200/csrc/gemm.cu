@@ -1,15 +1,13 @@
-// Dense linear layer on the 5th-generation tensor cores:  C[M,N] = act(A[M,K] . W[N,K]^T + bias)
+// Dense linear layer on the Hopper tensor cores:  C[M,N] = act(A[M,K] . W[N,K]^T + bias)
 //
-// Persistent, warp-specialised sm_100a kernel (one CTA per SM):
-//   warp 0     TMA producer: 128x64 A tiles and 256x64 W tiles (128-byte swizzle) into a 4-stage
-//              shared-memory ring, completion on mbarriers
-//   warp 1     tcgen05.mma issuer (single elected thread): UMMA 128x256x16, bf16 x bf16 -> fp32,
-//              accumulators in TMEM, double-buffered (2 x 256 columns) so the epilogue of tile i
-//              overlaps the main loop of tile i+1
-//   warps 2-5  epilogue: tcgen05.ld TMEM -> registers, + bias, activation, bf16 pack, swizzled
-//              st.shared, TMA store (clips the M / N tails)
-// Tiles are rasterised in groups of 16 M-blocks so the concurrently resident tiles share A and W
-// panels in L2.
+// Persistent, warp-specialised sm_90a kernel (one CTA per SM, 3 warpgroups):
+//   warpgroup 0     TMA producer (one thread): 128x64 A tiles and 256x64 W tiles (128-byte swizzle) into a
+//                   4-stage shared-memory ring, completion on mbarriers
+//   warpgroups 1-2  consumers: each owns 64 rows of the 128x256 tile, wgmma m64n256k16 (bf16 x bf16 -> fp32,
+//                   accumulators in registers) with one k-block of MMAs in flight; then the epilogue - bias,
+//                   activation, bf16 pack, swizzled st.shared, TMA store (clips the M / N tails) - while the
+//                   producer already fills the ring for the next tile
+// Tiles are rasterised in groups of M-blocks so the concurrently resident tiles share A and W panels in L2.
 //
 // Replaces torch.matmul / te.Linear at long_vita_megatron/core/tensor_parallel/layers.py:270,409 and
 // the nn.Linear calls of modeling_intern_vit.py:131,141,190-191 / resampler_projector.py:19-23.
@@ -22,19 +20,12 @@
 
 namespace lv {
 
-constexpr int G_BM = 128, G_BK = 64, G_STAGES = 4;
+constexpr int G_BM = 128, G_BN = 256, G_BK = 64, G_STAGES = 4;
 constexpr int G_A_BYTES = G_BM * G_BK * 2;          // 16 KB
-constexpr int G_C_BYTES = G_BM * 64 * 2;            // 16 KB staging per 64-column chunk
-constexpr int G_THREADS = 192;
-// The N-tile width is a template parameter: 256 (UMMA 128x256x16, the default: least shared-memory traffic per flop)
-// or 128.  With few M-blocks - a context-parallel rank holds S / cp tokens - 128 x 256 tiles can leave the last wave
-// of the persistent grid mostly empty (M = 2304, N = 5120: 360 tiles on 148 SMs = 2.43 waves); 128 x 128 tiles
-// quantise finer (720 tiles = 4.86 waves).  launch_gemm picks the width with the better wave efficiency.
-template <int BN>
-struct GemmCfg {
-  static constexpr int B_BYTES = BN * G_BK * 2;     // 32 KB / 16 KB
-  static constexpr int SMEM = G_STAGES * (G_A_BYTES + B_BYTES) + 2 * G_C_BYTES + 256 + 1024;  // + barriers + align slack
-};
+constexpr int G_B_BYTES = G_BN * G_BK * 2;          // 32 KB
+constexpr int G_C_BYTES = 64 * 64 * 2;              // 8 KB staging per 64 x 64 output chunk (two per consumer)
+constexpr int G_THREADS = 384;
+constexpr int G_SMEM = G_STAGES * (G_A_BYTES + G_B_BYTES) + 4 * G_C_BYTES + 256 + 1024;  // + barriers + align slack
 
 __device__ __forceinline__ float act_apply(float t, int act) {
   if (act == 1) return 0.5f * t * (1.f + erff(t * 0.70710678118654752440f));
@@ -55,26 +46,20 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
   nb = r / gsz;
 }
 
-template <int G_BN>
 __global__ void __launch_bounds__(G_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmC, const __nv_bfloat16* __restrict__ bias, int M, int N,
                      int K, int act, int gm) {
-  constexpr int G_B_BYTES = GemmCfg<G_BN>::B_BYTES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + G_STAGES * G_A_BYTES;
   uint8_t* sC = sB + G_STAGES * G_B_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sC + 2 * G_C_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sC + 4 * G_C_BYTES);
   uint64_t* full = bars;                  // [G_STAGES]
-  uint64_t* empty = bars + G_STAGES;      // [G_STAGES]
-  uint64_t* acc_full = bars + 2 * G_STAGES;       // [2]
-  uint64_t* acc_empty = bars + 2 * G_STAGES + 2;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * G_STAGES + 4);
+  uint64_t* empty = bars + G_STAGES;      // [G_STAGES]: one arrival per consumer warpgroup
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int num_m = (M + G_BM - 1) / G_BM, num_n = (N + G_BN - 1) / G_BN;
   const int num_tiles = num_m * num_n;
   const int num_kb = (K + G_BK - 1) / G_BK;
@@ -85,26 +70,16 @@ __global__ void __launch_bounds__(G_THREADS, 1)
     tma_prefetch_desc(&tmC);
     for (int i = 0; i < G_STAGES; ++i) {
       mbar_init(&full[i], 1);
-      mbar_init(&empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&acc_full[i], 1);
-      mbar_init(&acc_empty[i], 4);
+      mbar_init(&empty[i], 2);
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------- TMA producer -------------------------------
-    if (lane == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -122,186 +97,120 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer ---------------------------------
-    // warp-uniform control flow, one elected lane issues: descriptors stay in uniform registers
-    {
-      constexpr uint32_t idesc = make_idesc_bf16(G_BM, G_BN, 0, 0);
-      const uint64_t adesc0 = make_smem_desc(smem_u32(sA), 16, 1024);
-      const uint64_t bdesc0 = make_smem_desc(smem_u32(sB), 16, 1024);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        mbar_wait(&acc_empty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * G_BN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = adesc0 + (uint64_t)((stage * G_A_BYTES) >> 4);
-          const uint64_t bdesc = bdesc0 + (uint64_t)((stage * G_B_BYTES) >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < G_BK / 16; ++kk)
-              umma_ss(d_tmem, adesc + 2 * kk, bdesc + 2 * kk, idesc, (kb | kk) != 0 ? 1u : 0u);
-            umma_commit(&empty[stage]);  // smem slot reusable once these MMAs have read it
-          }
-          __syncwarp();
-          if (++stage == G_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (elect_one()) umma_commit(&acc_full[as]);
-        __syncwarp();
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-    }
   } else {
-    // ------------------------------- epilogue -----------------------------------
-    const int quad = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int row = quad * 32 + lane;          // row of the 128-row tile
-    const int epi_tid = (warp - 2) * 32 + lane;
-    int as = 0;
-    uint32_t aphase = 0;
+    // ------------------------------- consumers ----------------------------------
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;                          // 64-row half of the tile
+    const int wg_tid = threadIdx.x & 127;
+    const int warp = wg_tid >> 5, lane = wg_tid & 31;
+    const int r_lo = warp * 16 + (lane >> 2);       // accumulator rows r_lo and r_lo + 8 (of 64)
+    const int cq = 2 * (lane & 3);                  // first of the two columns of each 8-column group
+    uint8_t* stg_base = sC + cw * 2 * G_C_BYTES;
+    const uint64_t adesc0 = make_smem_desc(smem_u32(sA) + cw * 8192, 16, 1024);
+    const uint64_t bdesc0 = make_smem_desc(smem_u32(sB), 16, 1024);
+    int stage = 0;
+    uint32_t phase = 0;
     uint32_t chunk_counter = 0;
+    float acc[128];
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int mb, nb;
       tile_coords(tile, num_m, num_n, gm, mb, nb);
-      mbar_wait(&acc_full[as], aphase);
-      tc_fence_after();
-      if (act == 3) {
-        // Fused SwiGLU: W rows are interleaved (gate_i, up_i), so accumulator columns (2i, 2i+1) hold
-        // gate_i and up_i; out[:, i] = bf16(silu(bf16 gate)) * bf16(up) - the exact rounding sequence of
-        // the un-fused GEMM + lv_swiglu pair - and the stored tile is 128 columns wide.
-#pragma unroll 1
-        for (int cc = 0; cc < G_BN / 128; ++cc) {
-          uint32_t packed[32];
+      int prev_stage = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        const uint64_t adesc = adesc0 + (uint64_t)((stage * G_A_BYTES) >> 4);
+        const uint64_t bdesc = bdesc0 + (uint64_t)((stage * G_B_BYTES) >> 4);
 #pragma unroll
-          for (int hlf = 0; hlf < 2; ++hlf) {
-            uint32_t r0[32], r1[32];
-            const uint32_t taddr = tmem_base + (uint32_t(quad * 32) << 16) + as * G_BN + cc * 128 + hlf * 64;
-            tmem_ld32(taddr, r0);
-            tmem_ld32(taddr + 32, r1);
-            tmem_wait_ld();
-            if (cc == G_BN / 128 - 1 && hlf == 1) {
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(&acc_empty[as]);
-            }
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              float o[4];
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const float g0 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(r0[j + 2 * e])));
-                const float u0 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(r0[j + 2 * e + 1])));
-                const float g1 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(r1[j + 2 * e])));
-                const float u1 = __bfloat162float(__float2bfloat16_rn(__uint_as_float(r1[j + 2 * e + 1])));
-                o[e] = __bfloat162float(__float2bfloat16_rn(__fdividef(g0, 1.f + __expf(-g0)))) * u0;
-                o[2 + e] = __bfloat162float(__float2bfloat16_rn(__fdividef(g1, 1.f + __expf(-g1)))) * u1;
-              }
-              packed[hlf * 16 + j / 4] = pack_bf16(o[0], o[1]);          // out cols hlf*32 + j/2 .. +1
-              packed[hlf * 16 + 8 + j / 4] = pack_bf16(o[2], o[3]);      // out cols hlf*32 + 16 + j/2 .. +1
-            }
-          }
-          uint8_t* stg = sC + (chunk_counter & 1) * G_C_BYTES;
-          if (epi_tid == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-          named_bar_sync(1, 128);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const uint32_t off = row * 128 + ((j ^ (row & 7)) << 4);
-            *reinterpret_cast<uint4*>(stg + off) =
-                make_uint4(packed[4 * j], packed[4 * j + 1], packed[4 * j + 2], packed[4 * j + 3]);
-          }
-          fence_proxy_async_smem();
-          named_bar_sync(2, 128);
-          if (epi_tid == 0) {
-            tma_store_2d(&tmC, stg, nb * (G_BN / 2) + cc * 64, mb * G_BM);
-            tma_store_commit();
-          }
-          ++chunk_counter;
+        for (int kk = 0; kk < G_BK / 16; ++kk) wgmma_ss_n256(acc, adesc + 2 * kk, bdesc + 2 * kk, (kb | kk) != 0 ? 1u : 0u);
+        wgmma_commit();
+        // the k-block before this one has retired: its ring slot may be refilled
+        wgmma_wait<1>();
+        wgmma_keep(acc);
+        if (prev_stage >= 0 && wg_tid == 0) mbar_arrive(&empty[prev_stage]);
+        prev_stage = stage;
+        if (++stage == G_STAGES) {
+          stage = 0;
+          phase ^= 1;
         }
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1;
-        }
-        continue;
       }
-#pragma unroll 1
-      for (int c = 0; c < G_BN / 64; ++c) {
-        uint32_t r0[32], r1[32];
-        const uint32_t taddr = tmem_base + (uint32_t(quad * 32) << 16) + as * G_BN + c * 64;
-        tmem_ld32(taddr, r0);
-        tmem_ld32(taddr + 32, r1);
-        tmem_wait_ld();
-        if (c == G_BN / 64 - 1) {
-          // all TMEM reads of this accumulator are done: hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_empty[as]);
-        }
-        const int n0 = nb * G_BN + c * 64;
-        uint32_t packed[32];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          float v0 = __uint_as_float(r0[j]), v1 = __uint_as_float(r0[j + 1]);
-          float w0 = __uint_as_float(r1[j]), w1 = __uint_as_float(r1[j + 1]);
-          if (bias != nullptr) {
-            const int ca = n0 + j, cb = n0 + 32 + j;
-            const float b0 = ca < N ? __bfloat162float(bias[ca]) : 0.f;
-            const float b1 = ca + 1 < N ? __bfloat162float(bias[ca + 1]) : 0.f;
-            const float b2 = cb < N ? __bfloat162float(bias[cb]) : 0.f;
-            const float b3 = cb + 1 < N ? __bfloat162float(bias[cb + 1]) : 0.f;
-            v0 += b0;
-            v1 += b1;
-            w0 += b2;
-            w1 += b3;
-          }
-          if (act != 0) {
-            // nn.Linear rounds its output to bf16 before the activation module sees it
-            v0 = act_apply(__bfloat162float(__float2bfloat16_rn(v0)), act);
-            v1 = act_apply(__bfloat162float(__float2bfloat16_rn(v1)), act);
-            w0 = act_apply(__bfloat162float(__float2bfloat16_rn(w0)), act);
-            w1 = act_apply(__bfloat162float(__float2bfloat16_rn(w1)), act);
-          }
-          packed[j / 2] = pack_bf16(v0, v1);
-          packed[16 + j / 2] = pack_bf16(w0, w1);
-        }
-        uint8_t* stg = sC + (chunk_counter & 1) * G_C_BYTES;
+      wgmma_wait<0>();
+      wgmma_keep(acc);
+      if (wg_tid == 0) mbar_arrive(&empty[prev_stage]);
+
+      // ------------------------------- epilogue -----------------------------------
+      // Output chunks of 64 x 64: staged (128-byte swizzle, the layout of the TMA map) and stored with TMA.  The
+      // chunk loops are unrolled so that every accumulator index is a compile-time constant (registers, not stack).
+      auto stage_begin = [&]() -> uint8_t* {
+        uint8_t* stg = stg_base + (chunk_counter & 1) * G_C_BYTES;
         // the TMA store that last read this staging buffer (two chunks ago) must have drained
-        if (epi_tid == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-        named_bar_sync(1, 128);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const uint32_t off = row * 128 + ((j ^ (row & 7)) << 4);
-          *reinterpret_cast<uint4*>(stg + off) =
-              make_uint4(packed[4 * j], packed[4 * j + 1], packed[4 * j + 2], packed[4 * j + 3]);
-        }
+        if (wg_tid == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
+        named_bar_sync(1 + cw, 128);
+        return stg;
+      };
+      auto stage_end = [&](uint8_t* stg, int col0) {
         fence_proxy_async_smem();
-        named_bar_sync(2, 128);
-        if (epi_tid == 0) {
-          tma_store_2d(&tmC, stg, n0, mb * G_BM);
+        named_bar_sync(1 + cw, 128);
+        if (wg_tid == 0) {
+          tma_store_2d(&tmC, stg, col0, mb * G_BM + cw * 64);
           tma_store_commit();
         }
         ++chunk_counter;
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
+      };
+      if (act == 3) {
+        // Fused SwiGLU: W rows are interleaved (gate_i, up_i), so accumulator columns (2i, 2i+1) - held by the same
+        // thread - are gate_i and up_i; out[:, i] = bf16(silu(bf16 gate)) * bf16(up), the exact rounding sequence of
+        // the un-fused GEMM + lv_swiglu pair.  Output chunk c covers 8-column groups 16c .. 16c + 15.
+#pragma unroll
+        for (int c = 0; c < G_BN / 128; ++c) {
+          uint8_t* stg = stage_begin();
+#pragma unroll
+          for (int jj = 0; jj < 16; ++jj) {
+            const int j = c * 16 + jj;
+            const int oc = 4 * jj + (lane & 3);           // output column inside the chunk
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float g = __bfloat162float(__float2bfloat16_rn(acc[4 * j + 2 * h]));
+              const float u = __bfloat162float(__float2bfloat16_rn(acc[4 * j + 2 * h + 1]));
+              const float o = __bfloat162float(__float2bfloat16_rn(__fdividef(g, 1.f + __expf(-g)))) * u;
+              const int row = r_lo + 8 * h;
+              *reinterpret_cast<__nv_bfloat16*>(stg + row * 128 + (((oc >> 3) ^ (row & 7)) << 4) + (oc & 7) * 2) =
+                  __float2bfloat16_rn(o);
+            }
+          }
+          stage_end(stg, nb * (G_BN / 2) + c * 64);
+        }
+      } else {
+#pragma unroll
+        for (int c = 0; c < G_BN / 64; ++c) {
+          uint8_t* stg = stage_begin();
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = c * 8 + jj;
+            const int col = nb * G_BN + 8 * j + cq;
+            float b0 = 0.f, b1 = 0.f;
+            if (bias != nullptr) {
+              b0 = col < N ? __bfloat162float(bias[col]) : 0.f;
+              b1 = col + 1 < N ? __bfloat162float(bias[col + 1]) : 0.f;
+            }
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float v0 = acc[4 * j + 2 * h] + b0, v1 = acc[4 * j + 2 * h + 1] + b1;
+              if (act != 0) {
+                // nn.Linear rounds its output to bf16 before the activation module sees it
+                v0 = act_apply(__bfloat162float(__float2bfloat16_rn(v0)), act);
+                v1 = act_apply(__bfloat162float(__float2bfloat16_rn(v1)), act);
+              }
+              const int row = r_lo + 8 * h;
+              *reinterpret_cast<uint32_t*>(stg + row * 128 + ((jj ^ (row & 7)) << 4) + cq * 2) = pack_bf16(v0, v1);
+            }
+          }
+          stage_end(stg, nb * G_BN + c * 64);
+        }
       }
     }
-    if (epi_tid == 0) tma_store_wait_all0();
+    if (wg_tid == 0) tma_store_wait_all0();
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -468,10 +377,8 @@ static int launch_gemv(const void* A, const void* W, const void* bias, void* C, 
   return LV_OK;
 }
 
-template <int G_BN>
-static int launch_gemm_t(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K,
-                         int64_t lda, int64_t ldw, int64_t ldc, int act, cudaStream_t s) {
-  constexpr int G_SMEM = GemmCfg<G_BN>::SMEM;
+static int launch_gemm(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K,
+                       int64_t lda, int64_t ldw, int64_t ldc, int act, cudaStream_t s) {
   CUtensorMap tmA, tmB, tmC;
   {
     const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
@@ -490,67 +397,27 @@ static int launch_gemm_t(const void* A, const void* W, const void* bias, void* C
   {
     const uint64_t dims[2] = {(uint64_t)(act == 3 ? N / 2 : N), (uint64_t)M};
     const uint64_t str[2] = {2, (uint64_t)ldc * 2};
-    const uint32_t box[2] = {64, G_BM};
+    const uint32_t box[2] = {64, 64};
     int r = encode_tmap_bf16(&tmC, C, 2, dims, str, box, true);
     if (r) return r;
   }
   static PerDeviceOnce attr_once;
   int attr_dev;
   if (attr_once.needed(&attr_dev)) {
-    LV_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<G_BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
+    LV_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
     attr_once.done(attr_dev);
   }
   const int64_t tiles = ((M + G_BM - 1) / G_BM) * ((N + G_BN - 1) / G_BN);
   const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
   // M-blocks per rasterisation group: the A panel of a group (gm x 128 rows x K) stays in L2 while its tiles sweep
-  // the N-blocks, and W is re-read from HBM once per group, so DRAM traffic ~ A + C + (num_m / gm) * W.  Round 2 ncu
-  // inside the bench step, gm = 16: QKV 1107 MB vs 526 MB algorithmic, gate|up 3248 vs 982, down (K = 13824: a 57 MB
-  // panel, A is re-read too) 3096 vs 840.  The group is sized so that the A panel takes ~40 MB of the 126 MB L2 but
-  // never below 16 M-blocks (K = 5120 -> 30: gate|up 3248 -> 2271 MB; K = 13824 -> 16: a group of 11 measured 3462 MB,
-  // worse than 16 - fewer M-blocks per group also means more W passes); LV_GEMM_GM forces a value for A/B runs.
-  static const int gm_env = [] {
-    const char* e = getenv("LV_GEMM_GM");
-    const int v = e ? atoi(e) : 0;
-    return (v >= 1 && v <= 256) ? v : 0;
-  }();
-  int gm = gm_env;
-  if (gm == 0) {
-    gm = (int)((40ll << 20) / (256 * K));
-    gm = gm < 16 ? 16 : (gm > 64 ? 64 : gm);
-  }
-  gemm_bf16_kernel<G_BN><<<grid, G_THREADS, G_SMEM, s>>>(tmA, tmB, tmC, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M,
-                                                         (int)N, (int)K, act, gm);
+  // the N-blocks, and W is re-read from HBM once per group, so DRAM traffic ~ A + C + (num_m / gm) * W.  The group is
+  // sized so that the A panel takes ~16 MB of the 50 MB L2, but never fewer than 8 M-blocks.
+  int gm = (int)((16ll << 20) / (256 * K));
+  gm = gm < 8 ? 8 : (gm > 64 ? 64 : gm);
+  gemm_bf16_kernel<<<grid, G_THREADS, G_SMEM, s>>>(tmA, tmB, tmC, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M,
+                                                   (int)N, (int)K, act, gm);
   LV_CHECK_LAUNCH("gemm_bf16_kernel");
   return LV_OK;
-}
-
-// Fraction of the persistent grid's tile slots that do work: tiles / (waves * SMs).
-static double wave_efficiency(int64_t tiles, int sms) {
-  const int64_t waves = (tiles + sms - 1) / sms;
-  return (double)tiles / (double)(waves * sms);
-}
-
-static int launch_gemm(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K,
-                       int64_t lda, int64_t ldw, int64_t ldc, int act, cudaStream_t s) {
-  // LV_GEMM_BN=128 / 256 forces the N-tile width (A/B runs).  Measured round 2 (tools/bench_kernels.py, M = 2304):
-  // 128-wide tiles run at ~0.75x the per-tile rate of 256-wide ones (UMMA 128x128x16 reads 8 KB of shared memory per
-  // 64 cycles - the full 128 B/clk - while TMA refills the ring), which costs more than the fuller last wave gains
-  // (O-proj 825 vs 1102 TFLOP/s), so 256 stays the default everywhere; LV_GEMM_BN=auto applies the wave heuristic.
-  static const int bn_env = [] {
-    const char* e = getenv("LV_GEMM_BN");
-    if (e != nullptr && e[0] == 'a') return 0;
-    const int v = e ? atoi(e) : 256;
-    return (v == 128 || v == 256) ? v : 256;
-  }();
-  int bn = bn_env;
-  if (bn == 0) {
-    const int64_t mb = (M + G_BM - 1) / G_BM;
-    const double e256 = wave_efficiency(mb * ((N + 255) / 256), sm_count());
-    const double e128 = wave_efficiency(mb * ((N + 127) / 128), sm_count());
-    bn = (e128 > 1.08 * e256) ? 128 : 256;
-  }
-  if (bn == 128) return launch_gemm_t<128>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
-  return launch_gemm_t<256>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
 }
 
 }  // namespace lv
@@ -572,8 +439,8 @@ int lv_gemm_bias_act(const void* A, const void* W, const void* bias, void* C, in
   if (M == 0) return LV_OK;
   LV_BIND_DEVICE(A);
   // Weight-stream GEMV for decode-sized M - unless the tensor-core kernel already has a tile for every SM (the LM head:
-  // 594 N-tiles; measured 0.275 ms = 87 % of HBM there against 0.341 ms for the GEMV, round 2)
-  if (M <= 4 && gemv_enabled() && (N + 255) / 256 < sm_count() && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
+  // 594 N-tiles)
+  if (M <= 4 && gemv_enabled() && (N + G_BN - 1) / G_BN < sm_count() && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(W) & 15) == 0)
     return launch_gemv(A, W, bias, C, M, N, K, lda, ldw, ldc, act, (cudaStream_t)stream);
   return launch_gemm(A, W, bias, C, M, N, K, lda, ldw, ldc, act, (cudaStream_t)stream);

@@ -1,4 +1,4 @@
-"""B200-native Long-VITA forward with the reference's HF `forward()` surface.
+"""H100-native Long-VITA forward with the reference's HF `forward()` surface.
 
 `LongVITAModel.forward` / `LongVITAForCausalLM.forward` keep the argument list of
 long_vita/models/long_vita_qwen2_intern/modeling_long_vita.py:74-89 and :238-255, and the

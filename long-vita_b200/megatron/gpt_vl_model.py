@@ -1,4 +1,4 @@
-"""`GPTVLModel.forward` on the B200 kernels (SURVEY.md 8a-15) - Megatron-free.
+"""`GPTVLModel.forward` on the H100 kernels (SURVEY.md 8a-15) - Megatron-free.
 
 Mirrors long_vita_megatron/core/models/multimodal/gpt_vl_model.py:233-416: same argument list, same
 `external_inputs` conventions, same embedding merge modes
@@ -43,7 +43,7 @@ class B200GPTVLModel:
                  post_process: bool = True, cp=None, is_instruction_dataset: bool = False,
                  output_multiplier_scale: Optional[float] = None, output_logit_softcapping: Optional[float] = None):
         if not (pre_process and post_process):
-            raise NotImplementedError("pipeline parallelism is not built (14B bf16 fits one B200: pp = 1)")
+            raise NotImplementedError("pipeline parallelism is not built (14B bf16 fits one 80 GB H100: pp = 1)")
         self.config = cfg
         self.pre_process, self.post_process = pre_process, post_process
         self.cp = cp

@@ -79,7 +79,7 @@ class B200TransformerLayer(torch.nn.Module):
         self._rope_cache = (None, None, None)
         if int(getattr(config, "tensor_model_parallel_size", 1) or 1) > 1:
             raise NotImplementedError("B200TransformerLayer holds whole weights: tensor_model_parallel_size must be 1 "
-                                      "(14B bf16 fits one B200; the BASELINE configs are CP x DP)")
+                                      "(14B bf16 fits one 80 GB H100; the BASELINE configs are CP x DP)")
         self.cp_size = int(getattr(config, "context_parallel_size", 1) or 1)
         self._cp_ctx = None
         self.cp_group = getattr(config, "cp_group", None)   # tests / Megatron-free callers may hand the group in
@@ -173,7 +173,7 @@ class B200TransformerLayer(torch.nn.Module):
     # -- training: the same layer out of differentiable pieces (ops.*_autograd) --------------------------------
     def _forward_train(self, hidden_states, rotary_pos_emb):
         """Forward that records an autograd graph: every operator is a torch.autograd.Function over the C-ABI kernels
-        (RMSNorm / SwiGLU / RoPE backward kernels, `lv_attn_bwd`, and the tcgen05 GEMM for dX and dW).  It works on the
+        (RMSNorm / SwiGLU / RoPE backward kernels, `lv_attn_bwd`, and the wgmma GEMM for dX and dW).  It works on the
         Megatron parameter layouts directly (grouped QKV rows, fc1 = cat(gate, up)), so gradients land on the
         parameters Megatron's optimizer owns; the fused-epilogue / in-place shortcuts of the inference path are not
         used here (the un-fused gate|up activation is what the SwiGLU backward needs)."""

@@ -212,7 +212,7 @@ def attention(q, k, v, *, causal: bool, scale: Optional[float] = None):
 
 
 def _sm_count(device) -> int:
-    return torch.cuda.get_device_properties(device).multi_processor_count if torch.cuda.is_available() else 148
+    return torch.cuda.get_device_properties(device).multi_processor_count if torch.cuda.is_available() else 132
 
 
 def attention_decode(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, length: int, *,
@@ -515,7 +515,7 @@ def masked_linear_dgrad(grad_out: torch.Tensor, weight: torch.Tensor, logit_mask
 
 def masked_linear_wgrad(grad_out: torch.Tensor, h: torch.Tensor, logit_mask: torch.Tensor):
     """dW of masked_linear: dY^T . masked_select(h) -> [vocab, c] (layers.py:451-456, 512-520: `grad_output.t()
-    .matmul(total_input)`).  Runs on the same tcgen05 GEMM with the contraction over the M selected rows: both
+    .matmul(total_input)`).  Runs on the same wgmma GEMM with the contraction over the M selected rows: both
     operands are transposed once ([vocab, M] and [c, M]; M is the number of answer tokens) and M is zero-padded
     to a multiple of 8 (the GEMM's K granularity)."""
     _need_cuda_bf16(grad_out, h)
@@ -619,7 +619,7 @@ def lm_head_ce_fwd(sel: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor
 def lm_head_ce_bwd(sel: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor, lse: torch.Tensor, dloss: torch.Tensor,
                    need_dsel: bool = True, need_dw: bool = False, vocab_chunk: int = 16384):
     """Backward of lm_head_ce_fwd, chunk by chunk: the chunk's logits are recomputed (one GEMM), turned into
-    d_logits = (softmax - onehot) * dloss in place (`lv_ce_grad`), and contracted by the same tcgen05 GEMM:
+    d_logits = (softmax - onehot) * dloss in place (`lv_ce_grad`), and contracted by the same wgmma GEMM:
     d_sel += d_logits @ W[chunk] (fp32 accumulation across chunks), dW[chunk] = d_logits^T @ sel
     (layers.py:443-456, 512-520).  Returns (d_sel [M, c] bf16 or None, dW [vocab, c] bf16 or None)."""
     M, c = sel.shape
@@ -774,7 +774,7 @@ def rope_autograd(x, cos, sin):
 
 
 class _LinearFn(torch.autograd.Function):
-    """y = x W^T + b on the tcgen05 GEMM; dX = dY W and dW = dY^T X reuse the same kernel on operands transposed once
+    """y = x W^T + b on the wgmma GEMM; dX = dY W and dW = dY^T X reuse the same kernel on operands transposed once
     per call (the [N, K] operand of each product must be K-contiguous); the token count is zero-padded to a multiple
     of 8 for the weight gradient (the GEMM's K granularity)."""
 

@@ -14,6 +14,7 @@ from long_vita_b200 import cp as CP
 from long_vita_b200.config import LongVITAConfig
 from long_vita_b200.synthetic import build_prompt
 from oracle import ops as O
+from oracle import ref_loader
 
 
 def _prompt(n_frames=6, cp=4):
@@ -124,7 +125,15 @@ def test_shard_prompt_equals_the_references_own_get_batch_on_this_cp_rank():
     assert torch.equal(O.index_of_a_in_b(a, b), want)
 
 
-def _sync_worker(rank, world, port):
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+
+
+def _sync_local(sh):
+    """Per-token "logits" [b, s_local, 3] of one rank's shard, as forward_step hands them to sync_output."""
+    return torch.stack([sh.input_ids[0].float(), sh.position_ids.float(), sh.position_ids.float() * 2], dim=-1).unsqueeze(0)
+
+
+def _sync_worker(rank, world, port, out_path=None):
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
@@ -134,8 +143,7 @@ def _sync_worker(rank, world, port):
         S = ids.shape[1]
         sh = CP.shard_prompt(ids, idx, world, rank, 256)
         gen = ref_loader.load_megatron_generation(world, rank, dist.group.WORLD)
-        # per-token "logits" [b, s_local, 3] of this rank's shard, as forward_step hands them to sync_output
-        local = torch.stack([sh.input_ids[0].float(), sh.position_ids.float(), sh.position_ids.float() * 2], dim=-1).unsqueeze(0)
+        local = _sync_local(sh)
         full = gen.sync_output(local)
         assert full.shape == (1, S, 3)
         assert torch.equal(full[0, :, 1], torch.arange(S).float())                  # global order restored
@@ -144,19 +152,40 @@ def _sync_worker(rank, world, port):
         gathered = [torch.empty_like(local) for _ in range(world)]
         dist.all_gather(gathered, local)
         assert torch.equal(torch.cat(gathered, dim=1)[:, CP.zigzag_unpermute_index(S, world)], full)
+        if out_path is not None and rank == 0:
+            torch.save({"world": world, "n_frames": 5, "full": full.clone()}, out_path)
     finally:
         dist.destroy_process_group()
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="/root/reference not mounted (GPU box)")
-def test_references_own_sync_output_restores_global_order_from_our_shards():
-    """Live, 2 ranks over gloo: the reference's inference-side gather (generation.py:542-566, executed from
-    /root/reference) applied to the shards cp.shard_prompt produced returns the sequence in global order, and
-    equals cp.zigzag_unpermute_index on the concatenated shards."""
+def reference_sync_output(world, out_path):
+    """Runs the reference's sync_output on `world` gloo ranks (asserting the live checks) and stores rank 0's result."""
     with socket.socket() as s:
         s.bind(("127.0.0.1", 0))
         port = s.getsockname()[1]
-    mp.spawn(_sync_worker, args=(2, port), nprocs=2, join=True)
+    mp.spawn(_sync_worker, args=(world, port, out_path), nprocs=world, join=True)
+
+
+def test_shards_concatenate_to_the_references_own_sync_output_golden():
+    """tests/golden/ref_sync_output.pt: what the reference's inference-side gather (generation.py:542-566) returned for
+    the shards cp.shard_prompt produced on 2 ranks (recorded by tests/golden/make_golden.py).  The concatenated shards,
+    put back in order by cp.zigzag_unpermute_index, must equal it."""
+    gold = torch.load(os.path.join(GOLD, "ref_sync_output.pt"))
+    world = gold["world"]
+    cfg, ids, idx = _prompt(gold["n_frames"], world)
+    S = ids.shape[1]
+    cat = torch.cat([_sync_local(CP.shard_prompt(ids, idx, world, r, 256)) for r in range(world)], dim=1)
+    assert torch.equal(cat[:, CP.zigzag_unpermute_index(S, world)], gold["full"])
+
+
+@pytest.mark.skipif(not ref_loader.available(), reason="the reference checkout is not available")
+def test_references_own_sync_output_restores_global_order_from_our_shards(tmp_path):
+    """Live, 2 ranks over gloo: the reference's inference-side gather (generation.py:542-566, executed from the
+    reference checkout) applied to the shards cp.shard_prompt produced returns the sequence in global order, and
+    equals cp.zigzag_unpermute_index on the concatenated shards.  The recorded fixture must agree."""
+    reference_sync_output(2, str(tmp_path / "sync.pt"))
+    live = torch.load(str(tmp_path / "sync.pt"))
+    assert torch.equal(live["full"], torch.load(os.path.join(GOLD, "ref_sync_output.pt"))["full"])
 
 
 # ---- key-tile visiting order of the fused exchange kernel (csrc/attn_fwd.cu: KvWalk, cp_copier) ----
@@ -169,13 +198,11 @@ def _order_list(cp, rank, ring):
     return out
 
 
-def _walk(n0, n1, order, tc):
-    """KvWalk: the tiles [0, lo) both query tiles see first, then [lo, hi), each range in chunk-priority order."""
-    lo, hi = min(n0, n1), max(n0, n1)
+def _walk(n, order, tc):
+    """KvWalk: the tiles [0, n) a query tile sees, in chunk-priority order."""
     seq = []
-    for a, b in ((0, lo), (lo, hi)):
-        for ch in order:
-            seq += list(range(max(a, ch * tc), min(b, (ch + 1) * tc)))
+    for ch in order:
+        seq += list(range(ch * tc, min(n, (ch + 1) * tc)))
     return seq
 
 
@@ -195,8 +222,7 @@ def _copier_blocks(nb, order, tc):
 
 def test_visiting_order_model_of_the_exchange_kernel():
     """A restatement of the kernel's index logic (not the kernel - its parity is tests/test_gpu_cp.py): every key tile a
-    query tile may see is visited exactly once, the shorter query tile takes part in a PREFIX of the steps, the copier
-    stages every needed block once, and in ring order the first blocks are the rank's own."""
+    query tile may see is visited exactly once, the copier stages every needed block once, and in ring order the first blocks are the rank's own."""
     import random
 
     rnd = random.Random(0)
@@ -214,15 +240,11 @@ def test_visiting_order_model_of_the_exchange_kernel():
                     else:
                         assert staged == list(range(nb))
                     for _ in range(25):
-                        n1 = rnd.randint(0, nb)
-                        n0 = rnd.randint(0, n1)
-                        if rnd.random() < 0.2:
-                            n0, n1 = n1, 0                          # second query tile out of range
-                        seq = _walk(n0, n1, order, tc)
-                        assert sorted(seq) == list(range(max(n0, n1)))
-                        assert sorted(seq[: min(n0, n1)]) == list(range(min(n0, n1)))
+                        n = rnd.randint(0, nb)
+                        seq = _walk(n, order, tc)
+                        assert sorted(seq) == list(range(n))
                         if not ring:
-                            assert seq == list(range(max(n0, n1)))  # global order: what the single-device kernel does
+                            assert seq == list(range(n))            # global order: what the single-device kernel does
 
 
 def test_shared_context_cache_is_bounded_and_evicts_least_recently_used():

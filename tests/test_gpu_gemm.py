@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 GEMM (+bias, +GELU) and patch embedding vs the CPU oracle."""
+"""GPU parity: wgmma GEMM (+bias, +GELU) and patch embedding vs the CPU oracle."""
 import pytest
 import torch
 import torch.nn.functional as F

@@ -7,6 +7,7 @@
   replaced by the CPU oracle (tests/hostlogic.py), against oracle.model.long_vita_forward.
   This checks composition and indexing only; kernel parity is the `-m gpu` suite.
 """
+import os
 import types
 
 import pytest
@@ -16,15 +17,20 @@ from long_vita_b200.config import LongVITAConfig
 from long_vita_b200.megatron import checkpoint as ck
 from long_vita_b200.weights import synthetic_state_dict
 from oracle import model as OM
+from oracle import ref_loader
 from tests.hostlogic import oracle_ops
 from tests.util import rel_fro
 
 
-@pytest.fixture(scope="module")
-def tiny():
+def tiny_setup():
     cfg = LongVITAConfig.tiny(layers=2, vit_layers=1)
     hf = synthetic_state_dict(cfg, seed=77, dtype=torch.bfloat16, perturb=True)
     return cfg, hf, ck.hf_to_mcore(hf, cfg)
+
+
+@pytest.fixture(scope="module")
+def tiny():
+    return tiny_setup()
 
 
 def test_checkpoint_roundtrip_is_bit_exact(tiny):
@@ -76,13 +82,17 @@ def _inputs(cfg, s=300, n_img=1, seed=5):
     return ids, images, torch.stack([torch.zeros_like(idx_s), idx_s])
 
 
-@pytest.fixture(scope="module")
-def model(tiny):
+def build_model(mc, cfg):
     from long_vita_b200.megatron.gpt_vl_model import B200GPTVLModel
 
-    cfg, hf, mc = tiny
     with oracle_ops():
         return B200GPTVLModel(cfg, mc)
+
+
+@pytest.fixture(scope="module")
+def model(tiny):
+    cfg, hf, mc = tiny
+    return build_model(mc, cfg)
 
 
 def _oracle_logits(cfg, hf, ids, images, idx, rows):
@@ -376,22 +386,30 @@ def test_masked_lm_head_forward_and_dgrad_equal_the_references_own_function():
     assert torch.equal(dx[:, 0].float().abs().sum(-1) == 0, gold["dx"][:, 0].abs().sum(-1) == 0)   # same zero rows
 
 
-@pytest.mark.skipif(not __import__("os").path.isdir("/root/reference"), reason="/root/reference not mounted (GPU box)")
-def test_checkpoint_layout_is_the_inverse_of_the_references_own_converter():
-    """Live: the reference's `convert_checkpoint_from_megatron_to_transformers` (tools/hf2mcore_long_vita.py:373-510,
-    executed from /root/reference) walks a Megatron-shaped module tree built from `checkpoint.hf_to_mcore(hf)` and
-    fills the reference's own HF model; that model's state dict must be `hf` again, bit for bit - so our mcore names
-    and row orders are exactly the ones the reference's converter reads.  (The converter hard-codes the ViT
-    geometry 1024 / 16 heads, so the vision tower has the real width here.)"""
-    import types
-    from dataclasses import replace
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
-    from oracle import ref_loader
+
+def _converter_case():
+    """Tiny geometry with the real ViT width (the reference's converter hard-codes 1024 / 16 heads): HF weights and
+    the mcore layout checkpoint.hf_to_mcore makes of them."""
+    from dataclasses import replace
 
     base = LongVITAConfig.tiny(layers=2, vit_layers=1)
     cfg = replace(base, visual=replace(base.visual, hidden_size=1024, num_attention_heads=16, intermediate_size=64))
     hf = synthetic_state_dict(cfg, seed=404, dtype=torch.float32, perturb=True)
-    mg = ref_loader.module_tree_from_state_dict(ck.hf_to_mcore(hf, cfg))
+    return cfg, hf, ck.hf_to_mcore(hf, cfg)
+
+
+def _sha(t):
+    import hashlib
+
+    return hashlib.sha256(t.contiguous().view(torch.int32).numpy().tobytes()).hexdigest()
+
+
+def run_reference_converter(cfg, hf, mc):
+    """The reference's `convert_checkpoint_from_megatron_to_transformers` (tools/hf2mcore_long_vita.py:373-510) on a
+    Megatron-shaped module tree holding `mc`; returns the state dict of the reference HF model it filled."""
+    mg = ref_loader.module_tree_from_state_dict(mc)
     hfmodel = ref_loader.build_reference_long_vita(cfg, {k: torch.zeros_like(v) for k, v in hf.items()})
     args = types.SimpleNamespace(
         fp16=False, bf16=False, num_query_groups=cfg.num_key_value_heads, hidden_size=cfg.hidden_size,
@@ -400,28 +418,109 @@ def test_checkpoint_layout_is_the_inverse_of_the_references_own_converter():
         vit_args=types.SimpleNamespace(hidden_size=1024, num_query_groups=16, num_attention_heads=16))
     convert = ref_loader.load_checkpoint_converter()
     convert(mg, hfmodel, args)                     # asserts internally that every parameter was copied exactly once
-    got = hfmodel.state_dict()
+    return hfmodel.state_dict()
+
+
+def converter_golden():
+    """What tests/golden/ref_checkpoint_converter.pt stores: the mcore layout (names, shapes, content hashes) that the
+    reference's converter turns back into exactly `hf` - checked here before it is stored."""
+    cfg, hf, mc = _converter_case()
+    got = run_reference_converter(cfg, hf, mc)
+    assert set(got) == set(hf) and all(torch.equal(got[k], hf[k]) for k in hf)
+    return {"seed": 404, "hf_sha": {k: _sha(v) for k, v in hf.items()},
+            "mcore": {k: (tuple(v.shape), _sha(v)) for k, v in mc.items()}}
+
+
+def test_checkpoint_layout_matches_the_references_own_converter_golden():
+    """tests/golden/ref_checkpoint_converter.pt: the mcore names, shapes and contents that the reference's own
+    converter maps back to the HF weights bit for bit (recorded from it by tests/golden/make_golden.py).
+    checkpoint.hf_to_mcore must still produce exactly that layout."""
+    gold = torch.load(os.path.join(GOLD, "ref_checkpoint_converter.pt"))
+    cfg, hf, mc = _converter_case()
+    assert {k: _sha(v) for k, v in hf.items()} == gold["hf_sha"]     # same synthetic weights as when recorded
+    assert set(mc) == set(gold["mcore"])
+    for k, v in mc.items():
+        assert (tuple(v.shape), _sha(v)) == gold["mcore"][k], k
+
+
+@pytest.mark.skipif(not ref_loader.available(), reason="the reference checkout is not available")
+def test_checkpoint_layout_is_the_inverse_of_the_references_own_converter():
+    """Live: the reference's converter walks a Megatron-shaped module tree built from `checkpoint.hf_to_mcore(hf)` and
+    fills the reference's own HF model; that model's state dict must be `hf` again, bit for bit - so our mcore names
+    and row orders are exactly the ones the reference's converter reads.  The recorded fixture must agree."""
+    cfg, hf, mc = _converter_case()
+    got = run_reference_converter(cfg, hf, mc)
     assert set(got) == set(hf)
     for k in hf:
         assert torch.equal(got[k], hf[k]), k
+    gold = torch.load(os.path.join(GOLD, "ref_checkpoint_converter.pt"))
+    assert gold == converter_golden()
 
 
-@pytest.mark.skipif(not __import__("os").path.isdir("/root/reference"), reason="/root/reference not mounted (GPU box)")
-def test_forward_glue_equals_the_references_own_gptvl_forward(tiny, model):
-    """Live: the reference's `GPTVLModel.forward` (gpt_vl_model.py:233-416) is executed from /root/reference on a
-    stand-in `self` whose sub-modules are the reference's OWN LanguageModelEmbedding and RotaryEmbedding, plus this
-    build's vision tower / decoder layers / output GEMM for the arithmetic in between.  Everything the
-    two forwards do around those calls - external_inputs routing, the embedding merge, rotary table, logit_mask,
-    labels masked_select, [s b h] -> [b s h] - must then agree bit for bit with B200GPTVLModel.forward."""
-    import os
-    import types
+# ---- GPTVLModel.forward glue (gpt_vl_model.py:233-416) ----
+# The training-tail switches (:352-369, :393-395) each case runs under: instruction-dataset shift, logit scale, soft-capping.
+_GLUE_VARIANTS = [dict(is_instruction_dataset=True), dict(output_multiplier_scale=0.5), dict(output_logit_softcapping=30.0),
+                  dict(is_instruction_dataset=True, output_multiplier_scale=2.0, output_logit_softcapping=20.0)]
+_GLUE_DEFAULTS = dict(is_instruction_dataset=False, output_multiplier_scale=None, output_logit_softcapping=None)
+GLUE_SAMPLE = 17      # stored fixture: every 17th element of each flattened output
 
-    from oracle import ref_loader
 
-    cfg, hf, mc = tiny
+def glue_cases(cfg):
+    """(name, switches, inputs, keyword arguments) of every call the glue test makes."""
     ids, images, idx = _inputs(cfg)
     s = ids.shape[1]
-    args = types.SimpleNamespace(output_multiplier_scale=None, output_logit_softcapping=None, is_instruction_dataset=False)
+    mask = torch.zeros(1, s, dtype=torch.bool)
+    mask[0, 270:] = True
+    labels = torch.randint(0, cfg.vocab_size, (1, s), generator=torch.Generator().manual_seed(1))
+    pos = torch.arange(s).unsqueeze(0)
+    ext = {"images": images, "indices": idx}
+    ip = types.SimpleNamespace(external_inputs=ext, key_value_memory_dict={}, logit_mask=mask, use_kv_cache=False)
+    base = [("ext", dict(external_inputs=ext)), ("ext_mask", dict(external_inputs=ext, logit_mask=mask)),
+            ("inference_params", dict(inference_params=ip)),
+            ("ext_mask_labels", dict(external_inputs=ext, logit_mask=mask, labels=labels)), ("text_only", dict())]
+    cases = [(name, {}, kw) for name, kw in base]
+    for i, variant in enumerate(_GLUE_VARIANTS):
+        for name, kw in (("ext_mask_labels", base[3][1]), ("ext_mask", base[1][1])):
+            cases.append((f"{name}/variant{i}", variant, kw))
+    return ids, pos, cases
+
+
+def run_glue(model, cfg, call, set_switches=lambda sw: None):
+    """Runs every glue case through `call(ids, pos, kw)` (with the switches applied to the model and through
+    `set_switches`) and returns {name: (output of call, output of this build's model, output of the un-fused tail or None)}."""
+    ids, pos, cases = glue_cases(cfg)
+    out = {}
+    for name, variant, kw in cases:
+        sw = {**_GLUE_DEFAULTS, **variant}
+        for k_, v_ in sw.items():
+            setattr(model, k_, v_)
+        set_switches(sw)
+        try:
+            want = call(ids, pos, kw)
+            got = model(ids, pos, None, **kw)
+            unfused = None
+            if "labels" in kw and set(variant) <= {"is_instruction_dataset"}:   # the fused tail takes these
+                model.fused_loss = False
+                unfused = model(ids, pos, None, **kw)
+                model.fused_loss = True
+        finally:
+            for k_, v_ in _GLUE_DEFAULTS.items():
+                setattr(model, k_, v_)
+            set_switches(_GLUE_DEFAULTS)
+        out[name] = (want, got, unfused)
+    return out
+
+
+def reference_glue_outputs(cfg, model):
+    """The reference's `GPTVLModel.forward` (gpt_vl_model.py:233-416), executed from the reference checkout on a
+    stand-in `self` whose sub-modules are the reference's OWN LanguageModelEmbedding and RotaryEmbedding, plus this
+    build's vision tower / decoder layers / output GEMM (oracle arithmetic) for the work in between; returns
+    run_glue's table."""
+    import socket
+
+    import torch.distributed as dist
+
+    args = types.SimpleNamespace(**_GLUE_DEFAULTS)
     ref_forward = ref_loader.load_class_methods(
         "long_vita_megatron/core/models/multimodal/gpt_vl_model.py", "GPTVLModel", {"forward"},
         namespace={"Tensor": torch.Tensor, "InferenceParams": object, "PackedSeqParams": object, "get_args": lambda: args,
@@ -466,58 +565,57 @@ def test_forward_glue_equals_the_references_own_gptvl_forward(tiny, model):
         embedding=embedding, position_embedding_type="rope", rotary_pos_emb=rotary, decoder=decoder, config=None,
         unused=torch.zeros(cfg.hidden_size, dtype=torch.bfloat16), share_embeddings_and_output_weights=False,
         output_layer=output_layer, compute_language_model_loss=loss_fn)
-    mask = torch.zeros(1, s, dtype=torch.bool)
-    mask[0, 270:] = True
-    labels = torch.randint(0, cfg.vocab_size, (1, s), generator=torch.Generator().manual_seed(1))
-    pos = torch.arange(s).unsqueeze(0)
-    ext = {"images": images, "indices": idx}
-    ip = types.SimpleNamespace(external_inputs=ext, key_value_memory_dict={}, logit_mask=mask, use_kv_cache=False)
-    import socket
-
-    import torch.distributed as dist
-
     with socket.socket() as sock:
         sock.bind(("127.0.0.1", 0))
         port = sock.getsockname()[1]
     dist.init_process_group("gloo", rank=0, world_size=1, init_method=f"tcp://127.0.0.1:{port}")   # forward asks get_rank()
     try:
         with oracle_ops(), cpu_placement():
-            cases = [dict(external_inputs=ext), dict(external_inputs=ext, logit_mask=mask), dict(inference_params=ip),
-                     dict(external_inputs=ext, logit_mask=mask, labels=labels), dict()]
-            for kw in cases:
-                want = ref_forward(me, ids, pos, None, **kw)
-                got = model(ids, pos, None, **kw)
-                if "labels" in kw:
-                    # fused LM head + chunked cross-entropy (8f-3): same bf16 logits, fp32 log-sum-exp summed per chunk
-                    assert got.shape == want.shape and torch.allclose(got, want, rtol=1e-6, atol=1e-5), sorted(kw)
-                    model.fused_loss = False        # the un-fused tail reproduces the reference's glue bit for bit
-                    got = model(ids, pos, None, **kw)
-                    model.fused_loss = True
-                assert got.shape == want.shape and torch.equal(got, want), sorted(kw)
-            # the switches of the training tail (:352-369, :393-395): instruction-dataset shift, logit scale, soft-capping
-            for variant in (dict(is_instruction_dataset=True), dict(output_multiplier_scale=0.5),
-                            dict(output_logit_softcapping=30.0),
-                            dict(is_instruction_dataset=True, output_multiplier_scale=2.0, output_logit_softcapping=20.0)):
-                for k_, v_ in variant.items():
-                    setattr(args, k_, v_)
-                    setattr(model, k_, v_)
-                try:
-                    for kw in (dict(external_inputs=ext, logit_mask=mask, labels=labels), dict(external_inputs=ext, logit_mask=mask)):
-                        want = ref_forward(me, ids, pos, None, **kw)
-                        got = model(ids, pos, None, **kw)
-                        assert got.shape == want.shape, (variant, sorted(kw))
-                        if "labels" in kw and set(variant) == {"is_instruction_dataset"}:      # the fused tail takes this one
-                            assert torch.allclose(got, want, rtol=1e-6, atol=1e-5), variant
-                            model.fused_loss = False
-                            got = model(ids, pos, None, **kw)
-                            model.fused_loss = True
-                        assert torch.equal(got, want), (variant, sorted(kw))
-                finally:
-                    for k_ in variant:
-                        setattr(args, k_, False if k_ == "is_instruction_dataset" else None)
-                        setattr(model, k_, False if k_ == "is_instruction_dataset" else None)
+            return run_glue(model, cfg, lambda ids, pos, kw: ref_forward(me, ids, pos, None, **kw),
+                            lambda sw: [setattr(args, k_, v_) for k_, v_ in sw.items()])
     finally:
         dist.destroy_process_group()
+
+
+def glue_golden(table):
+    """The stored form of the reference's outputs: shape and every GLUE_SAMPLE-th element (fp32)."""
+    return {name: (tuple(want.shape), want.detach().float().reshape(-1)[::GLUE_SAMPLE].clone())
+            for name, (want, _, _) in table.items()}
+
+
+def test_forward_glue_matches_the_references_own_gptvl_forward_golden(tiny, model):
+    """tests/golden/ref_gptvl_forward_glue.pt: the reference's own GPTVLModel.forward on these inputs (recorded by
+    tests/golden/make_golden.py, see reference_glue_outputs).  B200GPTVLModel.forward - external_inputs routing, the
+    embedding merge, rotary table, logit_mask, labels masked_select, [s b h] -> [b s h], the training-tail switches -
+    must reproduce it.  Bound: 2e-3 relative (bf16 rounding of the logits; any routing error is O(1))."""
+    cfg, hf, mc = tiny
+    gold = torch.load(os.path.join(GOLD, "ref_gptvl_forward_glue.pt"))
+    with oracle_ops():
+        table = run_glue(model, cfg, lambda ids, pos, kw: None)
+    assert set(table) == set(gold)
+    for name, (_, got, unfused) in table.items():
+        shape, want = gold[name]
+        for out in (got,) if unfused is None else (got, unfused):
+            assert tuple(out.shape) == shape, name
+            assert rel_fro(out.float().reshape(-1)[::GLUE_SAMPLE], want) < 2e-3, name
+
+
+@pytest.mark.skipif(not ref_loader.available(), reason="the reference checkout is not available")
+def test_forward_glue_equals_the_references_own_gptvl_forward(tiny, model):
+    """Live: the reference's `GPTVLModel.forward` against B200GPTVLModel.forward, bit for bit (the fused LM head +
+    chunked cross-entropy within fp32 rounding, its un-fused tail bit for bit); the recorded fixture must agree."""
+    cfg, hf, mc = tiny
+    table = reference_glue_outputs(cfg, model)
+    for name, (want, got, unfused) in table.items():
+        assert got.shape == want.shape, name
+        if unfused is not None:
+            # fused LM head + chunked cross-entropy (8f-3): same bf16 logits, fp32 log-sum-exp summed per chunk
+            assert torch.allclose(got, want, rtol=1e-6, atol=1e-5), name
+            got = unfused           # the un-fused tail reproduces the reference's glue bit for bit
+        assert torch.equal(got, want), name
+    gold = torch.load(os.path.join(GOLD, "ref_gptvl_forward_glue.pt"))
+    for name, (shape, sample) in glue_golden(table).items():
+        assert gold[name][0] == shape and rel_fro(sample, gold[name][1]) < 2e-3, name
 
 
 def test_masked_lm_head_autograd_matches_reference_formulas():

@@ -44,7 +44,7 @@ def test_tile_grid_equals_the_oracle_and_the_fixture():
         assert (gx * S, gy * S) == tuple(gp)
 
 
-@pytest.mark.skipif(not ref_loader.available(), reason="/root/reference not mounted")
+@pytest.mark.skipif(not ref_loader.available(), reason="the reference checkout is not available")
 def test_tile_grid_equals_the_references_own_dynamic_preprocess():
     sys.path.insert(0, GOLD)
     from make_golden import reference_dynamic_grid

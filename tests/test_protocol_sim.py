@@ -1,108 +1,10 @@
-"""The mbarrier protocols of the pipelined backward kernel (attn_bwd2_kernel, tools/sim_bwd2_protocol.py) and of the
-forward kernel (attn_fwd_kernel, tools/sim_fwd_protocol.py) checked by discrete-event simulation: random interleavings
-of the warp roles and the tensor pipe must neither deadlock nor touch an operand that is not ready.  Runs in a few
-seconds on the CPU."""
+"""The context-parallel exchange protocol of the attention kernel (ready words, buffer parity, exit wait;
+tools/sim_cp_protocol.py) checked by discrete-event simulation: ranks at random relative speeds must neither deadlock
+nor read a buffer that is not ready.  Runs in a few seconds on the CPU."""
 import importlib.util
 import os
-import random
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _sim():
-    spec = importlib.util.spec_from_file_location("sim_bwd2", os.path.join(ROOT, "tools", "sim_bwd2_protocol.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-def test_backward_v2_protocol_has_no_deadlock_or_stale_operand():
-    sim = _sim()
-    for seed in range(80):
-        rng = random.Random(7000 + seed)
-        items = [rng.choice([0, 1, 1, 2, 3, 5, 8]) for _ in range(rng.randint(1, 7))]
-        sim.Sim(items, seed).run()
-
-
-def test_the_simulator_detects_a_wrong_parity():
-    sim = _sim()
-
-    class Broken(sim.Sim):
-        def producer(self):                      # waits for the wrong phase of res_empty
-            for k, nvis in enumerate(self.items):
-                yield ("wait", "res_empty", k & 1)
-                self.later("res_full")
-
-    try:
-        Broken([2, 1], 0).run()
-    except (RuntimeError, AssertionError):
-        return
-    raise AssertionError("a producer waiting on the wrong res_empty parity was not detected")
-
-
-def _fwd():
-    spec = importlib.util.spec_from_file_location("sim_fwd", os.path.join(ROOT, "tools", "sim_fwd_protocol.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
-
-
-FWD_CONFIGS = ((2, 1), (4, 1), (4, 2))      # (K / V ring stages, Q buffers): head_dim 128, 64, 64 with LV_ATTN_QBUF64=2
-
-
-def test_forward_protocol_has_no_deadlock_or_operand_hazard():
-    sim = _fwd()
-    for seed in range(40):
-        items = sim.random_items(random.Random(5000 + seed))
-        for ns, qb in FWD_CONFIGS:
-            sim.Sim(items, seed, ns, qb).run()
-    # the ViT's work list (S = 1025: four full query-block pairs and a last block whose second tile is out of range)
-    vit = ([(9, 9)] * 4 + [(9, 0)]) * 3
-    for seed in range(5):
-        for ns, qb in FWD_CONFIGS:
-            sim.Sim(vit, seed, ns, qb).run()
-
-
-def test_forward_simulator_reproduces_the_round_2_o_free_deadlock():
-    """The first multi-item run at head_dim 64 hung on the GPU: o_free completed a phase in every item and the issuer
-    consumed the phase of a tile without key tiles at the end of the item - after that tile's epilogue warps could
-    already have arrived for the current item too.  The simulation of that version deadlocks on the ViT's work list;
-    the shipped protocol (phases only in items where the tile has key tiles) does not."""
-    sim = _fwd()
-    vit = ([(9, 9)] * 2 + [(9, 0)] + [(9, 9)]) * 2
-    hung = 0
-    for seed in range(20):
-        sim.Sim(vit, seed, 4, 1).run()
-        try:
-            sim.Sim(vit, seed, 4, 1, round2_bug=True).run()
-        except RuntimeError as e:
-            assert "deadlock" in str(e) and "o_free1" in str(e)
-            hung += 1
-    assert hung > 0, "the round-2 o_free protocol did not deadlock in the simulation"
-
-    class IssuerCountsEveryItem(sim.Sim):          # a plain phase-count mismatch between the two sides is seen as well
-        def of_counts(self, n0, n1):
-            return True, True
-
-    try:
-        IssuerCountsEveryItem(vit, 0, 4, 1).run()
-    except RuntimeError as e:
-        assert "deadlock" in str(e)
-        return
-    raise AssertionError("the o_free phase mismatch was not detected")
-
-
-def test_forward_simulator_sees_every_missing_wait():
-    sim = _fwd()
-    for skip in ("p_full", "p_half", "k_empty", "v_empty", "q_empty", "o_full"):
-        caught = 0
-        for seed in range(12):
-            items = sim.random_items(random.Random(5000 + seed))
-            try:
-                sim.Sim(items, seed, 2, 1, skip=[skip]).run()
-            except (RuntimeError, AssertionError):
-                caught += 1
-        assert caught > 0, f"leaving out the {skip} wait went unnoticed"
 
 
 def _cp():

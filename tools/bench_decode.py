@@ -66,7 +66,7 @@ def main():
     try:
         peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]
     except Exception:  # noqa: BLE001
-        peak = 6650.0
+        peak = 3350.0       # H100 SXM data sheet (HBM3), the same fallback as bench.py
     # kernel-only: the decode attention of one layer at this context
     q = torch.randn(cfg.num_attention_heads, cfg.head_dim, device="cuda", dtype=torch.bfloat16)
     for _ in range(3):

@@ -1,6 +1,6 @@
-"""Per-kernel timing on one B200 (CUDA events on the launching stream, warm-up, L2 flush between
-timed launches) next to the same-box comparators the reference would run (flash-attn 2.8 sm_100
-build, cuDNN SDPA, cuBLAS via torch.matmul).  Writes gpurun_out/kernels.json.
+"""Per-kernel timing on one H100 (CUDA events on the launching stream, warm-up, L2 flush between
+timed launches) next to the same-box comparators the reference would run (flash-attn 2.8,
+cuDNN SDPA, cuBLAS via torch.matmul).  Writes the JSON given by --out (default kernels.json).
 
   python tools/bench_kernels.py [--only attn|gemm|elem] [--quick]
 """
@@ -21,8 +21,9 @@ try:
     PEAKS = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
 except Exception:
     pass
-HBM = PEAKS.get("hbm_gbs", 6650.0)
-TF = PEAKS.get("bf16_tflops", 1590.0)
+# without MEASURED_PEAKS.json: the H100 SXM data sheet (dense bf16, HBM3), the same fallback as bench.py
+HBM = PEAKS.get("hbm_gbs", 3350.0)
+TF = PEAKS.get("bf16_tflops", 989.0)
 
 _flush = None
 
@@ -146,7 +147,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", default=None)
     ap.add_argument("--quick", action="store_true")
-    ap.add_argument("--out", default=os.path.join(ROOT, "gpurun_out", "kernels.json"))
+    ap.add_argument("--out", default="kernels.json")
     a = ap.parse_args()
     results = []
     if a.only in (None, "attn"):
