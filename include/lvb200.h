@@ -108,6 +108,36 @@ int64_t lv_attn_bwd_ws_bytes(int64_t batch, int64_t hq, int64_t sq);
 int lv_attn_bwd(const lv_attn_bwd_params* p, lv_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Document-masked attention over one packed row of training samples (`--reset-attention-mask`),
+ * forward and backward.
+ *
+ * Replaces the packed-sample attention of the reference: on GPU, _flash_attention_forward called
+ * with the reset position ids (long_vita_megatron/core/transformer/dot_product_attention.py:374-390),
+ * which transformers turns into flash_attn_varlen_func over the documents; on NPU, the varlen flash
+ * attention fed with actual_seq_len as the document ends (long_vita_modellink/core/transformer/
+ * dot_product_attention.py:334-365, 373-382, 460-470).  Same mask as Megatron's
+ * get_ltor_masks_and_position_ids(reset_attention_mask=True) (training/utils.py:192-249).
+ *
+ * The row holds n_docs documents with boundaries cu_seqlens = {0 = c_0 < c_1 < ... < c_n = sk}
+ * (int32, device memory; the layout of flash-attn varlen, Megatron's PackedSeqParams and
+ * transformers; the reference's actual_seq_len is c_1 .. c_n).  Key j is visible to query i iff
+ * both lie in the same document and j <= i.  `a` / `p` are filled as for lv_attn_fwd / lv_attn_bwd
+ * with batch = 1, sq = sk, causal = 1, q_seg_len = sq, q_seg_pos = {0, 0}, kv_pos0 = 0; any other
+ * value returns LV_EINVAL.  Key tiles that lie wholly in earlier documents are skipped, so the cost
+ * follows the visible pairs sum_i L_i (L_i + 1) / 2 rather than S (S + 1) / 2.  With n_docs = 1 the
+ * results are bit-identical to lv_attn_fwd / lv_attn_bwd with causal = 1.  No workspace beyond
+ * lv_attn_bwd's; deterministic (no atomics).  The kernels clamp every index they derive from
+ * cu_seqlens (memory-safe on a malformed table), but the result is only defined for a valid one.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct lv_attn_docs {
+  const int32_t* cu_seqlens;  /* device, [n_docs + 1]: 0 = c0 < c1 < ... < c_n = sk */
+  int64_t n_docs;
+} lv_attn_docs;
+
+int lv_attn_docs_fwd(const lv_attn_params* a, const lv_attn_docs* docs, lv_stream_t stream);
+int lv_attn_docs_bwd(const lv_attn_bwd_params* p, const lv_attn_docs* docs, lv_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * Context-parallel attention (forward): zig-zag sequence sharding with the K/V exchange inside the
  * attention kernel.
  *

@@ -44,6 +44,12 @@ class AttnBwdParams(C.Structure):
     ]
 
 
+class AttnDocs(C.Structure):
+    """Mirror of `lv_attn_docs` (include/lvb200.h)."""
+
+    _fields_ = [("cu_seqlens", c_ptr), ("n_docs", c_i64)]
+
+
 class CpParams(C.Structure):
     """Mirror of `lv_cp_params` (include/lvb200.h)."""
 
@@ -62,6 +68,8 @@ SIGNATURES = {
     "lv_attn_fwd": (c_i32, [C.POINTER(AttnParams), c_ptr]),
     "lv_attn_bwd_ws_bytes": (c_i64, [c_i64, c_i64, c_i64]),
     "lv_attn_bwd": (c_i32, [C.POINTER(AttnBwdParams), c_ptr]),
+    "lv_attn_docs_fwd": (c_i32, [C.POINTER(AttnParams), C.POINTER(AttnDocs), c_ptr]),
+    "lv_attn_docs_bwd": (c_i32, [C.POINTER(AttnBwdParams), C.POINTER(AttnDocs), c_ptr]),
     "lv_attn_cp_fwd": (c_i32, [C.POINTER(AttnParams), C.POINTER(CpParams), c_ptr]),
     "lv_cp_check_fault": (c_i32, [c_ptr, c_ptr]),
     "lv_ipc_alloc": (c_i32, [c_i64, C.POINTER(c_ptr)]),

@@ -154,6 +154,14 @@ class CPBackwardMixin:
         return dq[0], dk, dv
 
 
+def _refuse_packing(cu_seqlens) -> None:
+    """Packed samples under context parallelism would need a document-aware exchange (the copier and the key walk of
+    lv_attn_cp_fwd); the reference's own CP path for packed samples is not runnable either.  Refuse, never ignore."""
+    if cu_seqlens is not None:
+        raise NotImplementedError("packed samples (cu_seqlens / --reset-attention-mask) under context parallelism are "
+                                  "not supported")
+
+
 class _CPAttentionFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, q, k, v, cp_ctx, scale):
@@ -172,10 +180,12 @@ class _CPAttentionFn(torch.autograd.Function):
         return dq, dk, dv, None, None
 
 
-def cp_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cp_ctx, scale: Optional[float] = None) -> torch.Tensor:
+def cp_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cp_ctx, scale: Optional[float] = None,
+                 cu_seqlens=None) -> torch.Tensor:
     """Differentiable context-parallel causal attention: q [T, hq, d], k / v [T, hkv, d] are this
     rank's zig-zag rows; returns [T, hq * d].  Forward = the fused in-kernel exchange
-    (`lv_attn_cp_fwd`), backward = CPBackwardMixin.attention_backward."""
+    (`lv_attn_cp_fwd`), backward = CPBackwardMixin.attention_backward.  Packed documents (`cu_seqlens`) raise."""
+    _refuse_packing(cu_seqlens)
     return _CPAttentionFn.apply(q, k, v, cp_ctx, scale)
 
 
@@ -281,19 +291,22 @@ class CPContext(CPBackwardMixin):
         return self.qkv[self.epoch & 1]
 
     def attention(self, out: Optional[torch.Tensor] = None, scale: Optional[float] = None,
-                  lse: Optional[torch.Tensor] = None) -> torch.Tensor:
+                  lse: Optional[torch.Tensor] = None, cu_seqlens=None) -> torch.Tensor:
         """Causal attention of the local queries (already RoPE'd, inside qkv_buffer()) over the whole
         sequence; K/V of the other ranks are pulled by the kernel.  Returns [T, hq*d]; `lse` ([1, hq, T] fp32,
-        optional) receives the log-sum-exp."""
+        optional) receives the log-sum-exp.  Packed documents (`cu_seqlens`) raise NotImplementedError."""
+        _refuse_packing(cu_seqlens)
         assert self.fused_qkv
         buf = self.qkv[self.epoch & 1]
         return self._launch(buf.data_ptr(), (self.T * self.row, self.row, self.d), out, scale, lse)
 
     def attention_separate(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out=None, scale=None,
-                           return_lse: bool = False):
+                           return_lse: bool = False, cu_seqlens=None):
         """q [T, hq, d], k/v [T, hkv, d] (strided views are fine): K|V are copied into the peer-mapped
         buffer (T * 2 hkv d elements - small next to the attention itself), Q is read in place.
-        With return_lse also returns the log-sum-exp [1, hq, T] fp32 (what the backward needs)."""
+        With return_lse also returns the log-sum-exp [1, hq, T] fp32 (what the backward needs).  Packed documents
+        (`cu_seqlens`) raise NotImplementedError."""
+        _refuse_packing(cu_seqlens)
         assert not self.fused_qkv
         buf = self.qkv[self.epoch & 1].view(self.T, 2, self.hkv, self.d)
         buf[:, 0].copy_(k)

@@ -124,7 +124,7 @@ int encode_tmap_bf16(CUtensorMap* out, const void* base, int rank, const uint64_
 
 extern "C" {
 
-int lv_version(void) { return 1 * 1000 + 0; }
+int lv_version(void) { return 1 * 1000 + 1; }
 
 const char* lv_last_error(void) { return lv::g_err; }
 

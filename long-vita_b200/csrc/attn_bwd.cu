@@ -8,6 +8,12 @@
 // Recomputing S in both passes costs 7 GEMM-units instead of the minimal 5, but needs no atomics
 // (bit-reproducible dQ) and no dQ transposes.
 //
+// Document mode (DOCS, lv_attn_docs_bwd; see docs.cuh): pass B's key steps start at the 64-key tile holding the
+// document start of the query tile's first row; pass A streams a 64-row query tile only if it starts before the end of
+// the document of the key tile's last key.  Per element, a key is visible iff it is not after the query and lies in
+// its document: kpos >= doc_start(qpos) in pass B (queries are rows), qpos < doc_end(kpos) in pass A (keys are rows) -
+// the same predicate for kpos <= qpos, evaluated on the row side so it costs one lookup per row and item.
+//
 // Replaces flash-attn 2's backward, reached in the reference through autograd of
 // flash_attn_func / TE AttnFuncWithCP (dot_product_attention.py:318-326, 374-390).
 #include <cuda_bf16.h>
@@ -17,6 +23,7 @@
 #include <stdlib.h>
 
 #include "common.cuh"
+#include "docs.cuh"
 #include "ptx.cuh"
 
 namespace lv {
@@ -31,6 +38,7 @@ struct BwdKParams {
   int n_items;
   const float* lse;     // [b, hq, sq] natural log
   const float* delta;   // [b, hq, sq]
+  DocsKParams docs;     // document mode only
 };
 
 // delta = rowsum(dO * O)
@@ -133,7 +141,7 @@ __device__ __forceinline__ int item_tile(const BwdKParams& p, int item) {
   return (MODE == 1 && p.causal) ? n - 1 - r : r;
 }
 
-template <int D, int MODE>
+template <int D, int MODE, bool DOCS>
 __global__ void __launch_bounds__(BW_THREADS, 1)
     attn_bwd_kernel(const __grid_constant__ CUtensorMap tmR0, const __grid_constant__ CUtensorMap tmR1,
                     const __grid_constant__ CUtensorMap tmS0, const __grid_constant__ CUtensorMap tmS1,
@@ -185,6 +193,11 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
     if (hi < 0) return 0;
     return (int)min((long long)n_k64, hi / 64 + 1);
   };
+  // MODE 1, document mode: first 64-key tile visible to 128-row query tile t (query row == position there)
+  auto k_first = [&](int t) -> int { return DOCS ? doc_start(p.docs, t * 128) / 64 : 0; };
+  // MODE 0, document mode: one past the last query row that can see a key of [key0, key0 + 128) - the end of the
+  // document holding the last key (< sk) of the range
+  auto q_end = [&](int key0) -> int { return DOCS ? doc_end(p.docs, min(key0 + 127, p.sk - 1), p.sk) : 0x7fffffff; };
 
   if (warp < 4) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
@@ -213,12 +226,13 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
           tma_load_4d(sR1 + bx * 16384, &tmR1, res_full, bx * 64, t * 128, head, b, kEvictFirst);
         }
         if (MODE == 0) {
+          const int qend = q_end(t * 128);
           for (int g = 0; g < G; ++g)
             for (int qt = 0; qt < n_q64; ++qt)
-              if (q_sees(p, qt, (long long)t * 128)) load_str(qt, head * G + g, b);
+              if (q_sees(p, qt, (long long)t * 128) && qt * 64 < qend) load_str(qt, head * G + g, b);
         } else {
           const int n = n_k_steps(t);
-          for (int kt = 0; kt < n; ++kt) load_str(kt, head / G, b);
+          for (int kt = k_first(t); kt < n; ++kt) load_str(kt, head / G, b);
         }
       }
     }
@@ -247,6 +261,19 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
 #pragma unroll
       for (int i = 0; i < D / 2; ++i) acc0[i] = acc1[i] = 0.f;
       const int rrow0 = t * 128 + c * 64;                  // first resident row of this warpgroup
+      // document mode, per resident row r of this thread: MODE 0 (rows = keys) the number of queries that see key r -
+      // they are r .. doc_end(r) - 1 (0 for a row past the end) -, MODE 1 (rows = queries) the start of r's document
+      int drow0 = 0, drow1 = 0;
+      if (DOCS) {
+        const int r0 = rrow0 + r_lo, r1 = r0 + 8;
+        if (MODE == 0) {
+          drow0 = r0 < p.sk ? doc_end(p.docs, r0, p.sk) - r0 : 0;
+          drow1 = r1 < p.sk ? doc_end(p.docs, r1, p.sk) - r1 : 0;
+        } else {
+          drow0 = doc_start(p.docs, min(r0, p.sq - 1));
+          drow1 = doc_start(p.docs, min(r1, p.sq - 1));
+        }
+      }
       mbar_wait(res_full, item_cnt & 1);
 
       // one streamed tile: rows / columns -> masking, P, dS, the two accumulating products
@@ -292,8 +319,14 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
                 const float lse2 = st_buf[8 * jj + cq + e];
                 const float dl = st_buf[64 + 8 * jj + cq + e];
                 const long long qpos = qp + 8 * jj + cq + e;
-                const bool vis0 = qv && kv0 && (!p.causal || kpos0 <= qpos);
-                const bool vis1 = qv && kv1 && (!p.causal || kpos1 <= qpos);
+                bool vis0, vis1;
+                if (DOCS) {   // query qi sees key k iff k <= qi < doc_end(k)
+                  vis0 = (unsigned)(qi - (rrow0 + r_lo)) < (unsigned)drow0;
+                  vis1 = (unsigned)(qi - (rrow0 + r_lo + 8)) < (unsigned)drow1;
+                } else {
+                  vis0 = qv && kv0 && (!p.causal || kpos0 <= qpos);
+                  vis1 = qv && kv1 && (!p.causal || kpos1 <= qpos);
+                }
                 pr[e] = vis0 ? ex2(fmaf(x[4 * jj + e], scale_log2, -lse2)) : 0.f;
                 pr[2 + e] = vis1 ? ex2(fmaf(x[4 * jj + 2 + e], scale_log2, -lse2)) : 0.f;
                 ds[e] = pr[e] * (dp[4 * jj + e] - dl) * scale;
@@ -319,8 +352,8 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
                 const int ki = row64 * 64 + 8 * jj + cq + e;
                 const long long kpos = p.kv_pos0 + ki;
                 const bool kv = ki < p.sk;
-                const bool vis0 = qv0 && kv && (!p.causal || kpos <= qpos0);
-                const bool vis1 = qv1 && kv && (!p.causal || kpos <= qpos1);
+                const bool vis0 = qv0 && kv && (!p.causal || kpos <= qpos0) && (!DOCS || kpos >= drow0);
+                const bool vis1 = qv1 && kv && (!p.causal || kpos <= qpos1) && (!DOCS || kpos >= drow1);
                 pr[e] = vis0 ? ex2(fmaf(x[4 * jj + e], scale_log2, -lse0)) : 0.f;
                 pr[2 + e] = vis1 ? ex2(fmaf(x[4 * jj + 2 + e], scale_log2, -lse1)) : 0.f;
                 ds[e] = pr[e] * (dp[4 * jj + e] - dl0) * scale;
@@ -347,13 +380,19 @@ __global__ void __launch_bounds__(BW_THREADS, 1)
       };
 
       if (MODE == 0) {
+        // document mode: a streamed tile this warpgroup's keys cannot see (all its queries past the document of the
+        // keys) is masked element-wise; only the 128-key tile's range is skipped
+        const int qend = q_end(t * 128);
         for (int g = 0; g < G; ++g)
           for (int qt = 0; qt < n_q64; ++qt)
-            if (q_sees(p, qt, (long long)t * 128)) step(qt, head * G + g, q_sees(p, qt, (long long)rrow0));
+            if (q_sees(p, qt, (long long)t * 128) && qt * 64 < qend) step(qt, head * G + g, q_sees(p, qt, (long long)rrow0));
       } else {
         const int n = n_k_steps(t);
         const long long my_last = q_row_pos(p, rrow0) + 63 - p.kv_pos0;   // last key index this half sees
-        for (int kt = 0; kt < n; ++kt) step(kt, head, !p.causal || (long long)kt * 64 <= my_last);
+        // document mode: the first key this half sees is the document start of its first row
+        const int my_first = DOCS ? doc_start(p.docs, min(rrow0, p.sq - 1)) : 0;
+        for (int kt = k_first(t); kt < n; ++kt)
+          step(kt, head, (!p.causal || (long long)kt * 64 <= my_last) && (!DOCS || kt * 64 + 63 >= my_first));
       }
 
       // ---------------- epilogue: bf16 outputs staged in this warpgroup's half of the resident tiles -> TMA ----------
@@ -387,8 +426,8 @@ static int make_map(CUtensorMap* m, const void* ptr, int64_t D, int64_t s, int64
   return encode_tmap_bf16(m, ptr, 4, dims, st, box, true);
 }
 
-template <int D>
-static int launch_bwd(const lv_attn_bwd_params* a, cudaStream_t s) {
+template <int D, bool DOCS = false>
+static int launch_bwd(const lv_attn_bwd_params* a, cudaStream_t s, const DocsKParams* docs = nullptr) {
   const lv_attn_params* f = &a->fwd;
   constexpr int SMEM = BwdCfg<D>::SMEM;
   // resident operands: 128-row boxes; streamed operands and outputs: 64-row boxes
@@ -432,23 +471,24 @@ static int launch_bwd(const lv_attn_bwd_params* a, cudaStream_t s) {
   p.n_kt = (int)((f->sk + 127) / 128);
   p.lse = f->lse;
   p.delta = a->delta_ws;
+  p.docs = DOCS ? *docs : DocsKParams{nullptr, 0};
   static PerDeviceOnce attr_once;
   int attr_dev;
   if (attr_once.needed(&attr_dev)) {
-    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<D, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<D, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<D, 0, DOCS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_bwd_kernel<D, 1, DOCS>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
     attr_once.done(attr_dev);
   }
   {
     p.n_items = p.batch * p.hkv * p.n_kt;
     const int grid = p.n_items < sm_count() ? p.n_items : sm_count();
-    attn_bwd_kernel<D, 0><<<grid, BW_THREADS, SMEM, s>>>(tmKr, tmVr, tmQs, tmdOs, tmdV, tmdK, p);
+    attn_bwd_kernel<D, 0, DOCS><<<grid, BW_THREADS, SMEM, s>>>(tmKr, tmVr, tmQs, tmdOs, tmdV, tmdK, p);
     LV_CHECK_LAUNCH("attn_bwd_kernel<dKdV>");
   }
   {
     p.n_items = p.batch * p.hq * p.n_qt;
     const int grid = p.n_items < sm_count() ? p.n_items : sm_count();
-    attn_bwd_kernel<D, 1><<<grid, BW_THREADS, SMEM, s>>>(tmQr, tmdOr, tmKs, tmVs, tmdQ, tmdQ, p);
+    attn_bwd_kernel<D, 1, DOCS><<<grid, BW_THREADS, SMEM, s>>>(tmQr, tmdOr, tmKs, tmVs, tmdQ, tmdQ, p);
     LV_CHECK_LAUNCH("attn_bwd_kernel<dQ>");
   }
   return LV_OK;
@@ -460,7 +500,7 @@ using namespace lv;
 
 extern "C" int64_t lv_attn_bwd_ws_bytes(int64_t batch, int64_t hq, int64_t sq) { return batch * hq * sq * (int64_t)sizeof(float); }
 
-extern "C" int lv_attn_bwd(const lv_attn_bwd_params* a, lv_stream_t stream) {
+static int check_bwd_params(const lv_attn_bwd_params* a) {
   LV_CHECK_ARG(a != nullptr, "lv_attn_bwd: null params");
   const lv_attn_params* f = &a->fwd;
   LV_CHECK_ARG(f->q && f->k && f->v && f->out && f->lse, "lv_attn_bwd: q, k, v, out and lse of the forward pass are required");
@@ -473,8 +513,28 @@ extern "C" int lv_attn_bwd(const lv_attn_bwd_params* a, lv_stream_t stream) {
     LV_CHECK_ARG(f->q_strides[i] % 8 == 0 && f->k_strides[i] % 8 == 0 && f->v_strides[i] % 8 == 0 && f->o_strides[i] % 2 == 0 &&
                      a->do_strides[i] % 8 == 0 && a->dq_strides[i] % 8 == 0 && a->dk_strides[i] % 8 == 0 && a->dv_strides[i] % 8 == 0,
                  "lv_attn_bwd: strides must be multiples of 8 elements (16 bytes)");
+  return LV_OK;
+}
+
+extern "C" int lv_attn_bwd(const lv_attn_bwd_params* a, lv_stream_t stream) {
+  int rc = check_bwd_params(a);
+  if (rc) return rc;
+  const lv_attn_params* f = &a->fwd;
   LV_BIND_DEVICE(f->q);
   cudaStream_t s = (cudaStream_t)stream;
   if (f->d == 128) return launch_bwd<128>(a, s);
   return launch_bwd<64>(a, s);
+}
+
+extern "C" int lv_attn_docs_bwd(const lv_attn_bwd_params* a, const lv_attn_docs* docs, lv_stream_t stream) {
+  int rc = check_bwd_params(a);
+  if (rc) return rc;
+  const lv_attn_params* f = &a->fwd;
+  rc = check_docs_params(f, docs, "lv_attn_docs_bwd");
+  if (rc) return rc;
+  LV_BIND_DEVICE(f->q);
+  const DocsKParams dk{docs->cu_seqlens, (int)docs->n_docs};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (f->d == 128) return launch_bwd<128, true>(a, s, &dk);
+  return launch_bwd<64, true>(a, s, &dk);
 }

@@ -1,5 +1,5 @@
 // Fused attention forward for sm_90a: softmax(scale * Q K^T + mask) V with online softmax, GQA,
-// causal / zig-zag-causal / no mask, LSE output.
+// causal / zig-zag-causal / document-causal (packed samples) / no mask, LSE output.
 //
 // One persistent CTA per SM, 3 warpgroups, warp-specialised:
 //   warp 0          TMA producer: one 128-row Q tile per work item and a K ring + V ring of 128-row
@@ -13,6 +13,11 @@
 //                   overlap one's softmax with the other's MMAs; nothing enforces that order.  At the end O is
 //                   normalised, staged in the warpgroup's half of the (now free) Q tile and stored with TMA.
 //
+// Document mode (DOCS, lv_attn_docs_fwd): the query tile's key walk starts at the tile holding the document start of
+// its first row instead of tile 0; tiles wholly before that document are never loaded.  Masks apply on the diagonal
+// tiles, the ragged last tile and on tiles below the document start of the warpgroup's last row, where every row gets
+// its own lower bound doc_start(row).
+//
 // Reference call sites replaced: flash_attn_func / _flash_attention_forward in
 // long_vita_megatron/core/transformer/dot_product_attention.py:318-326, 374-390 and
 // long_vita/models/long_vita_qwen2_intern/flash_attention.py:52-74.
@@ -22,6 +27,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "docs.cuh"
 #include "ptx.cuh"
 
 namespace lv {
@@ -41,6 +47,7 @@ struct AttnKParams {
   int block_major; // 1: order work items (q-block, kv-head, head) - global longest-first; 0: (kv-head, q-block, head)
   int serpentine;  // 1: odd rounds sweep the item list backwards (default); LV_ATTN_SCHED=0 turns it off for A/B runs
   float* lse;
+  DocsKParams docs;  // document mode only
 };
 
 // Context-parallel extension (zig-zag layout, training/utils.py:329-341).  Every rank keeps its own
@@ -318,11 +325,13 @@ __device__ __forceinline__ void split_item(const AttnKParams& p, int item, int& 
 
 struct WorkItem {
   int b, h, kvh;
-  int n;             // kv tiles the query tile attends to (0: nothing to do)
+  int j0;            // first kv tile the query tile attends to (document mode; 0 otherwise)
+  int n;             // one past the last kv tile the query tile attends to (0: nothing to do)
   long long qpos;    // global position of row 0 of the query tile
   int row0;          // local row index of row 0 of the query tile
 };
 
+template <bool DOCS>
 __device__ __forceinline__ WorkItem decode_item(const AttnKParams& p, int item) {
   WorkItem w;
   const int G = p.hq / p.hkv;
@@ -345,6 +354,9 @@ __device__ __forceinline__ WorkItem decode_item(const AttnKParams& p, int item) 
     }
   }
   w.n = n;
+  // document mode (qpos == row0, kv_pos0 == 0): start at the tile that holds the document start of the first row;
+  // doc_start(row0) <= row0 < (the diagonal tile + 1) * 128, so every query tile keeps at least its diagonal
+  w.j0 = DOCS ? doc_start(p.docs, w.row0) / A_BN : 0;
   return w;
 }
 
@@ -373,7 +385,7 @@ __device__ __forceinline__ void mma_pv(float (&o)[D / 2], const uint32_t (&pk)[3
   }
 }
 
-template <int D, bool CP>
+template <int D, bool CP, bool DOCS>
 __global__ void __launch_bounds__(A_THREADS, 1)
     attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmO,
@@ -421,9 +433,9 @@ __global__ void __launch_bounds__(A_THREADS, 1)
         uint32_t item_cnt = 0, kcnt = 0, vcnt = 0;
         KvWalk walk;
         for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
-          const WorkItem w = decode_item(p, item);
+          const WorkItem w = decode_item<DOCS>(p, item);
           if (CP) walk.begin(w.n);
-          const int pre = min(NS, w.n);
+          const int pre = min(NS, w.n - w.j0);
           auto load_tile = [&](int j) {
             int g = j;            // global key tile visited in step j
             if (CP) {
@@ -461,12 +473,12 @@ __global__ void __launch_bounds__(A_THREADS, 1)
           };
           // The Q load of this item waits for the previous item's epilogue (O is staged in the Q tile); its first key
           // tiles do not (their ring slots free up as the previous item's last MMAs retire), so they are requested first.
-          for (int j = 0; j < pre; ++j) load_tile(j);
+          for (int j = w.j0; j < w.j0 + pre; ++j) load_tile(j);
           mbar_wait(q_empty, (item_cnt & 1) ^ 1);
           mbar_arrive_expect_tx(q_full, Cfg::TILE_BYTES);
           for (int bx = 0; bx < Cfg::BOXES; ++bx)
             tma_load_4d(sQ + bx * 16384, &tmQ, q_full, bx * 64, w.row0, w.h, w.b, kEvictFirst);
-          for (int j = pre; j < w.n; ++j) load_tile(j);
+          for (int j = w.j0 + pre; j < w.n; ++j) load_tile(j);
         }
       }
     } else if (warp >= 2) {
@@ -489,7 +501,7 @@ __global__ void __launch_bounds__(A_THREADS, 1)
     uint32_t item_cnt = 0, kcnt = 0, vcnt = 0;
 
     for (int round = 0, item; (item = sched_item(round, p.n_items, p.serpentine)) >= 0; ++round, ++item_cnt) {
-      const WorkItem w = decode_item(p, item);
+      const WorkItem w = decode_item<DOCS>(p, item);
       const int n = w.n;
       // global positions of this thread's two query rows
       const long long qpos0 = w.qpos + c * 64 + r_lo, qpos1 = qpos0 + 8;
@@ -502,12 +514,20 @@ __global__ void __launch_bounds__(A_THREADS, 1)
         const long long jd = dd < 0 ? 0 : dd / A_BN + 1;
         if (jd < j_mask) j_mask = (int)jd;
       }
+      // document mode: the first visible key of each of this thread's rows, and of the warpgroup's last row (tiles
+      // below it hold keys of an earlier document for some row and need the mask)
+      int ds0 = 0, ds1 = 0, ds_last = 0;
+      if (DOCS) {
+        ds0 = doc_start(p.docs, min((int)qpos0, p.sq - 1));
+        ds1 = doc_start(p.docs, min((int)qpos1, p.sq - 1));
+        ds_last = doc_start(p.docs, min((int)w.qpos + c * 64 + 63, p.sq - 1));
+      }
       float o[D / 2];
 #pragma unroll
       for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
       float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // running max (log2 domain) and sum per row
       mbar_wait(q_full, item_cnt & 1);
-      for (int j = 0; j < n; ++j) {
+      for (int j = w.j0; j < n; ++j) {
         int g = j;         // global key tile of this step (context parallelism visits them out of order)
         if (CP) g = walk.next(cpp);
         const int kst = kcnt % NS;
@@ -521,14 +541,16 @@ __global__ void __launch_bounds__(A_THREADS, 1)
         wgmma_keep(s);
         if (wg_tid == 0) mbar_arrive(&k_empty[kst]);
 
-        // ---- mask (only diagonal tiles and the ragged last key tile) ----
-        if (g >= j_mask) {
+        // ---- mask (only diagonal tiles and the ragged last key tile; document mode: also tiles below a row's
+        //      document start) ----
+        if (g >= j_mask || (DOCS && g * A_BN < ds_last)) {
           const long long kidx0 = (long long)g * A_BN;
           long long lim0 = p.sk - kidx0, lim1 = lim0;                 // first invalid column of each row
           if (p.causal) {
             lim0 = min(lim0, qpos0 - p.kv_pos0 - kidx0 + 1);
             lim1 = min(lim1, qpos1 - p.kv_pos0 - kidx0 + 1);
           }
+          const int lo0 = ds0 - (int)kidx0, lo1 = ds1 - (int)kidx0;   // first visible column (document mode)
 #pragma unroll
           for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
@@ -536,6 +558,8 @@ __global__ void __launch_bounds__(A_THREADS, 1)
               const int col = 8 * jj + cq + e;
               if (col >= lim0) s[4 * jj + e] = -INFINITY;
               if (col >= lim1) s[4 * jj + 2 + e] = -INFINITY;
+              if (DOCS && col < lo0) s[4 * jj + e] = -INFINITY;
+              if (DOCS && col < lo1) s[4 * jj + 2 + e] = -INFINITY;
             }
           }
         }
@@ -631,8 +655,8 @@ __global__ void __launch_bounds__(A_THREADS, 1)
   }
 }
 
-template <int D, bool CP>
-static int launch_attn(const lv_attn_params* a, const CpKParams* cp, cudaStream_t s) {
+template <int D, bool CP, bool DOCS = false>
+static int launch_attn(const lv_attn_params* a, const CpKParams* cp, cudaStream_t s, const DocsKParams* docs = nullptr) {
   using Cfg = AttnCfg<D>;
   CUtensorMap tmQ, tmK, tmV, tmO;
   const uint32_t box[4] = {64, 128, 1, 1};
@@ -682,10 +706,11 @@ static int launch_attn(const lv_attn_params* a, const CpKParams* cp, cudaStream_
     return (e != nullptr && e[0] == '0') ? 0 : 1;
   }();
   p.serpentine = serp;
+  p.docs = DOCS ? *docs : DocsKParams{nullptr, 0};
   static PerDeviceOnce attr_once;   // one per template instantiation
   int attr_dev;
   if (attr_once.needed(&attr_dev)) {
-    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, CP>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_TOTAL));
+    LV_CHECK_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, CP, DOCS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_TOTAL));
     attr_once.done(attr_dev);
   }
   int grid = p.n_items < sm_count() ? p.n_items : sm_count();
@@ -695,7 +720,7 @@ static int launch_attn(const lv_attn_params* a, const CpKParams* cp, cudaStream_
     cpp = *cp;
     grid = sm_count();   // every copier warp takes part, also when there are fewer work items than SMs
   }
-  attn_fwd_kernel<D, CP><<<grid, A_THREADS, Cfg::SMEM_TOTAL, s>>>(tmQ, tmK, tmV, tmO, p, cpp);
+  attn_fwd_kernel<D, CP, DOCS><<<grid, A_THREADS, Cfg::SMEM_TOTAL, s>>>(tmQ, tmK, tmV, tmO, p, cpp);
   LV_CHECK_LAUNCH("attn_fwd_kernel");
   return LV_OK;
 }
@@ -729,6 +754,18 @@ extern "C" int lv_attn_fwd(const lv_attn_params* a, lv_stream_t stream) {
   cudaStream_t s = (cudaStream_t)stream;
   if (a->d == 128) return launch_attn<128, false>(a, nullptr, s);
   return launch_attn<64, false>(a, nullptr, s);
+}
+
+extern "C" int lv_attn_docs_fwd(const lv_attn_params* a, const lv_attn_docs* docs, lv_stream_t stream) {
+  int rc = check_attn_params(a);
+  if (rc) return rc;
+  rc = check_docs_params(a, docs, "lv_attn_docs_fwd");
+  if (rc) return rc;
+  LV_BIND_DEVICE(a->q);
+  const DocsKParams dk{docs->cu_seqlens, (int)docs->n_docs};
+  cudaStream_t s = (cudaStream_t)stream;
+  if (a->d == 128) return launch_attn<128, false, true>(a, nullptr, s, &dk);
+  return launch_attn<64, false, true>(a, nullptr, s, &dk);
 }
 
 extern "C" int lv_attn_cp_fwd(const lv_attn_params* a, const lv_cp_params* c, lv_stream_t stream) {

@@ -5,7 +5,10 @@
   dropout=, scaling=, **kw) -> (out[b,s,h,d], None)`); `register()` installs it under the name
   "b200_fa" so a stock HF Qwen2 / Long-VITA model runs on it with
   `attn_implementation="b200_fa"` where the reference passes "flash_attention_2"
-  (tools/inference_long_vita.py:816).
+  (tools/inference_long_vita.py:816).  Packed rows are honoured as transformers' `_flash_attention_forward` honours
+  them: pre-computed `cu_seq_lens_q` / `cu_seq_lens_k` in the kwargs (equal: self-attention), or batch-1
+  `position_ids` that are not one increasing run (its `_is_packed_sequence`), whose restarts at 0 are the document
+  boundaries (`prepare_fa_kwargs_from_position_ids`).  Attention then stays inside each document (lv_attn_docs_fwd).
 * `B200FlashAttention` replaces `InternAttention.inner_attn`
   (long_vita/models/long_vita_qwen2_intern/modeling_intern_vit.py:140-141, 173-175): same
   constructor and `forward(qkv[B,S,3,H,D], key_padding_mask=None, causal=False, ...)
@@ -21,6 +24,35 @@ import torch
 from .. import ops
 
 NAME = "b200_fa"
+
+_POS_CACHE = [None, None, None]   # (position_ids tensor, its version, cu_seqlens): one lookup per forward, not per layer
+
+
+def _is_packed_sequence(position_ids, batch_size: int) -> bool:
+    """transformers' rule (modeling_flash_attention_utils._is_packed_sequence): batch 1 and the positions are not
+    `arange(s) + min`."""
+    if position_ids is None or batch_size != 1:
+        return False
+    ramp = torch.arange(position_ids.shape[-1], device=position_ids.device) + position_ids.min()
+    return bool((ramp - position_ids).abs().sum())
+
+
+def _packed_cu_seqlens(query, kwargs):
+    cu_q, cu_k = kwargs.get("cu_seq_lens_q"), kwargs.get("cu_seq_lens_k")
+    if cu_q is not None or cu_k is not None:
+        if cu_q is None or cu_k is None or not torch.equal(cu_q, cu_k):
+            raise NotImplementedError("b200_fa: packed rows need cu_seq_lens_q == cu_seq_lens_k (self-attention)")
+        return cu_q.to(device=query.device, dtype=torch.int32).contiguous()
+    pos = kwargs.get("position_ids")
+    if pos is None:
+        return None
+    if _POS_CACHE[0] is pos and _POS_CACHE[1] == pos._version:
+        return _POS_CACHE[2]
+    cu = None
+    if _is_packed_sequence(pos, query.shape[0]):
+        cu = ops.packed_cu_seqlens(pos, device=query.device, seq_len=query.shape[2])
+    _POS_CACHE[:] = [pos, pos._version, cu]
+    return cu
 
 
 def b200_attention_forward(module, query, key, value, attention_mask=None, dropout: float = 0.0,
@@ -46,7 +78,11 @@ def b200_attention_forward(module, query, key, value, attention_mask=None, dropo
             raise NotImplementedError(f"b200_fa: unsupported attention_mask rank {attention_mask.dim()}")
     if is_causal is None:
         is_causal = bool(getattr(module, "is_causal", True)) and query.shape[2] > 1
-    out = ops.attention_fwd(query, key, value, causal=is_causal, scale=scaling, layout="bhsd")   # [b,h,s,d]
+    cu = _packed_cu_seqlens(query, kwargs)
+    if cu is not None and not is_causal:
+        raise NotImplementedError("b200_fa: packed rows without a causal mask are not supported")
+    out = ops.attention_fwd(query, key, value, causal=is_causal, scale=scaling, layout="bhsd",
+                            **ops.docs_kwargs(cu))                                                   # [b,h,s,d]
     return out.transpose(1, 2), None
 
 

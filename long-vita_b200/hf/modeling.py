@@ -317,8 +317,18 @@ class LongVITAModel(_WeightHolderModule):
         flash_attn_kwargs.pop("max_cache_len", None)
         if cache_position is None:
             cache_position = torch.arange(past_len, past_len + s, device=x.device)     # modeling_long_vita.py:153-158
+        attn_kwargs = {}
         if position_ids is None:
             position_ids = cache_position.unsqueeze(0)
+        else:
+            # packed samples: positions restarting at 0 inside the row are sample boundaries; attention stays inside
+            # each sample, as transformers' flash_attention_2 does for the reference (tools/inference_long_vita.py:816)
+            cu = ops.packed_cu_seqlens(position_ids, device=x.device, seq_len=s)
+            if cu is not None:
+                if cache is not None:
+                    raise NotImplementedError("packed samples (position ids restarting at 0) cannot be combined with a "
+                                              "KV cache (use_cache / past_key_values)")
+                attn_kwargs = {"cu_seqlens": cu}
         cos, sin = ops.rope_table(position_ids.reshape(-1).to(torch.int64), self.inv_freq)
 
         all_hidden = () if output_hidden_states else None
@@ -326,7 +336,7 @@ class LongVITAModel(_WeightHolderModule):
         for li, layer in enumerate(self.layers):
             if output_hidden_states:
                 all_hidden += ((x if delta is None else x + delta).view(1, s, -1),)
-            x, delta = layer.forward(x, delta, cos, sin, {}, cache, li)
+            x, delta = layer.forward(x, delta, cos, sin, attn_kwargs, cache, li)
         if cache is not None:
             cache.commit()
         if delta is None:

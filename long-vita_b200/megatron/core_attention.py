@@ -18,13 +18,21 @@ registered after `import long_vita_megatron.megatron_adaptor` (megatron_adaptor.
 
 Megatron-core is NOT importable in the build container (un-vendored submodule, SURVEY.md fact 2), so
 nothing here imports it: the mask type is duck-typed by name and process-group lookups go through
-`parallel_state` only when context parallelism is on.  tests/test_gpu_surfaces.py (kernels) and
+`parallel_state` only when context parallelism is on.
+
+Packed samples (`--reset-position-ids --reset-attention-mask`, every shipped fine-tuning script): the data pipeline
+concatenates samples into one row and the training loop publishes the sample ends through
+`long_vita_megatron.training.utils.set_actual_seq_len` (training/utils.py:509-511; only set under
+`--reset-attention-mask`).  When that list has more than one entry, attention is causal inside each sample and blind
+across samples (lv_attn_docs_fwd / lv_attn_docs_bwd), the mask of get_ltor_masks_and_position_ids
+(training/utils.py:192-249).  tests/test_gpu_surfaces.py (kernels) and
 tests/test_surfaces_host.py (host logic, CPU) drive these objects with a stub that reproduces the
 ModuleSpec / build_module calling convention.
 """
 from __future__ import annotations
 
 import math
+import sys
 from functools import wraps
 from typing import Optional
 
@@ -39,8 +47,47 @@ def _is_causal(attn_mask_type) -> bool:
     return "causal" in name
 
 
-def _attention_sbhd(query, key, value, causal: bool, scale: float, cp_ctx=None):
+_CU_CACHE = [None, None]   # (sample ends, device) -> cu_seqlens tensor of the current micro-batch
+
+
+def megatron_packed_ends():
+    """The sample ends of this micro-batch's packed row inside a Megatron job (`get_actual_seq_len()` of the reference's
+    training utils), or None: no Megatron job, no --reset-attention-mask, or a single sample."""
+    utils = sys.modules.get("long_vita_megatron.training.utils")   # imported by the training loop that publishes it
+    if utils is None or not hasattr(utils, "get_actual_seq_len"):
+        return None
+    ends = utils.get_actual_seq_len()
+    return None if ends is None or len(ends) <= 1 else ends
+
+
+def megatron_cu_seqlens(seq_len: int, device) -> Optional[torch.Tensor]:
+    """cu_seqlens of the packed row of this micro-batch (None if it is not packed).  The int32 device copy is made once
+    per micro-batch (when the list changes) and shared by every layer."""
+    ends = megatron_packed_ends()
+    if ends is None:
+        return None
+    key = (tuple(int(e) for e in ends), str(device), int(seq_len))
+    if _CU_CACHE[0] != key:
+        _CU_CACHE[0], _CU_CACHE[1] = key, ops.packed_cu_seqlens(actual_seq_len=list(key[0]), device=device,
+                                                                 seq_len=seq_len)
+    return _CU_CACHE[1]
+
+
+def _attention_sbhd(query, key, value, causal: bool, scale: float, cp_ctx=None, cu_seqlens=None):
     sq, b, np_, hn = query.shape
+    if cu_seqlens is not None:
+        if cp_ctx is not None:
+            raise NotImplementedError("packed samples (--reset-attention-mask) under context parallelism are not supported")
+        if not causal:
+            raise NotImplementedError("packed samples need a causal attention mask")
+        if b != 1:
+            raise NotImplementedError("packed samples need micro-batch 1")
+        if torch.is_grad_enabled() and (query.requires_grad or key.requires_grad or value.requires_grad):
+            out = ops.attention(query.permute(1, 0, 2, 3), key.permute(1, 0, 2, 3), value.permute(1, 0, 2, 3),
+                                causal=True, scale=scale, cu_seqlens=cu_seqlens)   # [1, sq, np, hn]
+            return out.permute(1, 0, 2, 3).reshape(sq, b, np_ * hn)
+        out = ops.attention_fwd(query, key, value, causal=True, scale=scale, layout="sbhd", cu_seqlens=cu_seqlens)
+        return out.reshape(sq, b, np_ * hn)
     if cp_ctx is not None:
         if b != 1:
             raise AssertionError("context-parallel attention supports micro-batch 1 (the reference's long-context setting)")
@@ -85,6 +132,8 @@ class B200DotProductAttention(torch.nn.Module):
     def _cp(self, query, key):
         if self.cp_size <= 1 or not _is_causal(self.attn_mask_type):
             return None
+        if megatron_packed_ends() is not None:
+            raise NotImplementedError("packed samples (--reset-attention-mask) under context parallelism are not supported")
         sq, _, np_, hn = query.shape
         if self._cp_ctx is None or self._cp_ctx.S != sq * self.cp_size:
             # keyed on the sequence length of THIS call: a later micro-batch of another length gets its own buffers
@@ -102,7 +151,9 @@ class B200DotProductAttention(torch.nn.Module):
         )                                                                     # dot_product_attention.py:156-159
         mask_type = self.attn_mask_type if attn_mask_type is None else attn_mask_type
         causal = _is_causal(mask_type)
-        return _attention_sbhd(query, key, value, causal, self.softmax_scale, self._cp(query, key))
+        cp_ctx = self._cp(query, key)
+        cu = None if cp_ctx is not None else megatron_cu_seqlens(query.shape[0], query.device)
+        return _attention_sbhd(query, key, value, causal, self.softmax_scale, cp_ctx, cu)
 
 
 def b200_dot_product_attention_forward_wrapper(fn):
@@ -119,7 +170,8 @@ def b200_dot_product_attention_forward_wrapper(fn):
         mask_type = getattr(self, "attn_mask_type", None) if attn_mask_type is None else attn_mask_type
         hn = query.shape[-1]
         scale = getattr(self, "softmax_scale", None) or 1.0 / math.sqrt(hn)
-        return _attention_sbhd(query, key, value, _is_causal(mask_type), scale)
+        return _attention_sbhd(query, key, value, _is_causal(mask_type), scale,
+                               cu_seqlens=megatron_cu_seqlens(query.shape[0], query.device))
 
     return wrapper
 

@@ -20,6 +20,11 @@ What is kept from the reference and what is deliberately not:
   the [M, vocab] logits the masked head produced - off the hot path.
 * micro-batch 1 (the reference's long-context setting; `assert b == 1` at :325, :385).
 
+Packed samples (`--reset-position-ids --reset-attention-mask`): position ids that restart at 0 inside the row mark
+sample boundaries (compute_actual_seq_len, training/utils.py:53-57); attention is then causal within each sample and
+blind across samples (ops.packed_cu_seqlens -> lv_attn_docs_fwd), as the reference's flash-attention path does.  The
+boundaries are read once per forward.  Packing is not combined with context parallelism or a KV cache (both raise).
+
 Under context parallelism the caller passes this rank's shard exactly as
 `get_batch_on_this_cp_rank` (training/utils.py:252-343) produces it: zig-zag `input_ids`,
 `position_ids`, `logit_mask`, and `external_inputs = {images, src_indices, tgt_indices}`; pass the
@@ -165,16 +170,27 @@ class B200GPTVLModel:
         # RoPE: Megatron builds the table for positions 0..S-1 and slices it zig-zag under CP
         # (rotary_pos_embedding.py:36-47, 84-122); position_ids from get_batch_on_this_cp_rank are
         # exactly those positions, so the table is generated from them directly.
+        position_ids_default = position_ids is None
         if position_ids is None:
             assert self.cp is None, "context parallelism needs this rank's position_ids"
             p0 = 0 if cache is None else len(cache)
             position_ids = torch.arange(p0, p0 + s, device=x.device).unsqueeze(0)
         cos, sin = ops.rope_table(position_ids.reshape(-1).to(torch.int64), self.inv_freq)
+        attn_kwargs = {}
+        if not position_ids_default:
+            cu = ops.packed_cu_seqlens(position_ids, device=x.device, seq_len=s)
+            if cu is not None:
+                if self.cp is not None:
+                    raise NotImplementedError("packed samples (position ids restarting at 0) under context parallelism "
+                                              "are not supported")
+                if cache is not None:
+                    raise NotImplementedError("packed samples cannot be combined with a KV cache")
+                attn_kwargs = {"cu_seqlens": cu}
 
         delta = None
         for li, layer in enumerate(self.layers):
             if self.cp is None:
-                x, delta = layer.forward(x, delta, cos, sin, {}, cache, li)
+                x, delta = layer.forward(x, delta, cos, sin, attn_kwargs, cache, li)
             else:
                 x, delta = layer.forward_cp(x, delta, cos, sin, self.cp)
         if cache is not None:

@@ -21,6 +21,10 @@ tools/hf2mcore_long_vita.py:486-507):
 then its k, then its v; hf2mcore_long_vita.py:488-498); it is re-ordered once, lazily, into
 [all q | all k | all v] so that q/k/v are uniformly strided views of one GEMM output.
 
+Packed samples (`--reset-attention-mask`): when the training loop has published more than one sample end through
+`long_vita_megatron.training.utils.set_actual_seq_len`, attention is causal within each sample only
+(core_attention.megatron_cu_seqlens; lv_attn_docs_fwd / lv_attn_docs_bwd).  Not combined with context parallelism.
+
 Inference takes the fused path (GEMM epilogues, in-place RoPE, fused add + norm).  When gradients are enabled and
 anything requires grad, `_forward_train` builds the same layer from differentiable pieces whose backward passes are
 kernels too (`lv_rmsnorm_bwd`, `lv_swiglu_bwd`, `lv_attn_bwd`, the GEMM on transposed operands).
@@ -32,6 +36,7 @@ from typing import Optional
 import torch
 
 from .. import ops
+from .core_attention import megatron_cu_seqlens, megatron_packed_ends
 
 
 class _Params(torch.nn.Module):
@@ -112,6 +117,8 @@ class B200TransformerLayer(torch.nn.Module):
         reduce-scatter backward).  None when context_parallel_size == 1."""
         if self.cp_size <= 1:
             return None
+        if megatron_packed_ends() is not None:
+            raise NotImplementedError("packed samples (--reset-attention-mask) under context parallelism are not supported")
         if self._cp_ctx is None or self._cp_ctx.S != s * self.cp_size:
             from ..cp import CPContext
 
@@ -161,7 +168,8 @@ class B200TransformerLayer(torch.nn.Module):
         if cp_ctx is not None:
             att = cp_ctx.attention_separate(q, k, v)                               # [s, np * hn]
         else:
-            att = ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True)
+            att = ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True,
+                                    **ops.docs_kwargs(megatron_cu_seqlens(s, hidden_states.device)))
         o = ops.linear(att.view(s, np_ * hn), self.self_attention.linear_proj.weight)
         hcur, x = ops.rmsnorm(o, self.mlp.linear_fc1.layer_norm_weight, self.eps, residual=x)
         a = ops.linear(hcur, self._fc1_w, act="swiglu")
@@ -198,7 +206,8 @@ class B200TransformerLayer(torch.nn.Module):
 
             att = cp_attention(q.contiguous(), k, v, cp_ctx)                                    # [s, np * hn]
         else:
-            att = ops.attention(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True)   # [1, s, np, hn]
+            att = ops.attention(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True,
+                                **ops.docs_kwargs(megatron_cu_seqlens(s, hidden_states.device)))    # [1, s, np, hn]
         o = ops.linear_autograd(att.reshape(s, np_ * hn), a.linear_proj.weight)
         hcur, x = ops.rmsnorm_autograd(o, self.mlp.linear_fc1.layer_norm_weight, self.eps, residual=x)
         gate_up = ops.linear_autograd(hcur, self.mlp.linear_fc1.weight)                         # cat(gate, up)

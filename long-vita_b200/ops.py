@@ -13,7 +13,7 @@ from typing import Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import AttnBwdParams, AttnParams
+from ._lib import AttnBwdParams, AttnDocs, AttnParams
 
 
 def _stream() -> int:
@@ -81,6 +81,104 @@ def launch_count() -> int:
 
 
 # ------------------------------------------------------------------------------------------------
+# packed documents (`--reset-position-ids --reset-attention-mask`)
+# ------------------------------------------------------------------------------------------------
+def _check_cu_host(cu, seq_len: Optional[int]) -> Tuple[int, ...]:
+    cu = tuple(int(c) for c in cu)
+    if len(cu) < 2 or cu[0] != 0 or any(b <= a for a, b in zip(cu, cu[1:])):
+        raise ValueError(f"cu_seqlens must be 0 = c0 < c1 < ... < c_n (got {list(cu[:8])}{' ...' if len(cu) > 8 else ''})")
+    if seq_len is not None and cu[-1] != seq_len:
+        raise ValueError(f"cu_seqlens ends at {cu[-1]}, the packed row has {seq_len} tokens")
+    if cu[-1] >= 2 ** 31:
+        raise ValueError("cu_seqlens: sequence too long for int32 boundaries")
+    return cu
+
+
+def _mark_cu(cu_host: Tuple[int, ...], device) -> torch.Tensor:
+    """int32 device tensor of validated boundaries; remembers the host copy so later calls neither sync nor re-check."""
+    t = torch.tensor(cu_host, dtype=torch.int32, device=device)
+    t._lv_cu_host = cu_host
+    return t
+
+
+def packed_cu_seqlens(position_ids: Optional[torch.Tensor] = None, actual_seq_len=None, *, device=None,
+                      seq_len: Optional[int] = None) -> Optional[torch.Tensor]:
+    """Document boundaries of one packed row, or None when the row holds a single sample.
+
+    `actual_seq_len` is the reference's list of cumulative sample ends (long_vita/data/dataset_qwen2.py:160-166,
+    published by training/utils.py:509-511): cu_seqlens = [0] + actual_seq_len.  From `position_ids` ([1, s], [s, 1] as
+    Megatron stores them, or [s]) the boundaries are the rows after row 0 whose position is 0 - compute_actual_seq_len
+    (training/utils.py:53-57), and transformers' prepare_fa_kwargs_from_position_ids for a row starting at 0.  A row
+    whose positions never restart (including a zig-zag context-parallel shard, whose positions jump upwards) is not
+    packed.  Returns a validated int32 tensor on `device` (default: that of position_ids, else the current CUDA
+    device).  Call it once per forward: it reads the boundaries to the host (one synchronisation), the attention calls
+    of every layer then reuse the tensor without another one.  Raises ValueError for micro-batch > 1, for packed
+    position ids that do not start at 0, and for boundaries that are not strictly increasing or do not end at
+    `seq_len`."""
+    if (position_ids is None) == (actual_seq_len is None):
+        raise ValueError("packed_cu_seqlens: pass exactly one of position_ids and actual_seq_len")
+    if actual_seq_len is not None:
+        ends = [int(e) for e in (actual_seq_len.reshape(-1).tolist() if torch.is_tensor(actual_seq_len) else actual_seq_len)]
+        if len(ends) <= 1:
+            if seq_len is not None and len(ends) == 1 and ends[0] != seq_len:
+                raise ValueError(f"actual_seq_len ends at {ends[0]}, the packed row has {seq_len} tokens")
+            return None
+        cu = _check_cu_host([0] + ends, seq_len)
+    else:
+        pos = position_ids
+        if pos.dim() == 2:
+            if pos.shape[0] != 1 and pos.shape[1] != 1:
+                raise ValueError(f"packed documents need micro-batch 1 (position_ids {tuple(pos.shape)})")
+        elif pos.dim() != 1:
+            raise ValueError(f"position_ids must be [1, s], [s, 1] or [s], got {tuple(pos.shape)}")
+        flat = pos.reshape(-1).cpu()
+        starts = (torch.nonzero(flat[1:] == 0).view(-1) + 1).tolist()
+        if not starts:
+            return None
+        if int(flat[0]) != 0:
+            raise ValueError(f"packed position_ids must start at 0 (got {int(flat[0])})")
+        cu = _check_cu_host([0] + starts + [flat.numel()], seq_len)
+        if device is None:
+            device = pos.device
+    if device is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return _mark_cu(cu, device)
+
+
+def _docs_arg(cu_seqlens: torch.Tensor, seq_len: int):
+    """(AttnDocs, host boundaries) of a cu_seqlens tensor; checked on the host unless packed_cu_seqlens made it."""
+    _need_cuda(cu_seqlens, torch.int32)
+    host = getattr(cu_seqlens, "_lv_cu_host", None)
+    if host is None or host[-1] != seq_len or len(host) != cu_seqlens.numel():
+        host = _check_cu_host(cu_seqlens.reshape(-1).tolist(), seq_len)
+    elif not cu_seqlens.is_contiguous():
+        raise ValueError("cu_seqlens must be contiguous")
+    d = AttnDocs()
+    d.cu_seqlens, d.n_docs = cu_seqlens.data_ptr(), len(host) - 1
+    return d, host
+
+
+def _docs_flops(host, hq: int, d: int) -> float:
+    """Visible work of a packed row: 4 hq d sum_i L_i (L_i + 1) / 2."""
+    return 4.0 * hq * d * sum((b - a) * (b - a + 1) / 2 for a, b in zip(host, host[1:]))
+
+
+def docs_kwargs(cu_seqlens: Optional[torch.Tensor]) -> dict:
+    """`cu_seqlens=` for the attention calls of a packed row, nothing for an unpacked one: unpacked calls keep exactly
+    the arguments they had before document mode existed."""
+    return {} if cu_seqlens is None else {"cu_seqlens": cu_seqlens}
+
+
+def _check_docs_call(b, sq, sk, causal, q_seg_len, q_seg_pos, kv_pos0):
+    if not causal:
+        raise NotImplementedError("packed documents without a causal mask are not supported")
+    if b != 1 or sq != sk:
+        raise ValueError(f"packed documents need batch 1 and self-attention (got b={b}, sq={sq}, sk={sk})")
+    if q_seg_len is not None or q_seg_pos is not None or kv_pos0:
+        raise ValueError("packed documents take no q_seg_len / q_seg_pos / kv_pos0")
+
+
+# ------------------------------------------------------------------------------------------------
 # attention
 # ------------------------------------------------------------------------------------------------
 def attention_fwd(
@@ -96,17 +194,25 @@ def attention_fwd(
     q_seg_pos: Optional[Tuple[int, int]] = None,
     kv_pos0: int = 0,
     out: Optional[torch.Tensor] = None,
+    cu_seqlens: Optional[torch.Tensor] = None,
 ):
     """softmax(scale * q k^T + mask) v.  `layout` names the dimension order of q/k/v and of the
     returned tensor: "bshd" (flash-attn / HF), "sbhd" (Megatron, dot_product_attention.py:344) or
     "bhsd" (HF AttentionInterface).  Strided views are consumed in place (no .contiguous()) as
     long as the head dimension is contiguous and the other strides are multiples of 8 elements.
-    Returns out (same layout as q) or (out, lse[b, hq, sq] float32)."""
+    Returns out (same layout as q) or (out, lse[b, hq, sq] float32).
+
+    `cu_seqlens` (int32 [n_docs + 1], see packed_cu_seqlens) makes the row a packed stream of documents: each query
+    sees the keys of its own document up to itself (lv_attn_docs_fwd; batch 1, self-attention, causal only)."""
     _need_cuda_bf16(q, k, v)
     perm = {"bshd": (0, 1, 2, 3), "sbhd": (1, 0, 2, 3), "bhsd": (0, 2, 1, 3)}[layout]
     qv, kv_, vv = (t.permute(perm) for t in (q, k, v))  # views in b, s, h, d order
     b, sq, hq, d = qv.shape
     _, sk, hkv, _ = kv_.shape
+    docs = host = None
+    if cu_seqlens is not None:
+        _check_docs_call(b, sq, sk, causal, q_seg_len, q_seg_pos, kv_pos0)
+        docs, host = _docs_arg(cu_seqlens, sk)
 
     def ok(t):
         return t.stride(3) == 1 and all(s % 8 == 0 for s in t.stride()[:3])
@@ -138,9 +244,14 @@ def attention_fwd(
     p.q_seg_pos[0], p.q_seg_pos[1] = int(q_seg_pos[0]), int(q_seg_pos[1])
     p.kv_pos0 = int(kv_pos0)
     ev0 = _TIMER.start() if _TIMER is not None else None
-    _lib.check(_lib.lib().lv_attn_fwd(C.byref(p), _stream()), "lv_attn_fwd")
+    if docs is not None:
+        _lib.check(_lib.lib().lv_attn_docs_fwd(C.byref(p), C.byref(docs), _stream()), "lv_attn_docs_fwd")
+    else:
+        _lib.check(_lib.lib().lv_attn_fwd(C.byref(p), _stream()), "lv_attn_fwd")
     if ev0 is not None:
-        if causal and q_seg_len is None and sq == sk:
+        if docs is not None:
+            fl = _docs_flops(host, hq, d)
+        elif causal and q_seg_len is None and sq == sk:
             fl = 4.0 * b * hq * d * (sq * (sq + 1) / 2)
         else:
             fl = 4.0 * b * hq * d * sq * sk  # upper bound for masked / segmented calls
@@ -167,11 +278,15 @@ def _fill_attn_params(p, qv, kv_, vv, ov, lse, scale, causal, q_seg_len, q_seg_p
 
 
 def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[float] = None, q_seg_len=None,
-                  q_seg_pos=None, kv_pos0: int = 0):
-    """Gradients of attention_fwd (layout "bshd").  `out` / `lse` are the forward results.
-    Returns (dq, dk, dv) with the shapes of q, k, v."""
+                  q_seg_pos=None, kv_pos0: int = 0, cu_seqlens: Optional[torch.Tensor] = None):
+    """Gradients of attention_fwd (layout "bshd").  `out` / `lse` are the forward results, `cu_seqlens` the packed
+    documents the forward was called with.  Returns (dq, dk, dv) with the shapes of q, k, v."""
     _need_cuda_bf16(d_out, q, k, v, out)
     _need_cuda(lse, torch.float32)
+    docs = None
+    if cu_seqlens is not None:
+        _check_docs_call(q.shape[0], q.shape[1], k.shape[1], causal, q_seg_len, q_seg_pos, kv_pos0)
+        docs, _ = _docs_arg(cu_seqlens, k.shape[1])
 
     def fix(t):
         return t if (t.stride(3) == 1 and all(s % 8 == 0 for s in t.stride()[:3])) else t.contiguous()
@@ -187,28 +302,33 @@ def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[flo
     for name, t in (("do_strides", d_out), ("dq_strides", dq), ("dk_strides", dk), ("dv_strides", dv)):
         arr = getattr(p, name)
         arr[0], arr[1], arr[2] = t.stride(0), t.stride(1), t.stride(2)
-    _lib.check(_lib.lib().lv_attn_bwd(C.byref(p), _stream()), "lv_attn_bwd")
+    if docs is not None:
+        _lib.check(_lib.lib().lv_attn_docs_bwd(C.byref(p), C.byref(docs), _stream()), "lv_attn_docs_bwd")
+    else:
+        _lib.check(_lib.lib().lv_attn_bwd(C.byref(p), _stream()), "lv_attn_bwd")
     return dq, dk, dv
 
 
 class _AttentionFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, q, k, v, causal, scale):
-        out, lse = attention_fwd(q, k, v, causal=causal, scale=scale, return_lse=True)
+    def forward(ctx, q, k, v, causal, scale, cu_seqlens):
+        out, lse = attention_fwd(q, k, v, causal=causal, scale=scale, return_lse=True, **docs_kwargs(cu_seqlens))
         ctx.save_for_backward(q, k, v, out, lse)
-        ctx.causal, ctx.scale = causal, scale
+        ctx.causal, ctx.scale, ctx.cu_seqlens = causal, scale, cu_seqlens
         return out
 
     @staticmethod
     def backward(ctx, d_out):
         q, k, v, out, lse = ctx.saved_tensors
-        dq, dk, dv = attention_bwd(d_out.contiguous(), q, k, v, out, lse, causal=ctx.causal, scale=ctx.scale)
-        return dq, dk, dv, None, None
+        dq, dk, dv = attention_bwd(d_out.contiguous(), q, k, v, out, lse, causal=ctx.causal, scale=ctx.scale,
+                                   **docs_kwargs(ctx.cu_seqlens))
+        return dq, dk, dv, None, None, None
 
 
-def attention(q, k, v, *, causal: bool, scale: Optional[float] = None):
-    """Differentiable fused attention, "bshd" layout (the autograd twin of flash_attn_func)."""
-    return _AttentionFn.apply(q, k, v, causal, scale)
+def attention(q, k, v, *, causal: bool, scale: Optional[float] = None, cu_seqlens: Optional[torch.Tensor] = None):
+    """Differentiable fused attention, "bshd" layout (the autograd twin of flash_attn_func; with `cu_seqlens`, of
+    flash_attn_varlen_func over one packed row)."""
+    return _AttentionFn.apply(q, k, v, causal, scale, cu_seqlens)
 
 
 def _sm_count(device) -> int:
