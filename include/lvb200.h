@@ -269,6 +269,28 @@ int lv_rmsnorm_bwd(const void* x, const void* w, const void* dy, const void* add
                    int64_t rows, int64_t cols, float eps, lv_stream_t stream);
 int lv_swiglu_bwd(const void* gate_up, const void* dh, void* d_gate_up, int64_t rows, int64_t inter, lv_stream_t stream);
 
+/* Backward of the vision-tower operators (training InternViT and the projector through MegatronVisionModel,
+ * long_vita_megatron/pretrain_long_vita.py:310-596).  All reductions are deterministic: per-CTA fp32 partial rows that
+ * the caller adds, no atomics.
+ * LayerNorm (forward lv_layernorm): mean / rstd are recomputed from x in fp32; xhat = (x - mean) * rstd, g = dy * w,
+ *   dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) (+ add_in, the gradient arriving on the residual stream);
+ *   dw / db partial sums of dy * xhat / dy in dw_partials / db_partials, each [lv_layernorm_bwd_partials(rows, cols), cols]
+ *   float.  cols <= 8192 (ViT norms: 1024; pre-projection LayerNorm: 4096).  dx may be NULL (then add_in must be NULL
+ *   too): only the dw / db partials are written, for a norm whose input needs no gradient.
+ * GELU: dx = dy * gelu'(pre) where pre is the bf16 pre-activation; approx as in lv_bias_gelu (0 erf, 1 tanh).
+ * Layer-scale residual, bias-free (out = x + y * ls): dy = bf16(dout * ls); dls partial sums of dout * y in
+ *   dls_partials [lv_ls_residual_bwd_partials(rows, cols), cols] float.  dx = dout needs no kernel.
+ * Pixel shuffle: dx [n, (1 +) hw*hw, c] from dout [n, (hw/2)^2, 4c], the exact inverse permutation of lv_pixel_shuffle
+ *   (bit-exact); with has_cls the class-token rows of dx are written as zeros. */
+int64_t lv_layernorm_bwd_partials(int64_t rows, int64_t cols);
+int lv_layernorm_bwd(const void* x, const void* w, const void* dy, const void* add_in, void* dx, float* dw_partials,
+                     float* db_partials, int64_t rows, int64_t cols, float eps, lv_stream_t stream);
+int lv_gelu_bwd(const void* pre, const void* dy, void* dx, int64_t rows, int64_t cols, int32_t approx, lv_stream_t stream);
+int64_t lv_ls_residual_bwd_partials(int64_t rows, int64_t cols);
+int lv_ls_residual_bwd(const void* dout, const void* y, const void* ls, void* dy, float* dls_partials, int64_t rows,
+                       int64_t cols, lv_stream_t stream);
+int lv_pixel_shuffle_bwd(const void* dout, void* dx, int64_t n, int64_t hw, int64_t c, int32_t has_cls, lv_stream_t stream);
+
 /* Merge of split-key partial attention results (flash-decoding, one new token against a K/V cache; the
  * reference has no such path - it re-prefills every generated token, generation.py:127-135).
  * o_part bf16 [n, G, hkv, d] and lse_part float [n, hkv, G] are what lv_attn_fwd returns when the G = hq/hkv
@@ -305,6 +327,12 @@ int64_t lv_patch_embed_ws_bytes(int64_t n, int64_t img, int64_t ps, int64_t C);
 int lv_patch_embed(const void* images, const void* W, const void* bias, const void* cls, const void* pos,
                    void* out, void* ws, int64_t n, int64_t img, int64_t ps, int64_t C,
                    lv_stream_t stream);
+
+/* The im2col step of lv_patch_embed on its own: col bf16 [n * (img/ps)^2, kpad], row p of image i = the patch's
+ * 3*ps*ps pixels in (channel, y, x) order, zero-padded to kpad (a multiple of 8, >= 3*ps*ps).  With it the conv weight
+ * gradient is one lv_gemm_bias_act call: dW[C, kpad] = dP^T . col, both operands transposed so that the token
+ * dimension is the contraction. */
+int lv_patch_im2col(const void* images, void* col, int64_t n, int64_t img, int64_t ps, int64_t kpad, lv_stream_t stream);
 
 /* Cross-entropy over vocabulary CHUNKS, fused with the logit-masked LM head (SURVEY.md 8f-3): replaces
  * `compute_language_model_loss(labels, logits)` = vocab_parallel_cross_entropy(logits.float(), labels) on a

@@ -91,6 +91,13 @@ SIGNATURES = {
     "lv_rmsnorm_bwd_partials": (c_i64, [c_i64, c_i64]),
     "lv_rmsnorm_bwd": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_f32, c_ptr]),
     "lv_swiglu_bwd": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_ptr]),
+    "lv_layernorm_bwd_partials": (c_i64, [c_i64, c_i64]),
+    "lv_layernorm_bwd": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_f32, c_ptr]),
+    "lv_gelu_bwd": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i32, c_ptr]),
+    "lv_ls_residual_bwd_partials": (c_i64, [c_i64, c_i64]),
+    "lv_ls_residual_bwd": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_ptr]),
+    "lv_pixel_shuffle_bwd": (c_i32, [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i32, c_ptr]),
+    "lv_patch_im2col": (c_i32, [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr]),
     "lv_frame_preprocess_ws_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i64]),
     "lv_frame_preprocess": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_ptr, c_ptr, c_ptr, c_ptr]),
     "lv_image_tiles_ws_bytes": (c_i64, [c_i64, c_i64]),

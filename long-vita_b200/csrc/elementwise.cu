@@ -605,6 +605,232 @@ __global__ void __launch_bounds__(256) ce_grad_kernel(const __nv_bfloat16* __res
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Backward of the vision-tower operators (training InternViT and the projector).
+// ---------------------------------------------------------------------------------------------
+// LayerNorm backward.  Forward (layernorm_kernel): y = (x - mean) * rstd * w + b with fp32 statistics of the bf16 row.
+// The statistics are recomputed here the same way, then
+//   xhat = (x - mean) * rstd;  g = dy * w;  dx = rstd * (g - mean(g) - xhat * mean(g * xhat)) [+ add_in]
+//   dw[j] = sum_rows dy[j] * xhat[j];  db[j] = sum_rows dy[j]
+// With dx == nullptr only dw / db are produced (the input of the norm needs no gradient).
+// Grid-stride over rows with dw / db partial sums in registers, one partial row per (CTA, row slot), summed by the
+// caller (no atomics, as rmsnorm_bwd_kernel).
+template <int TPR, int VPT>
+__global__ void __launch_bounds__(256) layernorm_bwd_kernel(const __nv_bfloat16* __restrict__ x,
+                                                            const __nv_bfloat16* __restrict__ w,
+                                                            const __nv_bfloat16* __restrict__ dy,
+                                                            const __nv_bfloat16* __restrict__ add_in,
+                                                            __nv_bfloat16* __restrict__ dx, float* __restrict__ dw_part,
+                                                            float* __restrict__ db_part, int64_t rows, int cols, float eps) {
+  constexpr int RPC = 256 / TPR;
+  __shared__ float red[RPC * (TPR > 32 ? TPR / 32 : 1)];
+  const int row_in_cta = threadIdx.x / TPR;
+  const int t = threadIdx.x % TPR;
+  const int nvec = cols / 8;
+  float dw_acc[VPT][8], db_acc[VPT][8];
+#pragma unroll
+  for (int i = 0; i < VPT; ++i)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) dw_acc[i][j] = db_acc[i][j] = 0.f;
+  for (int64_t base = (int64_t)blockIdx.x * RPC; base < rows; base += (int64_t)gridDim.x * RPC) {
+    const int64_t row = base + row_in_cta;
+    const bool row_ok = row < rows;
+    Vec8 xr[VPT], gr[VPT];
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int c = t + i * TPR;
+      if (row_ok && c < nvec) {
+        xr[i] = ldg_stream(x + row * cols + c * 8);
+        gr[i] = ldg_stream(dy + row * cols + c * 8);
+      }
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int c = t + i * TPR;
+      if (row_ok && c < nvec) {
+        float v[8];
+        unpack(xr[i], v);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) s += v[j];
+      }
+    }
+    const float mean = row_reduce_sum<TPR>(s, red, row_in_cta, t) / (float)cols;
+    float q = 0.f;
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int c = t + i * TPR;
+      if (row_ok && c < nvec) {
+        float v[8];
+        unpack(xr[i], v);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float d = v[j] - mean;
+          q += d * d;
+        }
+      }
+    }
+    const float rstd = rsqrtf(row_reduce_sum<TPR>(q, red, row_in_cta, t) / (float)cols + eps);
+    float sg = 0.f, sgx = 0.f;
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int c = t + i * TPR;
+      if (row_ok && c < nvec) {
+        float v[8], g[8], wv[8];
+        unpack(xr[i], v);
+        unpack(gr[i], g);
+        unpack(ldg_vec(w + c * 8), wv);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const float xh = (v[j] - mean) * rstd;
+          const float gw = g[j] * wv[j];
+          sg += gw;
+          sgx += gw * xh;
+          dw_acc[i][j] += g[j] * xh;
+          db_acc[i][j] += g[j];
+        }
+      }
+    }
+    if (dx == nullptr) continue;  // uniform across the CTA: the reductions below stay collective
+    const float mg = row_reduce_sum<TPR>(sg, red, row_in_cta, t) / (float)cols;
+    const float mgx = row_reduce_sum<TPR>(sgx, red, row_in_cta, t) / (float)cols;
+#pragma unroll
+    for (int i = 0; i < VPT; ++i) {
+      const int c = t + i * TPR;
+      if (row_ok && c < nvec) {
+        float v[8], g[8], wv[8], o[8];
+        unpack(xr[i], v);
+        unpack(gr[i], g);
+        unpack(ldg_vec(w + c * 8), wv);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) o[j] = rstd * (g[j] * wv[j] - mg - (v[j] - mean) * rstd * mgx);
+        if (add_in != nullptr) {
+          float a[8];
+          unpack(ldg_stream(add_in + row * cols + c * 8), a);
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[j] += a[j];
+        }
+        stg_vec(dx + row * cols + c * 8, pack(o));
+      }
+    }
+  }
+  const int64_t prow = (int64_t)blockIdx.x * RPC + row_in_cta;
+#pragma unroll
+  for (int i = 0; i < VPT; ++i) {
+    const int c = t + i * TPR;
+    if (c < nvec) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        dw_part[prow * cols + c * 8 + j] = dw_acc[i][j];
+        db_part[prow * cols + c * 8 + j] = db_acc[i][j];
+      }
+    }
+  }
+}
+
+// GELU backward: dx = dy * gelu'(pre), pre = the bf16 pre-activation (fc1 output with its bias).
+//   erf:  gelu'(x) = Phi(x) + x * phi(x)
+//   tanh: u = k (x + 0.044715 x^3), gelu'(x) = 0.5 (1 + tanh u) + 0.5 x (1 - tanh^2 u) k (1 + 3 * 0.044715 x^2)
+__device__ __forceinline__ float gelu_erf_grad(float x) {
+  return 0.5f * (1.f + erff(x * 0.70710678118654752440f)) + x * 0.3989422804014327f * __expf(-0.5f * x * x);
+}
+__device__ __forceinline__ float gelu_tanh_grad(float x) {
+  const float k = 0.7978845608028654f;
+  const float th = tanhf(k * (x + 0.044715f * x * x * x));
+  return 0.5f * (1.f + th) + 0.5f * x * (1.f - th * th) * k * (1.f + 3.f * 0.044715f * x * x);
+}
+
+__global__ void __launch_bounds__(256) gelu_bwd_kernel(const __nv_bfloat16* __restrict__ pre,
+                                                       const __nv_bfloat16* __restrict__ dy,
+                                                       __nv_bfloat16* __restrict__ dx, int64_t total_vec, int approx) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total_vec) return;
+  float v[8], g[8], o[8];
+  unpack(ldg_stream(pre + idx * 8), v);
+  unpack(ldg_stream(dy + idx * 8), g);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) o[j] = g[j] * (approx ? gelu_tanh_grad(v[j]) : gelu_erf_grad(v[j]));
+  stg_vec(dx + idx * 8, pack(o));
+}
+
+// Layer-scale residual backward (out = x + y * ls, bias-free): dy = bf16(dout * ls), dls[j] = sum_rows dout[j] * y[j].
+// A CTA covers 32 column vectors (256 columns) x LSB_ROWS row lanes; blockIdx.y strides over the rows.  The 8 row lanes
+// are folded through shared memory in a fixed order, so CTA row blockIdx.y writes partial row blockIdx.y of
+// dls_partials [gridDim.y, cols] (summed by the caller: deterministic).
+constexpr int LSB_ROWS = 8;
+
+__global__ void __launch_bounds__(256) ls_residual_bwd_kernel(const __nv_bfloat16* __restrict__ dout,
+                                                              const __nv_bfloat16* __restrict__ y,
+                                                              const __nv_bfloat16* __restrict__ ls,
+                                                              __nv_bfloat16* __restrict__ dy, float* __restrict__ dls_part,
+                                                              int64_t rows, int cols) {
+  __shared__ float red[LSB_ROWS][32 * 8 + 1];
+  const int nvec = cols / 8;
+  const int lane = threadIdx.x % 32, rl = threadIdx.x / 32;
+  const int c = blockIdx.x * 32 + lane;
+  float acc[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+  if (c < nvec) {
+    float l[8];
+    unpack(ldg_vec(ls + c * 8), l);
+    for (int64_t r = (int64_t)blockIdx.y * LSB_ROWS + rl; r < rows; r += (int64_t)gridDim.y * LSB_ROWS) {
+      float d[8], yv[8], o[8];
+      unpack(ldg_stream(dout + r * cols + c * 8), d);
+      unpack(ldg_stream(y + r * cols + c * 8), yv);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        o[j] = d[j] * l[j];
+        acc[j] += d[j] * yv[j];
+      }
+      stg_vec(dy + r * cols + c * 8, pack(o));
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) red[rl][lane * 8 + j] = acc[j];
+  __syncthreads();
+  // 256 threads, 256 columns of this CTA: thread k sums column k over the row lanes
+  const int k = threadIdx.x;
+  const int col = blockIdx.x * 256 + k;
+  if (col < cols) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < LSB_ROWS; ++i) s += red[i][k];
+    dls_part[(int64_t)blockIdx.y * cols + col] = s;
+  }
+}
+
+// Pixel-shuffle backward: the inverse permutation of pixel_shuffle_kernel.  Blocks [0, n (hw/2)^2) move one output
+// token's four c-wide segments back to their input rows; with has_cls, the n blocks after them zero the class-token rows.
+__global__ void __launch_bounds__(128) pixel_shuffle_bwd_kernel(const __nv_bfloat16* __restrict__ dout,
+                                                                __nv_bfloat16* __restrict__ dx, int64_t n, int hw, int c,
+                                                                int has_cls) {
+  const int h2n = hw / 2;
+  const int64_t in_tok_per_img = (int64_t)hw * hw + (has_cls ? 1 : 0);
+  const int vpc = c / 8;
+  const int64_t otoks = n * h2n * h2n;
+  const int64_t b = blockIdx.x;
+  if (b >= otoks) {  // class-token row of image b - otoks
+    Vec8 z;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) z.h[i] = __floats2bfloat162_rn(0.f, 0.f);
+    __nv_bfloat16* dst = dx + (b - otoks) * in_tok_per_img * c;
+    for (int v = threadIdx.x; v < vpc; v += blockDim.x) stg_vec(dst + v * 8, z);
+    return;
+  }
+  const int64_t img = b / (h2n * h2n);
+  const int rem = (int)(b % (h2n * h2n));
+  const int w2 = rem / h2n, h2 = rem % h2n;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int wi = q >> 1, hi = q & 1;
+    const int64_t itok = img * in_tok_per_img + (has_cls ? 1 : 0) + (int64_t)(2 * w2 + wi) * hw + (2 * h2 + hi);
+    const __nv_bfloat16* src = dout + b * 4 * c + (int64_t)q * c;
+    __nv_bfloat16* dst = dx + itok * c;
+    for (int v = threadIdx.x; v < vpc; v += blockDim.x) stg_vec(dst + v * 8, ldg_stream(src + v * 8));
+  }
+}
+
 }  // namespace lv
 
 using namespace lv;
@@ -891,6 +1117,104 @@ int lv_ce_grad(const void* logits, int64_t ld, void* dlogits, int64_t ldd, const
   ce_grad_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, (cudaStream_t)stream>>>(BF(logits), ld, BFM(dlogits), ldd, labels, lse,
                                                                                             dloss, rows, (int)cols, col0);
   LV_CHECK_LAUNCH("ce_grad_kernel");
+  return LV_OK;
+}
+
+int64_t lv_layernorm_bwd_partials(int64_t rows, int64_t cols) {
+  // rows of each partial buffer the kernel writes: gridDim * rows-per-CTA (same TPR choice as the launch below)
+  const int64_t nvec = cols / 8;
+  const int tpr = nvec <= 32 * 4 ? 32 : (nvec <= 128 * 4 ? 128 : 256);
+  const int64_t rpc = 256 / tpr;
+  int64_t grid = (rows + rpc - 1) / rpc;
+  const int64_t cap = 2 * (int64_t)lv::sm_count();
+  if (grid > cap) grid = cap;
+  if (grid < 1) grid = 1;
+  return grid * rpc;
+}
+
+int lv_layernorm_bwd(const void* x, const void* w, const void* dy, const void* add_in, void* dx, float* dw_partials,
+                     float* db_partials, int64_t rows, int64_t cols, float eps, lv_stream_t stream) {
+  LV_CHECK_ARG(x && w && dy && dw_partials && db_partials, "lv_layernorm_bwd: null pointer");
+  LV_CHECK_ARG(dx != nullptr || add_in == nullptr, "lv_layernorm_bwd: add_in needs dx");
+  LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0 && cols <= 8192, "lv_layernorm_bwd: cols=%lld must be a multiple of 8 and <= 8192", (long long)cols);
+  LV_CHECK_ARG(aligned16(x) && aligned16(w) && aligned16(dy) && aligned16(dx) && aligned16(add_in) && aligned16(dw_partials) &&
+                   aligned16(db_partials), "lv_layernorm_bwd: pointers must be 16-byte aligned");
+  LV_BIND_DEVICE(x);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t parts = lv_layernorm_bwd_partials(rows, cols);
+  if (rows == 0) {
+    LV_CHECK_CUDA(cudaMemsetAsync(dw_partials, 0, (size_t)parts * cols * 4, s));
+    LV_CHECK_CUDA(cudaMemsetAsync(db_partials, 0, (size_t)parts * cols * 4, s));
+    return LV_OK;
+  }
+  const int nvec = (int)(cols / 8);
+#define LAUNCH_LNB(TPR, VPT)                                                                                  \
+  layernorm_bwd_kernel<TPR, VPT><<<(unsigned)(parts / (256 / TPR)), 256, 0, s>>>(                             \
+      BF(x), BF(w), BF(dy), BF(add_in), BFM(dx), dw_partials, db_partials, rows, (int)cols, eps)
+  if (nvec <= 32 * 4)
+    LAUNCH_LNB(32, 4);
+  else if (nvec <= 128 * 4)
+    LAUNCH_LNB(128, 4);
+  else
+    LAUNCH_LNB(256, 4);
+#undef LAUNCH_LNB
+  LV_CHECK_LAUNCH("layernorm_bwd_kernel");
+  return LV_OK;
+}
+
+int lv_gelu_bwd(const void* pre, const void* dy, void* dx, int64_t rows, int64_t cols, int32_t approx, lv_stream_t stream) {
+  LV_CHECK_ARG(pre && dy && dx, "lv_gelu_bwd: null pointer");
+  LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0, "lv_gelu_bwd: cols=%lld must be a multiple of 8", (long long)cols);
+  LV_CHECK_ARG(approx == 0 || approx == 1, "lv_gelu_bwd: approx=%d must be 0 (erf) or 1 (tanh)", approx);
+  LV_CHECK_ARG(aligned16(pre) && aligned16(dy) && aligned16(dx), "lv_gelu_bwd: pointers must be 16-byte aligned");
+  if (rows == 0) return LV_OK;
+  LV_BIND_DEVICE(pre);
+  const int64_t total = rows * (cols / 8);
+  gelu_bwd_kernel<<<(unsigned)cdiv(total, 256), 256, 0, (cudaStream_t)stream>>>(BF(pre), BF(dy), BFM(dx), total, approx);
+  LV_CHECK_LAUNCH("gelu_bwd_kernel");
+  return LV_OK;
+}
+
+int64_t lv_ls_residual_bwd_partials(int64_t rows, int64_t cols) {
+  // rows of dls_partials the kernel writes (gridDim.y of the launch below): ~2 CTAs per SM, at least one row lane each
+  const int64_t gx = cdiv(cols, 256);
+  int64_t gy = 2 * (int64_t)lv::sm_count() / (gx > 0 ? gx : 1);
+  const int64_t need = cdiv(rows, LSB_ROWS);
+  if (gy > need) gy = need;
+  if (gy > 65535) gy = 65535;
+  if (gy < 1) gy = 1;
+  return gy;
+}
+
+int lv_ls_residual_bwd(const void* dout, const void* y, const void* ls, void* dy, float* dls_partials, int64_t rows,
+                       int64_t cols, lv_stream_t stream) {
+  LV_CHECK_ARG(dout && y && ls && dy && dls_partials, "lv_ls_residual_bwd: null pointer");
+  LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0, "lv_ls_residual_bwd: cols=%lld must be a multiple of 8", (long long)cols);
+  LV_CHECK_ARG(aligned16(dout) && aligned16(y) && aligned16(ls) && aligned16(dy) && aligned16(dls_partials),
+               "lv_ls_residual_bwd: pointers must be 16-byte aligned");
+  LV_BIND_DEVICE(dout);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t gy = lv_ls_residual_bwd_partials(rows, cols);
+  if (rows == 0) {
+    LV_CHECK_CUDA(cudaMemsetAsync(dls_partials, 0, (size_t)gy * cols * 4, s));
+    return LV_OK;
+  }
+  const dim3 grid((unsigned)cdiv(cols, 256), (unsigned)gy);
+  ls_residual_bwd_kernel<<<grid, 256, 0, s>>>(BF(dout), BF(y), BF(ls), BFM(dy), dls_partials, rows, (int)cols);
+  LV_CHECK_LAUNCH("ls_residual_bwd_kernel");
+  return LV_OK;
+}
+
+int lv_pixel_shuffle_bwd(const void* dout, void* dx, int64_t n, int64_t hw, int64_t c, int32_t has_cls, lv_stream_t stream) {
+  LV_CHECK_ARG(dout && dx, "lv_pixel_shuffle_bwd: null pointer");
+  LV_CHECK_ARG(n >= 0 && hw > 0 && hw % 2 == 0 && c > 0 && c % 8 == 0, "lv_pixel_shuffle_bwd: hw=%lld must be even, c=%lld a multiple of 8", (long long)hw, (long long)c);
+  LV_CHECK_ARG(aligned16(dout) && aligned16(dx), "lv_pixel_shuffle_bwd: pointers must be 16-byte aligned");
+  if (n == 0) return LV_OK;
+  const int64_t blocks = n * (hw / 2) * (hw / 2) + (has_cls ? n : 0);
+  LV_CHECK_ARG(blocks < (1ll << 31), "lv_pixel_shuffle_bwd: too many tokens");
+  LV_BIND_DEVICE(dout);
+  pixel_shuffle_bwd_kernel<<<(unsigned)blocks, 128, 0, (cudaStream_t)stream>>>(BF(dout), BFM(dx), n, (int)hw, (int)c, has_cls);
+  LV_CHECK_LAUNCH("pixel_shuffle_bwd_kernel");
   return LV_OK;
 }
 

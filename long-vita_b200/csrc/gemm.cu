@@ -476,4 +476,21 @@ int lv_patch_embed(const void* images, const void* W, const void* bias, const vo
   return LV_OK;
 }
 
+int lv_patch_im2col(const void* images, void* col, int64_t n, int64_t img, int64_t ps, int64_t kpad, lv_stream_t stream) {
+  LV_CHECK_ARG(images && col, "lv_patch_im2col: null pointer");
+  LV_CHECK_ARG(n >= 0 && img > 0 && ps > 0 && img % ps == 0, "lv_patch_im2col: bad geometry img=%lld ps=%lld", (long long)img, (long long)ps);
+  LV_CHECK_ARG(kpad >= 3 * ps * ps && kpad % 8 == 0 && kpad < (1ll << 31), "lv_patch_im2col: kpad=%lld must be a multiple of 8 and >= 3*ps*ps", (long long)kpad);
+  LV_CHECK_ARG((reinterpret_cast<uintptr_t>(images) & 15) == 0 && (reinterpret_cast<uintptr_t>(col) & 15) == 0,
+               "lv_patch_im2col: pointers must be 16-byte aligned");
+  if (n == 0) return LV_OK;
+  const int64_t P = (img / ps) * (img / ps);
+  LV_CHECK_ARG(n * P < (1ll << 31), "lv_patch_im2col: too many patches");
+  LV_BIND_DEVICE(images);
+  im2col_patch_kernel<<<(unsigned)(n * P), 128, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16*>(images),
+                                                                         reinterpret_cast<__nv_bfloat16*>(col), n, (int)img,
+                                                                         (int)ps, (int)kpad);
+  LV_CHECK_LAUNCH("im2col_patch_kernel");
+  return LV_OK;
+}
+
 }  // extern "C"

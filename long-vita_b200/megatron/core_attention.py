@@ -176,14 +176,42 @@ def b200_dot_product_attention_forward_wrapper(fn):
     return wrapper
 
 
-def register_b200_patches(patches_manager=None) -> None:
+def b200_gpt_vl_model_init_wrapper(orig_init):
+    """Decorates `GPTVLModel.__init__` (long_vita_megatron/core/models/multimodal/gpt_vl_model.py:72-114) so that the
+    reference's stock `vision_model_provider` (pretrain_long_vita.py:599-601, handed over as
+    `external_feature_model_provider` at :641-655) is replaced by `b200_vision_model_provider` at the moment the model
+    is built.  Patching the class rather than the provider's module-level name works however the training script is
+    started: `torchrun pretrain_long_vita.py` runs it as `__main__`, whose own copy of the function `model_provider`
+    passes, and a second import of `long_vita_megatron.pretrain_long_vita` would be a different function object.
+    Any other provider (a caller's own, or None) is passed through unchanged."""
+    from .vision_model import b200_vision_model_provider
+
+    @wraps(orig_init)
+    def __init__(self, *args, **kwargs):
+        prov = kwargs.get("external_feature_model_provider")
+        if prov is not None and getattr(prov, "__name__", "") == "vision_model_provider":
+            kwargs["external_feature_model_provider"] = b200_vision_model_provider
+        return orig_init(self, *args, **kwargs)
+
+    return __init__
+
+
+def register_b200_patches(patches_manager=None, vision_model: bool = False) -> None:
     """Register + apply the attention patch through the reference's own registry
     (long_vita_megatron/patch_utils.py:105-118).  Call after importing
-    long_vita_megatron.megatron_adaptor."""
+    long_vita_megatron.megatron_adaptor.
+
+    `vision_model=True` also builds the vision side (InternViT-300M + projector) as `B200VisionModel`, forward and
+    backward on the fused kernels (`b200_gpt_vl_model_init_wrapper`).  It is opt-in: the provider refuses
+    configurations it does not implement (tensor parallelism > 1, recompute, vision context parallelism, other towers),
+    and with the whole tower trained its backward is currently slower than the stock modules (DESIGN.md §8)."""
     if patches_manager is None:
         from long_vita_megatron.patch_utils import MindSpeedPatchesManager as patches_manager  # noqa: N813
     patches_manager.register_patch(
         "megatron.core.transformer.dot_product_attention.DotProductAttention.forward",
         b200_dot_product_attention_forward_wrapper,
     )
+    if vision_model:
+        patches_manager.register_patch("long_vita_megatron.core.models.multimodal.gpt_vl_model.GPTVLModel.__init__",
+                                       b200_gpt_vl_model_init_wrapper)
     patches_manager.apply_patches()

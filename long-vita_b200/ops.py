@@ -278,9 +278,20 @@ def _fill_attn_params(p, qv, kv_, vv, ov, lse, scale, causal, q_seg_len, q_seg_p
 
 
 def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[float] = None, q_seg_len=None,
-                  q_seg_pos=None, kv_pos0: int = 0, cu_seqlens: Optional[torch.Tensor] = None):
+                  q_seg_pos=None, kv_pos0: int = 0, cu_seqlens: Optional[torch.Tensor] = None,
+                  dq: Optional[torch.Tensor] = None, dk: Optional[torch.Tensor] = None, dv: Optional[torch.Tensor] = None):
     """Gradients of attention_fwd (layout "bshd").  `out` / `lse` are the forward results, `cu_seqlens` the packed
-    documents the forward was called with.  Returns (dq, dk, dv) with the shapes of q, k, v."""
+    documents the forward was called with.  Returns (dq, dk, dv) with the shapes of q, k, v.  `dq` / `dk` / `dv`, all
+    three or none, are caller buffers (strided views are fine, e.g. the per-head q / k / v columns of one dQKV buffer
+    laid out like the fused QKV GEMM output) that the kernel writes through their strides."""
+    if (dq is None) != (dk is None) or (dq is None) != (dv is None):
+        raise ValueError("attention_bwd: pass all of dq, dk, dv or none")
+    if dq is not None:
+        _need_cuda_bf16(dq, dk, dv)
+        for t, ref in ((dq, q), (dk, k), (dv, v)):
+            if t.shape != ref.shape or t.stride(3) != 1 or any(s % 8 for s in t.stride()[:3]):
+                raise ValueError("attention_bwd: dq / dk / dv must have the shapes of q / k / v, a contiguous head dimension "
+                                 "and strides that are multiples of 8 elements")
     _need_cuda_bf16(d_out, q, k, v, out)
     _need_cuda(lse, torch.float32)
     docs = None
@@ -292,8 +303,9 @@ def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[flo
         return t if (t.stride(3) == 1 and all(s % 8 == 0 for s in t.stride()[:3])) else t.contiguous()
 
     q, k, v, out, d_out = fix(q), fix(k), fix(v), fix(out), fix(d_out)
-    dq, dk, dv = torch.empty_like(q, memory_format=torch.contiguous_format), \
-        torch.empty_like(k, memory_format=torch.contiguous_format), torch.empty_like(v, memory_format=torch.contiguous_format)
+    if dq is None:
+        dq, dk, dv = torch.empty_like(q, memory_format=torch.contiguous_format), \
+            torch.empty_like(k, memory_format=torch.contiguous_format), torch.empty_like(v, memory_format=torch.contiguous_format)
     b, sq, hq, _ = q.shape
     delta = torch.empty((b, hq, sq), dtype=torch.float32, device=q.device)
     p = AttnBwdParams()
@@ -914,16 +926,23 @@ class _LinearFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = linear(dy2, weight.t().contiguous()).view(x.shape)          # [T, K] = dY [T, N] . (W^T)[K, N]^T
         if ctx.needs_input_grad[1]:
-            t = dy2.shape[0]
-            tp = (t + 7) // 8 * 8
-            dyt = torch.zeros((n_out, tp), dtype=torch.bfloat16, device=dy.device)
-            dyt[:, :t] = dy2.t()
-            xt = torch.zeros((k_in, tp), dtype=torch.bfloat16, device=dy.device)
-            xt[:, :t] = x2.t()
-            dw = linear(dyt, xt)                                             # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
+            dw = linear_wgrad(dy2, x2)
         if ctx.has_bias and ctx.needs_input_grad[2]:
-            db = dy2.float().sum(dim=0).to(torch.bfloat16)
+            db = dy2.float().sum(dim=0).to(dy2.dtype)
         return dx, dw, db
+
+
+def linear_wgrad(dy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
+    """dW [N, K] = dY^T [N, T] . X [T, K] on the wgmma GEMM: both operands are transposed once so that the token
+    dimension T is the contraction, zero-padded to a multiple of 8 (the GEMM's K granularity)."""
+    t, n_out = dy2.shape
+    k_in = x2.shape[1]
+    tp = (t + 7) // 8 * 8
+    dyt = torch.zeros((n_out, tp), dtype=dy2.dtype, device=dy2.device)
+    dyt[:, :t] = dy2.t()
+    xt = torch.zeros((k_in, tp), dtype=x2.dtype, device=x2.device)
+    xt[:, :t] = x2.t()
+    return linear(dyt, xt)                                                   # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
 
 
 def linear_autograd(x, weight, bias=None):
@@ -960,3 +979,235 @@ def pad_patch_weight(conv_weight: torch.Tensor) -> torch.Tensor:
     out = torch.zeros((Cc, kpad), dtype=conv_weight.dtype, device=conv_weight.device)
     out[:, :k] = flat
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# differentiable building blocks of the vision tower and the projector (training InternViT through
+# MegatronVisionModel, pretrain_long_vita.py:310-596).  Each backward is a kernel of liblvb200.so; the per-column
+# gradients (LayerNorm weight / bias, layer scale) come back as fp32 partial rows that are added here, and the
+# bias-like sums (conv bias, class token, position embedding, linear bias) are fp32 sums over tokens, as in
+# _LinearFn.
+# ------------------------------------------------------------------------------------------------
+def layernorm_bwd(x: torch.Tensor, weight: torch.Tensor, dy: torch.Tensor, eps: float = 1e-6,
+                  add_in: Optional[torch.Tensor] = None, need_dx: bool = True):
+    """Gradients of layernorm(x, weight, bias): returns (dx [+ add_in], dweight, dbias); dx is None (and not computed)
+    with need_dx=False."""
+    if not need_dx and add_in is not None:
+        raise ValueError("layernorm_bwd: add_in needs dx")
+    _need_cuda_bf16(x, weight, dy, add_in)
+    cols = x.shape[-1]
+    x2, dy2 = x.reshape(-1, cols).contiguous(), dy.reshape(-1, cols).contiguous()
+    a2 = None if add_in is None else add_in.reshape(-1, cols).contiguous()
+    rows = x2.shape[0]
+    parts = int(_lib.lib().lv_layernorm_bwd_partials(rows, cols))
+    dw_part = torch.empty((parts, cols), dtype=torch.float32, device=x.device)
+    db_part = torch.empty((parts, cols), dtype=torch.float32, device=x.device)
+    dx = torch.empty_like(x2) if need_dx else None
+    _lib.check(_lib.lib().lv_layernorm_bwd(x2.data_ptr(), weight.data_ptr(), dy2.data_ptr(), _ptr(a2), _ptr(dx),
+                                           dw_part.data_ptr(), db_part.data_ptr(), rows, cols, float(eps), _stream()),
+               "lv_layernorm_bwd")
+    return (None if dx is None else dx.view(x.shape)), dw_part.sum(dim=0).to(torch.bfloat16), db_part.sum(dim=0).to(torch.bfloat16)
+
+
+def gelu_bwd(pre: torch.Tensor, dy: torch.Tensor, approximate: str = "none"):
+    """dx = dy * gelu'(pre); `approximate` as in bias_gelu ("none" = erf, "tanh")."""
+    _need_cuda_bf16(pre, dy)
+    cols = pre.shape[-1]
+    p2, d2 = pre.reshape(-1, cols).contiguous(), dy.reshape(-1, cols).contiguous()
+    dx = torch.empty_like(p2)
+    _lib.check(_lib.lib().lv_gelu_bwd(p2.data_ptr(), d2.data_ptr(), dx.data_ptr(), p2.shape[0], cols,
+                                      1 if approximate == "tanh" else 0, _stream()), "lv_gelu_bwd")
+    return dx.view(pre.shape)
+
+
+def ls_residual_bwd(dout: torch.Tensor, y: torch.Tensor, ls: torch.Tensor):
+    """Gradients of ls_residual(x, y, ls) (no bias) with respect to y and ls: (bf16(dout * ls), sum_rows dout * y).
+    The gradient of x is dout itself."""
+    _need_cuda_bf16(dout, y, ls)
+    cols = y.shape[-1]
+    d2, y2 = dout.reshape(-1, cols).contiguous(), y.reshape(-1, cols).contiguous()
+    rows = y2.shape[0]
+    parts = int(_lib.lib().lv_ls_residual_bwd_partials(rows, cols))
+    dls_part = torch.empty((parts, cols), dtype=torch.float32, device=y.device)
+    dy = torch.empty_like(y2)
+    _lib.check(_lib.lib().lv_ls_residual_bwd(d2.data_ptr(), y2.data_ptr(), ls.contiguous().data_ptr(), dy.data_ptr(),
+                                             dls_part.data_ptr(), rows, cols, _stream()), "lv_ls_residual_bwd")
+    return dy.view(y.shape), dls_part.sum(dim=0).to(torch.bfloat16)
+
+
+def pixel_shuffle_bwd(dout: torch.Tensor, hw: int, has_cls: bool):
+    """[n, (hw/2)^2, 4c] -> [n, (1 +) hw*hw, c]: the inverse permutation of pixel_shuffle (class-token rows zero)."""
+    _need_cuda_bf16(dout)
+    dout = dout.contiguous()
+    n, _, c4 = dout.shape
+    c = c4 // 4
+    dx = torch.empty((n, hw * hw + (1 if has_cls else 0), c), dtype=torch.bfloat16, device=dout.device)
+    _lib.check(_lib.lib().lv_pixel_shuffle_bwd(dout.data_ptr(), dx.data_ptr(), n, hw, c, 1 if has_cls else 0, _stream()),
+               "lv_pixel_shuffle_bwd")
+    return dx
+
+
+def patch_im2col(images: torch.Tensor, patch: int, kpad: int):
+    """images [n, 3, S, S] -> col [n * (S/patch)^2, kpad]: each patch's pixels in (channel, y, x) order, zero-padded."""
+    _need_cuda_bf16(images)
+    images = images.contiguous()
+    n, _, size, _ = images.shape
+    col = torch.empty((n * (size // patch) ** 2, kpad), dtype=torch.bfloat16, device=images.device)
+    _lib.check(_lib.lib().lv_patch_im2col(images.data_ptr(), col.data_ptr(), n, size, patch, kpad, _stream()),
+               "lv_patch_im2col")
+    return col
+
+
+class _LayerNormFn(torch.autograd.Function):
+    """y = layernorm(x).  With `passthrough`, also returns x itself as the residual stream: the gradient arriving on
+    that second output is added to dx inside the backward kernel (`add_in`), so the residual branch of a pre-norm
+    block costs no separate add."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, eps, passthrough):
+        ctx.save_for_backward(x, weight)
+        ctx.eps, ctx.passthrough = eps, passthrough
+        y = layernorm(x, weight, bias, eps)
+        return (y, x.view_as(x)) if passthrough else y
+
+    @staticmethod
+    def backward(ctx, dy, ds=None):
+        x, weight = ctx.saved_tensors
+        need_dx = ctx.needs_input_grad[0]
+        dx, dw, db = layernorm_bwd(x, weight, dy.contiguous(), ctx.eps, add_in=ds if ctx.passthrough and need_dx else None,
+                                   need_dx=need_dx)
+        return dx, dw, db, None, None
+
+
+def layernorm_autograd(x, weight, bias, eps: float = 1e-6, passthrough: bool = False):
+    """Differentiable LayerNorm over the last dim; `passthrough=True` returns (y, x) (see _LayerNormFn)."""
+    return _LayerNormFn.apply(x, weight, bias, eps, passthrough)
+
+
+class _GeluFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pre, approximate):
+        ctx.save_for_backward(pre)
+        ctx.approximate = approximate
+        return bias_gelu(pre, None, approximate)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (pre,) = ctx.saved_tensors
+        return gelu_bwd(pre, dy.contiguous(), ctx.approximate), None
+
+
+def gelu_autograd(pre, approximate: str = "none"):
+    """gelu(pre) keeping the bf16 pre-activation for the backward (fc1 runs with act = 0 before it in training)."""
+    return _GeluFn.apply(pre, approximate)
+
+
+class _LSResidualFn(torch.autograd.Function):
+    """out = x + y * ls (bias-free; the ViT adds its biases in the GEMM epilogue)."""
+
+    @staticmethod
+    def forward(ctx, x, y, ls):
+        ctx.save_for_backward(y, ls)
+        return ls_residual(x, y, ls)
+
+    @staticmethod
+    def backward(ctx, dout):
+        y, ls = ctx.saved_tensors
+        dout = dout.contiguous()
+        dy = dls = None
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            dy, dls = ls_residual_bwd(dout, y, ls)
+        return dout, dy, dls
+
+
+def ls_residual_autograd(x, y, ls):
+    return _LSResidualFn.apply(x, y, ls)
+
+
+class _PixelShuffleFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, hw, has_cls):
+        ctx.hw, ctx.has_cls = hw, has_cls
+        return pixel_shuffle(x, hw, has_cls)
+
+    @staticmethod
+    def backward(ctx, dout):
+        return pixel_shuffle_bwd(dout, ctx.hw, ctx.has_cls), None, None
+
+
+def pixel_shuffle_autograd(x, hw: int, has_cls: bool):
+    """Differentiable drop-cls + pixel-shuffle x0.5 ([n, (1 +) hw*hw, c] -> [n, (hw/2)^2, 4c])."""
+    return _PixelShuffleFn.apply(x, hw, has_cls)
+
+
+class _PatchEmbedFn(torch.autograd.Function):
+    """out = cat(cls, conv(images)) + pos.  Saves only the images (the im2col matrix is rebuilt in the backward);
+    the conv weight gradient is dW[C, Kpad] = dP^T . col on the wgmma GEMM, with the padding columns dropped."""
+
+    @staticmethod
+    def forward(ctx, images, conv_w, conv_b, cls, pos, patch):
+        w_pad = pad_patch_weight(conv_w)
+        ctx.save_for_backward(images)
+        ctx.patch, ctx.kpad, ctx.w_shape = patch, w_pad.shape[1], conv_w.shape
+        ctx.cls_shape, ctx.pos_shape = cls.shape, pos.shape
+        return patch_embed(images, w_pad, conv_b, cls.reshape(-1), pos, patch)
+
+    @staticmethod
+    def backward(ctx, dout):
+        (images,) = ctx.saved_tensors
+        n, s, c = dout.shape
+        d = dout.contiguous()
+        dw = db = dcls = dpos = None
+        dp = d[:, 1:].reshape(n * (s - 1), c)
+        if ctx.needs_input_grad[1]:
+            col = patch_im2col(images, ctx.patch, ctx.kpad)
+            k = ctx.w_shape[1] * ctx.w_shape[2] * ctx.w_shape[3]
+            dw = linear_wgrad(dp, col)[:, :k].reshape(ctx.w_shape)
+        if ctx.needs_input_grad[2]:
+            db = dp.float().sum(dim=0).to(d.dtype)
+        if ctx.needs_input_grad[3]:
+            dcls = d[:, 0].float().sum(dim=0).to(d.dtype).reshape(ctx.cls_shape)
+        if ctx.needs_input_grad[4]:
+            dpos = d.float().sum(dim=0).to(d.dtype).reshape(ctx.pos_shape)
+        return None, dw, db, dcls, dpos, None
+
+
+def patch_embed_autograd(images, conv_w, conv_b, cls, pos, patch: int):
+    """Differentiable InternViT embedding: images [n, 3, S, S], conv_w [C, 3, patch, patch], conv_b [C], cls (C
+    elements, e.g. [1, 1, C]), pos [1 + (S/patch)^2, C] -> [n, 1 + (S/patch)^2, C].  Gradients: conv weight, conv bias,
+    class token (sum over frames of row 0), position embedding (sum over frames); none for the images."""
+    return _PatchEmbedFn.apply(images, conv_w, conv_b, cls, pos, patch)
+
+
+class _ViTAttentionFn(torch.autograd.Function):
+    """Non-causal attention over the output of the fused QKV GEMM, qkv [n, S, 3C] with Megatron's per-head row
+    interleave [H, (q, k, v), D]: q / k / v are strided views of it in both directions, and the backward writes dQ / dK
+    / dV through the same strides into one dQKV buffer that is the gradient of qkv (no re-layout, no stacking)."""
+
+    @staticmethod
+    def forward(ctx, qkv, heads, scale):
+        n, s, c3 = qkv.shape
+        d = c3 // (3 * heads)
+        v5 = qkv.view(n, s, heads, 3, d)
+        out, lse = attention_fwd(v5[:, :, :, 0], v5[:, :, :, 1], v5[:, :, :, 2], causal=False, scale=scale, return_lse=True)
+        ctx.save_for_backward(qkv, out, lse)
+        ctx.heads, ctx.scale = heads, scale
+        return out.view(n, s, heads * d)
+
+    @staticmethod
+    def backward(ctx, d_out):
+        qkv, out, lse = ctx.saved_tensors
+        n, s, c3 = qkv.shape
+        h = ctx.heads
+        d = c3 // (3 * h)
+        v5 = qkv.view(n, s, h, 3, d)
+        dqkv = torch.empty_like(qkv)
+        g5 = dqkv.view(n, s, h, 3, d)
+        attention_bwd(d_out.reshape(n, s, h, d).contiguous(), v5[:, :, :, 0], v5[:, :, :, 1], v5[:, :, :, 2], out, lse,
+                      causal=False, scale=ctx.scale, dq=g5[:, :, :, 0], dk=g5[:, :, :, 1], dv=g5[:, :, :, 2])
+        return dqkv, None, None
+
+
+def vit_attention(qkv, heads: int, scale: Optional[float] = None):
+    """Differentiable ViT self-attention on qkv [n, S, 3C] ([H, 3, D] columns) -> [n, S, C] (see _ViTAttentionFn)."""
+    return _ViTAttentionFn.apply(qkv, heads, scale)
