@@ -297,8 +297,8 @@ class CPContext(CPBackwardMixin):
         optional) receives the log-sum-exp.  Packed documents (`cu_seqlens`) raise NotImplementedError."""
         _refuse_packing(cu_seqlens)
         assert self.fused_qkv
-        buf = self.qkv[self.epoch & 1]
-        return self._launch(buf.data_ptr(), (self.T * self.row, self.row, self.d), out, scale, lse)
+        q = self.qkv[self.epoch & 1][:, : self.hq * self.d].view(self.T, self.hq, self.d)
+        return self._launch(q, out, scale, lse)
 
     def attention_separate(self, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out=None, scale=None,
                            return_lse: bool = False, cu_seqlens=None):
@@ -311,33 +311,25 @@ class CPContext(CPBackwardMixin):
         buf = self.qkv[self.epoch & 1].view(self.T, 2, self.hkv, self.d)
         buf[:, 0].copy_(k)
         buf[:, 1].copy_(v)
-        if q.stride(2) != 1 or q.stride(0) % 8 or q.stride(1) % 8:
-            q = q.contiguous()
+        from . import ops
+
         lse = torch.empty((1, self.hq, self.T), dtype=torch.float32, device=self.device) if return_lse else None
-        o = self._launch(q.data_ptr(), (self.T * q.stride(0), q.stride(0), q.stride(1)), out, scale, lse)
+        o = self._launch(ops.tma_view(q), out, scale, lse)
         return (o, lse) if return_lse else o
 
-    def _launch(self, q_ptr, q_strides, out, scale, lse=None):
-        from ._lib import AttnParams, CpParams
+    def _launch(self, q, out, scale, lse=None):
+        """q [T, hq, d]: this rank's queries, read in place.  K/V are the global-order staging buffers the kernel fills."""
+        from . import ops
+        from ._lib import CpParams
 
         T, hq, hkv, d = self.T, self.hq, self.hkv, self.d
         par = self.epoch & 1
         if out is None:
             out = torch.empty((T, hq * d), dtype=torch.bfloat16, device=self.device)
         c = self.S // (2 * self.cp)
-        a = AttnParams()
-        a.q, a.k, a.v, a.out = q_ptr, self.k_full.data_ptr(), self.v_full.data_ptr(), out.data_ptr()
-        a.lse = None if lse is None else lse.data_ptr()
-        a.batch, a.sq, a.sk, a.hq, a.hkv, a.d = 1, T, self.S, hq, hkv, d
-        a.q_strides[0], a.q_strides[1], a.q_strides[2] = q_strides
-        for arr in (a.k_strides, a.v_strides):
-            arr[0], arr[1], arr[2] = self.S * hkv * d, hkv * d, d
-        a.o_strides[0], a.o_strides[1], a.o_strides[2] = T * hq * d, hq * d, d
-        a.scale = float(scale if scale is not None else 1.0 / math.sqrt(d))
-        a.causal = 1
-        a.q_seg_len = c
-        a.q_seg_pos[0], a.q_seg_pos[1] = self.rank * c, (2 * self.cp - 1 - self.rank) * c
-        a.kv_pos0 = 0
+        a = ops.attn_params(q.unsqueeze(0), self.k_full.view(1, self.S, hkv, d), self.v_full.view(1, self.S, hkv, d),
+                            out.view(1, T, hq, d), lse, scale=scale, causal=True, q_seg_len=c,
+                            q_seg_pos=(self.rank * c, (2 * self.cp - 1 - self.rank) * c))
         cpp = CpParams()
         cpp.rank, cpp.cp, cpp.seq_total, cpp.epoch = self.rank, self.cp, self.S, self.epoch
         cpp.peer_tok_stride = self.row
@@ -348,8 +340,6 @@ class CPContext(CPBackwardMixin):
         cpp.my_ready = self.ready_ptr
         cpp.k_full, cpp.v_full, cpp.blk_flags = self.k_full.data_ptr(), self.v_full.data_ptr(), self.blk_flags.data_ptr()
         cpp.fault = self.fault.data_ptr()
-        from . import ops
-
         ev0 = ops._TIMER.start() if ops._TIMER is not None else None
         self._check(self.lib.lv_attn_cp_fwd(C.byref(a), C.byref(cpp), torch.cuda.current_stream().cuda_stream),
                     "lv_attn_cp_fwd")
@@ -362,6 +352,18 @@ class CPContext(CPBackwardMixin):
 # ------------------------------------------------------------------------------------------------
 # sharded prefill
 # ------------------------------------------------------------------------------------------------
+def exchange_attention(ctx, cache=None):
+    """Attention step (hf.modeling.run_layers) of a decoder layer on this rank's zig-zag shard: the QKV GEMM wrote
+    into `ctx.qkv_buffer()` and RoPE ran in place there; the fused kernel pulls the other ranks' K/V itself
+    (lv_attn_cp_fwd).  With `cache`, this rank's rows become its shard of the K/V cache."""
+    def attend(li, q, k, v):
+        if cache is not None:
+            cache.append(li, k, v)
+        return ctx.attention()
+
+    return attend
+
+
 class ContextParallelRunner:
     """LongVITAForCausalLM prefill with the sequence sharded zig-zag over the ranks of `group`."""
 
@@ -393,6 +395,7 @@ class ContextParallelRunner:
         """Every rank passes the FULL prompt (the reference broadcasts it, tasks/inference/module.py
         :340-356) and keeps its shard.  Returns the last-token logits [1, 1, vocab] on every rank."""
         from . import ops
+        from .hf.modeling import run_layers
 
         m = self.model.model
         cfg = self.model.config
@@ -413,12 +416,8 @@ class ContextParallelRunner:
 
             self.cache = KVCache(len(m.layers), T + -(-max_new_tokens // self.cp) + 1, cfg.num_key_value_heads, cfg.head_dim, dev)
             self.total_len = S
-        delta = None
-        for li, layer in enumerate(m.layers):
-            x, delta = layer.forward_cp(x, delta, cos, sin, ctx, self.cache, li)
-        if self.cache is not None:
-            self.cache.commit()
-        h, _ = ops.rmsnorm(delta, m.norm_w, cfg.rms_norm_eps, residual=x)
+        h = run_layers(m.layers, x, cos, sin, exchange_attention(ctx, self.cache), m.norm_w, cfg.rms_norm_eps,
+                       cache=self.cache, qkv_out=ctx.qkv_buffer)
         # logit mask: each rank projects its own last row; the globally-last token lives on rank 0
         # (chunk 2cp-1), generation.py:141-165
         row = sh.last_token_local if sh.last_token_local >= 0 else T - 1
@@ -441,23 +440,43 @@ class ContextParallelRunner:
         w = torch.softmax(allp[:, :, d], dim=0)                   # -inf (empty shard) -> weight 0
         return (allp[:, :, :d] * w.unsqueeze(-1)).sum(dim=0).to(torch.bfloat16)
 
+    def _shard_attention(self, append: bool):
+        """Attention step of one decoded token over the sharded cache (any split of the keys works for a query that
+        sees them all): this rank attends over its shard, `_merge` combines the ranks' (out, lse) pairs.  Only the rank
+        that owns the new position (`append`) adds its K/V row."""
+        from . import ops
+
+        cache = self.cache
+
+        def attend(li, q, k, v):
+            if append:
+                kc, vc, length = cache.append(li, k, v)
+            else:
+                kc, vc, length = cache.k[li], cache.v[li], len(cache)
+            if length > 0:
+                o_loc, lse_loc = ops.attention_decode(q[0], kc, vc, length, return_lse=True)
+            else:
+                hq, d = q.shape[1], q.shape[2]
+                o_loc = torch.zeros((hq, d), dtype=torch.bfloat16, device=q.device)
+                lse_loc = torch.full((hq,), float("-inf"), dtype=torch.float32, device=q.device)
+            return self._merge(o_loc, lse_loc)
+
+        return attend
+
     def decode(self, token: torch.Tensor) -> torch.Tensor:
         """One generated token after forward(..., use_cache=True): every rank runs the token through the
         (replicated) weights; attention reads only this rank's cache shard and the partial results are merged.
         The new K/V row goes to rank `position % cp`.  Returns the logits [1, 1, vocab] (same on every rank)."""
         from . import ops
+        from .hf.modeling import run_layers
 
         m = self.model.model
         cfg = self.model.config
         assert self.cache is not None, "call forward(..., use_cache=True) first"
         pos = self.total_len
-        owner = (pos % self.cp) == self.rank
         x = ops.embed_scatter(token.view(1, 1), m.embed_tokens)
         cos, sin = ops.rope_table(torch.tensor([pos], dtype=torch.int64, device=x.device), m.inv_freq)
-        delta = None
-        for li, layer in enumerate(m.layers):
-            x, delta = layer.forward(x, delta, cos, sin, {}, self.cache, li, shard_merge=self._merge, append=owner)
-        self.cache.commit()
+        h = run_layers(m.layers, x, cos, sin, self._shard_attention((pos % self.cp) == self.rank), m.norm_w,
+                       cfg.rms_norm_eps, cache=self.cache)
         self.total_len += 1
-        h, _ = ops.rmsnorm(delta, m.norm_w, cfg.rms_norm_eps, residual=x)
         return ops.linear(h, self.model.lm_head).view(1, 1, -1)

@@ -16,7 +16,8 @@ every token (long_vita_megatron/inference/text_generation/generation.py:127-135)
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from functools import partial
+from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
 
@@ -133,11 +134,15 @@ class DecoderLayer:
         self.ln1 = w[p + "input_layernorm.weight"]
         self.ln2 = w[p + "post_attention_layernorm.weight"]
 
-    def forward(self, x: torch.Tensor, delta: Optional[torch.Tensor], cos, sin, attn_kwargs, cache=None,
-                layer_idx: int = 0, shard_merge=None, append: bool = True) -> Tuple[torch.Tensor, torch.Tensor]:
-        """x [T, H] residual stream, `delta` the previous layer's MLP output not yet added
-        (the add is fused into this layer's first RMSNorm).  Returns (x, delta).  With `cache` the new
-        K/V rows are appended to it and attention runs over cache + new rows."""
+    def forward(self, x: torch.Tensor, delta: Optional[torch.Tensor], cos, sin, attend,
+                qkv_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """x [T, H] residual stream, `delta` the previous layer's MLP output not yet added (the add is fused into this
+        layer's first RMSNorm), or None.  Returns (x, delta).
+
+        `attend(q, k, v)` is the attention step: q [T, hq, d], k / v [T, hkv, d] are views of the QKV GEMM output,
+        after RoPE (skipped when `cos` is None); it returns the attention output ([T, hq * d] in any shape).
+        `qkv_out` is a caller buffer [T, (hq + 2 hkv) d] for the QKV GEMM, e.g. the peer-mapped buffer that the
+        context-parallel kernel reads the other ranks' K/V from."""
         cfg = self.cfg
         T = x.shape[0]
         hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -145,62 +150,93 @@ class DecoderLayer:
             h = ops.rmsnorm(x, self.ln1, cfg.rms_norm_eps)
         else:
             h, x = ops.rmsnorm(delta, self.ln1, cfg.rms_norm_eps, residual=x)
-        qkv = ops.linear(h, self.wqkv, self.bqkv)                      # [T, (hq + 2 hkv) d]
+        qkv = ops.linear(h, self.wqkv, self.bqkv, out=qkv_out)            # [T, (hq + 2 hkv) d]
         q = qkv[:, : hq * d].view(T, hq, d)
         k = qkv[:, hq * d : (hq + hkv) * d].view(T, hkv, d)
         v = qkv[:, (hq + hkv) * d :].view(T, hkv, d)
-        ops.rope(q, cos, sin, out=q)
-        ops.rope(k, cos, sin, out=k)
-        if cache is None:
-            att = ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True, **attn_kwargs)
-        elif T == 1 and shard_merge is not None:
-            # context-parallel decode: the cache is sharded over the ranks (any split of the keys works for a
-            # query that sees them all); this rank attends over its shard, `shard_merge` combines the ranks'
-            # (out, lse) pairs.  Only the rank that owns the new position appends its K/V row.
-            if append:
-                kc, vc, length = cache.append(layer_idx, k, v)
-            else:
-                kc, vc, length = cache.k[layer_idx], cache.v[layer_idx], len(cache)
-            if length > 0:
-                o_loc, lse_loc = ops.attention_decode(q[0], kc, vc, length, return_lse=True)
-            else:
-                o_loc = torch.zeros((hq, d), dtype=torch.bfloat16, device=x.device)
-                lse_loc = torch.full((hq,), float("-inf"), dtype=torch.float32, device=x.device)
-            att = shard_merge(o_loc, lse_loc)
-        else:
-            kc, vc, length = cache.append(layer_idx, k, v)
-            if T == 1:
-                att = ops.attention_decode(q[0], kc, vc, length)
-            else:      # first prefill (empty cache) or a chunk of new tokens: causal, aligned to the last key
-                att = ops.attention_fwd(q.unsqueeze(0), kc[:length].unsqueeze(0), vc[:length].unsqueeze(0), causal=True)
-        o = ops.linear(att.reshape(T, hq * d), self.wo)
+        if cos is not None:
+            ops.rope(q, cos, sin, out=q)
+            ops.rope(k, cos, sin, out=k)
+        o = ops.linear(attend(q, k, v).reshape(T, hq * d), self.wo)
         h, x = ops.rmsnorm(o, self.ln2, cfg.rms_norm_eps, residual=x)
         a = ops.linear(h, self.w_gate_up, act="swiglu")
         return x, ops.linear(a, self.w_down)
 
-    def forward_cp(self, x: torch.Tensor, delta: Optional[torch.Tensor], cos, sin, ctx, cache=None,
-                   layer_idx: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
-        """The same layer on this rank's zig-zag shard (`ctx` is the rank's cp.CPContext): the QKV GEMM
-        writes straight into the peer-mapped buffer, RoPE runs in place there, and the fused kernel
-        pulls the other ranks' K/V itself (lv_attn_cp_fwd)."""
-        cfg = self.cfg
-        T = x.shape[0]
-        hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
-        if delta is None:
-            h = ops.rmsnorm(x, self.ln1, cfg.rms_norm_eps)
-        else:
-            h, x = ops.rmsnorm(delta, self.ln1, cfg.rms_norm_eps, residual=x)
-        qkv = ops.linear(h, self.wqkv, self.bqkv, out=ctx.qkv_buffer()).view(T, -1)
-        q = qkv[:, : hq * d].view(T, hq, d)
-        k = qkv[:, hq * d : (hq + hkv) * d].view(T, hkv, d)
-        ops.rope(q, cos, sin, out=q)
-        ops.rope(k, cos, sin, out=k)
-        if cache is not None:      # this rank's zig-zag rows become its shard of the K/V cache
-            cache.append(layer_idx, k, qkv[:, (hq + hkv) * d :].view(T, hkv, d))
-        o = ops.linear(ctx.attention(), self.wo)
-        h, x = ops.rmsnorm(o, self.ln2, cfg.rms_norm_eps, residual=x)
-        a = ops.linear(h, self.w_gate_up, act="swiglu")
-        return x, ops.linear(a, self.w_down)
+
+def run_layers(layers, x: torch.Tensor, cos, sin, attend, norm_w: torch.Tensor, eps: float, *, cache=None,
+               qkv_out=None, hidden: Optional[list] = None) -> torch.Tensor:
+    """The decoder stack: x [T, H] embeddings -> the final RMSNorm of the last hidden state [T, H].
+
+    Each layer's MLP output is handed on as `delta` and added inside the next RMSNorm (the last one inside the final
+    norm).  `attend(layer_index, q, k, v)` is the attention step (DecoderLayer.forward); `qkv_out()`, if given, the QKV
+    GEMM's output buffer of the next layer.  The K/V rows appended to `cache` during the pass are committed at its
+    end.  `hidden` (a list) receives each layer's input hidden state."""
+    delta = None
+    for li, layer in enumerate(layers):
+        if hidden is not None:
+            hidden.append(x if delta is None else x + delta)
+        x, delta = layer.forward(x, delta, cos, sin, partial(attend, li), None if qkv_out is None else qkv_out())
+    if cache is not None:
+        cache.commit()
+    if delta is None:
+        return ops.rmsnorm(x, norm_w, eps)
+    return ops.rmsnorm(delta, norm_w, eps, residual=x)[0]
+
+
+def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None):
+    """The single-GPU attention step for run_layers.  Without `cache`: causal attention over this forward's rows
+    (inside each packed document with `cu_seqlens`).  With `cache`: the new K/V rows are appended to it and one new
+    token attends over the whole cache (flash-decoding), several new tokens over cache + new rows with the causal mask
+    aligned to the last key (the first prefill, or a chunk)."""
+    kw = ops.docs_kwargs(cu_seqlens)
+    if cache is None:
+        return lambda li, q, k, v: ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True, **kw)
+
+    def attend(li, q, k, v):
+        kc, vc, length = cache.append(li, k, v)
+        if q.shape[0] == 1:
+            return ops.attention_decode(q[0], kc, vc, length)
+        return ops.attention_fwd(q.unsqueeze(0), kc[:length].unsqueeze(0), vc[:length].unsqueeze(0), causal=True)
+
+    return attend
+
+
+def packed_rows(position_ids: torch.Tensor, seq_len: int, device, *, cache=None, cp=None) -> Optional[torch.Tensor]:
+    """cu_seqlens of a packed row (position ids restarting at 0 mark the sample boundaries; one host synchronisation),
+    or None when the row holds one sample.  Packing under context parallelism (`cp`) or with a K/V cache raises."""
+    cu = ops.packed_cu_seqlens(position_ids, device=device, seq_len=seq_len)
+    if cu is not None:
+        if cp is not None:
+            raise NotImplementedError("packed samples (position ids restarting at 0) under context parallelism are "
+                                      "not supported")
+        if cache is not None:
+            raise NotImplementedError("packed samples (position ids restarting at 0) cannot be combined with a KV cache "
+                                      "(use_cache / past_key_values / inference_params)")
+    return cu
+
+
+def rope_inv_freq(cfg: LongVITAConfig, device) -> torch.Tensor:
+    """Qwen2's RoPE frequencies 1 / theta^(2i / d), fp32."""
+    return (1.0 / (cfg.rope_theta ** (torch.arange(0, cfg.head_dim, 2, dtype=torch.int64).float()
+                                      / cfg.head_dim))).to(device)
+
+
+VISION_CHUNK = 256  # frames per ViT pass (MegatronVisionModel.forward_chunk, pretrain_long_vita.py:522-533)
+
+
+def vision_tower(cfg: LongVITAConfig, w: Dict[str, torch.Tensor]):
+    """(InternVisionModel, ResamplerProjector), or (None, None) for weights without a vision tower."""
+    if "model.vision_model.embeddings.class_embedding" not in w:
+        return None, None
+    return InternVisionModel(cfg, w), ResamplerProjector(cfg, w)
+
+
+def encode_images(vision_model, projection, images: torch.Tensor, chunk: int = VISION_CHUNK) -> torch.Tensor:
+    """images [n, 3, 448, 448] -> projected features [n, tokens_per_image, H], `chunk` frames per ViT pass."""
+    feats = []
+    for i in range(0, images.shape[0], chunk):
+        feats.append(projection(vision_model(images[i : i + chunk]), has_cls=True))
+    return feats[0] if len(feats) == 1 else torch.cat(feats, dim=0)
 
 
 def _map_tensors(obj, fn, seen=None):
@@ -239,26 +275,23 @@ class _WeightHolderModule(torch.nn.Module):
 
 
 class LongVITAModel(_WeightHolderModule):
-    def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor]):
+    def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor],
+                 layers: Optional[Iterable[DecoderLayer]] = None):
+        """`layers` replaces the decoder layers of `weights` (e.g. layers built one at a time, so that a layer's
+        unfused q/k/v and gate/up weights are freed before the next one is drawn)."""
         super().__init__()
         self.config = cfg
         self.embed_tokens = weights["model.embed_tokens.weight"]
         self.norm_w = weights["model.norm.weight"]
-        self.layers = [DecoderLayer(cfg, weights, i) for i in range(cfg.num_hidden_layers)]
-        has_vit = "model.vision_model.embeddings.class_embedding" in weights
-        self.vision_model = InternVisionModel(cfg, weights) if has_vit else None
-        self.vision_projection = ResamplerProjector(cfg, weights) if has_vit else None
-        self.inv_freq = (1.0 / (cfg.rope_theta ** (torch.arange(0, cfg.head_dim, 2, dtype=torch.int64).float()
-                                                    / cfg.head_dim))).to(self.embed_tokens.device)
-        self.vision_chunk = 256  # frames per ViT pass (pretrain_long_vita.py:522-533)
+        self.layers = ([DecoderLayer(cfg, weights, i) for i in range(cfg.num_hidden_layers)] if layers is None
+                       else list(layers))
+        self.vision_model, self.vision_projection = vision_tower(cfg, weights)
+        self.inv_freq = rope_inv_freq(cfg, self.embed_tokens.device)
+        self.vision_chunk = VISION_CHUNK
         self.default_new_tokens = 1024   # head-room of a cache created by use_cache=True (max_cache_len= overrides)
 
     def encode_images(self, images: torch.Tensor) -> torch.Tensor:
-        feats = []
-        for i in range(0, images.shape[0], self.vision_chunk):
-            vit = self.vision_model(images[i : i + self.vision_chunk])
-            feats.append(self.vision_projection(vit, has_cls=True))
-        return feats[0] if len(feats) == 1 else torch.cat(feats, dim=0)
+        return encode_images(self.vision_model, self.vision_projection, images, self.vision_chunk)
 
     def forward(
         self,
@@ -317,35 +350,19 @@ class LongVITAModel(_WeightHolderModule):
         flash_attn_kwargs.pop("max_cache_len", None)
         if cache_position is None:
             cache_position = torch.arange(past_len, past_len + s, device=x.device)     # modeling_long_vita.py:153-158
-        attn_kwargs = {}
+        cu = None
         if position_ids is None:
             position_ids = cache_position.unsqueeze(0)
         else:
             # packed samples: positions restarting at 0 inside the row are sample boundaries; attention stays inside
             # each sample, as transformers' flash_attention_2 does for the reference (tools/inference_long_vita.py:816)
-            cu = ops.packed_cu_seqlens(position_ids, device=x.device, seq_len=s)
-            if cu is not None:
-                if cache is not None:
-                    raise NotImplementedError("packed samples (position ids restarting at 0) cannot be combined with a "
-                                              "KV cache (use_cache / past_key_values)")
-                attn_kwargs = {"cu_seqlens": cu}
+            cu = packed_rows(position_ids, s, x.device, cache=cache)
         cos, sin = ops.rope_table(position_ids.reshape(-1).to(torch.int64), self.inv_freq)
 
-        all_hidden = () if output_hidden_states else None
-        delta = None
-        for li, layer in enumerate(self.layers):
-            if output_hidden_states:
-                all_hidden += ((x if delta is None else x + delta).view(1, s, -1),)
-            x, delta = layer.forward(x, delta, cos, sin, attn_kwargs, cache, li)
-        if cache is not None:
-            cache.commit()
-        if delta is None:
-            h = ops.rmsnorm(x, self.norm_w, cfg.rms_norm_eps)
-        else:
-            h, _ = ops.rmsnorm(delta, self.norm_w, cfg.rms_norm_eps, residual=x)
-        h = h.view(1, s, -1)
-        if output_hidden_states:
-            all_hidden += (h,)
+        hidden = [] if output_hidden_states else None
+        h = run_layers(self.layers, x, cos, sin, attention_step(cache, cu), self.norm_w, cfg.rms_norm_eps, cache=cache,
+                       hidden=hidden).view(1, s, -1)
+        all_hidden = tuple(t.view(1, s, -1) for t in hidden) + (h,) if output_hidden_states else None
         out = BaseOutput(last_hidden_state=h, past_key_values=cache, hidden_states=all_hidden)
         return out if (return_dict is None or return_dict) else out.to_tuple()
 
@@ -394,10 +411,11 @@ class GenerationDefaults:
 
 
 class LongVITAForCausalLM(_WeightHolderModule):
-    def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor]):
+    def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor],
+                 layers: Optional[Iterable[DecoderLayer]] = None):
         super().__init__()
         self.config = cfg
-        self.model = LongVITAModel(cfg, weights)
+        self.model = LongVITAModel(cfg, weights, layers)
         self.lm_head = weights["lm_head.weight"]
         self.generation_config = GenerationDefaults()
 
@@ -462,29 +480,9 @@ class LongVITAForCausalLM(_WeightHolderModule):
         for i in range(cfg.visual.num_hidden_layers):
             w.update(vit_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb))
         n_layers = cfg.num_hidden_layers if num_layers is None else num_layers
-        self = cls.__new__(cls)
-        torch.nn.Module.__init__(self)
-        self.config = cfg
-        self.lm_head = w["lm_head.weight"]
-        self.generation_config = GenerationDefaults()
-        model = LongVITAModel.__new__(LongVITAModel)
-        torch.nn.Module.__init__(model)
-        model.config = cfg
-        model.embed_tokens = w["model.embed_tokens.weight"]
-        model.norm_w = w["model.norm.weight"]
-        model.vision_model = InternVisionModel(cfg, w)
-        model.vision_projection = ResamplerProjector(cfg, w)
-        model.inv_freq = (1.0 / (cfg.rope_theta ** (torch.arange(0, cfg.head_dim, 2, dtype=torch.int64).float()
-                                                     / cfg.head_dim))).to(device)
-        model.vision_chunk = 256
-        model.default_new_tokens = 1024
-        model.layers = []
-        for i in range(n_layers):
-            lw = llm_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb)
-            model.layers.append(DecoderLayer(cfg, lw, i))
-            del lw
-        self.model = model
-        return self
+        layers = (DecoderLayer(cfg, llm_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb), i)
+                  for i in range(n_layers))
+        return cls(cfg, w, layers)
 
     def forward(
         self,

@@ -73,6 +73,31 @@ def megatron_cu_seqlens(seq_len: int, device) -> Optional[torch.Tensor]:
     return _CU_CACHE[1]
 
 
+def megatron_cp_context(cached, cp_size: int, seq_len: int, hq: int, hkv: int, hn: int, device, group=None):
+    """Context parallelism (zig-zag shards, training/utils.py:329-341): a layer receives this rank's `seq_len` rows
+    only, so attention must see the other ranks' K/V - `cp.CPContext` (fused in-kernel exchange forward, all-gather /
+    reduce-scatter backward).  Returns `cached` while it fits this length (a micro-batch of another length gets its own
+    buffers), None when context_parallel_size is 1.  `group` defaults to Megatron's context-parallel group."""
+    if cp_size <= 1:
+        return None
+    if megatron_packed_ends() is not None:
+        raise NotImplementedError("packed samples (--reset-attention-mask) under context parallelism are not supported")
+    if cached is not None and cached.S == seq_len * cp_size:
+        return cached
+    from ..cp import CPContext
+
+    if group is None:
+        from megatron.core import parallel_state as mpu   # only reached inside a Megatron job
+
+        group = mpu.get_context_parallel_group()
+    return CPContext.shared(group, seq_len * cp_size, hq, hkv, hn, device, fused_qkv=False)
+
+
+def records_grad(*ts) -> bool:
+    """Training or inference: an autograd graph is recorded when gradients are enabled and an input needs one."""
+    return torch.is_grad_enabled() and any(t.requires_grad for t in ts)
+
+
 def _attention_sbhd(query, key, value, causal: bool, scale: float, cp_ctx=None, cu_seqlens=None):
     sq, b, np_, hn = query.shape
     if cu_seqlens is not None:
@@ -82,28 +107,24 @@ def _attention_sbhd(query, key, value, causal: bool, scale: float, cp_ctx=None, 
             raise NotImplementedError("packed samples need a causal attention mask")
         if b != 1:
             raise NotImplementedError("packed samples need micro-batch 1")
-        if torch.is_grad_enabled() and (query.requires_grad or key.requires_grad or value.requires_grad):
-            out = ops.attention(query.permute(1, 0, 2, 3), key.permute(1, 0, 2, 3), value.permute(1, 0, 2, 3),
-                                causal=True, scale=scale, cu_seqlens=cu_seqlens)   # [1, sq, np, hn]
-            return out.permute(1, 0, 2, 3).reshape(sq, b, np_ * hn)
-        out = ops.attention_fwd(query, key, value, causal=True, scale=scale, layout="sbhd", cu_seqlens=cu_seqlens)
-        return out.reshape(sq, b, np_ * hn)
+    train = records_grad(query, key, value)
     if cp_ctx is not None:
         if b != 1:
             raise AssertionError("context-parallel attention supports micro-batch 1 (the reference's long-context setting)")
-        if torch.is_grad_enabled() and (query.requires_grad or key.requires_grad or value.requires_grad):
+        if train:
             from ..cp import cp_attention      # training: fused exchange forward + lv_attn_bwd / reduce-scatter backward
 
             out = cp_attention(query[:, 0], key[:, 0], value[:, 0], cp_ctx, scale)
         else:
             out = cp_ctx.attention_separate(query[:, 0], key[:, 0], value[:, 0], scale=scale)   # [sq, np*hn]
         return out.view(sq, 1, np_ * hn)
-    if torch.is_grad_enabled() and (query.requires_grad or key.requires_grad or value.requires_grad):
+    docs = ops.docs_kwargs(cu_seqlens)
+    if train:
         # training: differentiable path (lv_attn_bwd through torch.autograd.Function)
         out = ops.attention(query.permute(1, 0, 2, 3), key.permute(1, 0, 2, 3), value.permute(1, 0, 2, 3),
-                            causal=causal, scale=scale)                       # [b, sq, np, hn]
+                            causal=causal, scale=scale, **docs)                # [b, sq, np, hn]
         return out.permute(1, 0, 2, 3).reshape(sq, b, np_ * hn)
-    out = ops.attention_fwd(query, key, value, causal=causal, scale=scale, layout="sbhd")
+    out = ops.attention_fwd(query, key, value, causal=causal, scale=scale, layout="sbhd", **docs)
     return out.reshape(sq, b, np_ * hn)
 
 
@@ -129,29 +150,17 @@ class B200DotProductAttention(torch.nn.Module):
         self.cp_size = int(getattr(config, "context_parallel_size", 1) or 1)
         self._cp_ctx = None
 
-    def _cp(self, query, key):
-        if self.cp_size <= 1 or not _is_causal(self.attn_mask_type):
-            return None
-        if megatron_packed_ends() is not None:
-            raise NotImplementedError("packed samples (--reset-attention-mask) under context parallelism are not supported")
-        sq, _, np_, hn = query.shape
-        if self._cp_ctx is None or self._cp_ctx.S != sq * self.cp_size:
-            # keyed on the sequence length of THIS call: a later micro-batch of another length gets its own buffers
-            from megatron.core import parallel_state as mpu   # only reached inside a Megatron job
-
-            from ..cp import CPContext
-
-            self._cp_ctx = CPContext.shared(mpu.get_context_parallel_group(), sq * self.cp_size, np_, key.shape[2], hn,
-                                            query.device, fused_qkv=False)
-        return self._cp_ctx
-
     def forward(self, query, key, value, attention_mask=None, attn_mask_type=None, packed_seq_params=None):
         assert packed_seq_params is None, (
             "Packed sequence is not supported by B200DotProductAttention."     # same contract as the reference,
         )                                                                     # dot_product_attention.py:156-159
         mask_type = self.attn_mask_type if attn_mask_type is None else attn_mask_type
         causal = _is_causal(mask_type)
-        cp_ctx = self._cp(query, key)
+        cp_ctx = None
+        if _is_causal(self.attn_mask_type):
+            sq, _, np_, hn = query.shape
+            cp_ctx = self._cp_ctx = megatron_cp_context(self._cp_ctx, self.cp_size, sq, np_, key.shape[2], hn,
+                                                        query.device)
         cu = None if cp_ctx is not None else megatron_cu_seqlens(query.shape[0], query.device)
         return _attention_sbhd(query, key, value, causal, self.softmax_scale, cp_ctx, cu)
 

@@ -39,7 +39,9 @@ import torch
 
 from .. import ops
 from ..config import LongVITAConfig
-from ..hf.modeling import DecoderLayer, InternVisionModel, ResamplerProjector
+from ..cp import exchange_attention
+from ..hf.modeling import (VISION_CHUNK, DecoderLayer, attention_step, encode_images, packed_rows, rope_inv_freq,
+                           run_layers, vision_tower)
 from .checkpoint import mcore_to_hf
 
 
@@ -61,19 +63,13 @@ class B200GPTVLModel:
         self.output_weight = w["lm_head.weight"]
         self.layers = [DecoderLayer(cfg, w, i) for i in range(cfg.num_hidden_layers)
                        if f"model.layers.{i}.self_attn.q_proj.weight" in w]
-        has_vit = "model.vision_model.embeddings.class_embedding" in w
-        self.vit = InternVisionModel(cfg, w) if has_vit else None
-        self.vision_projection = ResamplerProjector(cfg, w) if has_vit else None
-        self.inv_freq = (1.0 / (cfg.rope_theta ** (torch.arange(0, cfg.head_dim, 2, dtype=torch.int64).float()
-                                                    / cfg.head_dim))).to(self.word_embeddings.device)
-        self.vision_chunk = 256                      # MegatronVisionModel.forward_chunk, pretrain_long_vita.py:522-533
+        self.vit, self.vision_projection = vision_tower(cfg, w)
+        self.inv_freq = rope_inv_freq(cfg, self.word_embeddings.device)
+        self.vision_chunk = VISION_CHUNK
 
     # -- external_feature_model(**external_inputs) (pretrain_long_vita.py:535-563) -----------------
     def external_feature_model(self, images: torch.Tensor, **_unused) -> torch.Tensor:
-        feats = []
-        for i in range(0, images.shape[0], self.vision_chunk):
-            feats.append(self.vision_projection(self.vit(images[i : i + self.vision_chunk]), has_cls=True))
-        return feats[0] if len(feats) == 1 else torch.cat(feats, dim=0)
+        return encode_images(self.vit, self.vision_projection, images, self.vision_chunk)
 
     # -- LanguageModelEmbedding.forward (language_model_embedding.py:91-134) -> [s, h] --------------
     def embedding(self, input_ids: torch.Tensor, position_ids, external_feature_dict: Optional[dict] = None):
@@ -170,35 +166,21 @@ class B200GPTVLModel:
         # RoPE: Megatron builds the table for positions 0..S-1 and slices it zig-zag under CP
         # (rotary_pos_embedding.py:36-47, 84-122); position_ids from get_batch_on_this_cp_rank are
         # exactly those positions, so the table is generated from them directly.
-        position_ids_default = position_ids is None
+        cu = None
         if position_ids is None:
             assert self.cp is None, "context parallelism needs this rank's position_ids"
             p0 = 0 if cache is None else len(cache)
             position_ids = torch.arange(p0, p0 + s, device=x.device).unsqueeze(0)
-        cos, sin = ops.rope_table(position_ids.reshape(-1).to(torch.int64), self.inv_freq)
-        attn_kwargs = {}
-        if not position_ids_default:
-            cu = ops.packed_cu_seqlens(position_ids, device=x.device, seq_len=s)
-            if cu is not None:
-                if self.cp is not None:
-                    raise NotImplementedError("packed samples (position ids restarting at 0) under context parallelism "
-                                              "are not supported")
-                if cache is not None:
-                    raise NotImplementedError("packed samples cannot be combined with a KV cache")
-                attn_kwargs = {"cu_seqlens": cu}
-
-        delta = None
-        for li, layer in enumerate(self.layers):
-            if self.cp is None:
-                x, delta = layer.forward(x, delta, cos, sin, attn_kwargs, cache, li)
-            else:
-                x, delta = layer.forward_cp(x, delta, cos, sin, self.cp)
-        if cache is not None:
-            cache.commit()
-        if delta is None:
-            h = ops.rmsnorm(x, self.final_layernorm, cfg.rms_norm_eps)
         else:
-            h, _ = ops.rmsnorm(delta, self.final_layernorm, cfg.rms_norm_eps, residual=x)
+            cu = packed_rows(position_ids, s, x.device, cache=cache, cp=self.cp)
+        cos, sin = ops.rope_table(position_ids.reshape(-1).to(torch.int64), self.inv_freq)
+
+        if self.cp is None:
+            h = run_layers(self.layers, x, cos, sin, attention_step(cache, cu), self.final_layernorm, cfg.rms_norm_eps,
+                           cache=cache)
+        else:
+            h = run_layers(self.layers, x, cos, sin, exchange_attention(self.cp), self.final_layernorm,
+                           cfg.rms_norm_eps, qkv_out=self.cp.qkv_buffer)
         hidden_states = h.view(s, 1, -1)
 
         # training tail, fused: masked row gather -> LM head -> per-token cross-entropy, chunked over the vocabulary so

@@ -31,12 +31,15 @@ kernels too (`lv_rmsnorm_bwd`, `lv_swiglu_bwd`, `lv_attn_bwd`, the GEMM on trans
 """
 from __future__ import annotations
 
+import types
+from functools import partial
 from typing import Optional
 
 import torch
 
 from .. import ops
-from .core_attention import megatron_cu_seqlens, megatron_packed_ends
+from ..hf.modeling import DecoderLayer, attention_step
+from .core_attention import megatron_cp_context, megatron_cu_seqlens, records_grad
 
 
 class _Params(torch.nn.Module):
@@ -78,9 +81,11 @@ class B200TransformerLayer(torch.nn.Module):
         self.mlp.linear_fc1.weight = P(2 * ffn, h)
         self.mlp.linear_fc2 = _Params()
         self.mlp.linear_fc2.weight = P(h, ffn)
-        self._qkv_w = None       # re-ordered copies of the parameters, rebuilt whenever a parameter changes
-        self._qkv_b = None
-        self._fused_versions = None
+        # the inference layer (hf.modeling.DecoderLayer) on re-ordered copies, rebuilt whenever a parameter changes
+        self._decoder = None
+        self._decoder_stamp = None
+        self._dims = types.SimpleNamespace(num_attention_heads=np_, num_key_value_heads=ng, head_dim=hn,
+                                           rms_norm_eps=self.eps)
         self._rope_cache = (None, None, None)
         if int(getattr(config, "tensor_model_parallel_size", 1) or 1) > 1:
             raise NotImplementedError("B200TransformerLayer holds whole weights: tensor_model_parallel_size must be 1 "
@@ -89,45 +94,33 @@ class B200TransformerLayer(torch.nn.Module):
         self._cp_ctx = None
         self.cp_group = getattr(config, "cp_group", None)   # tests / Megatron-free callers may hand the group in
 
-    # -- Megatron grouped QKV rows -> [q | k | v] -------------------------------------------------
-    def _ungroup(self):
-        np_, ng, hn = self.np, self.ng, self.hn
-        g = np_ // ng
-        w = self.self_attention.linear_qkv.weight.data.view(ng, g + 2, hn, -1)
-        b = self.self_attention.linear_qkv.bias.data.view(ng, g + 2, hn)
-        self._qkv_w = torch.cat([w[:, :g].reshape(np_ * hn, -1), w[:, g].reshape(ng * hn, -1),
-                                 w[:, g + 1].reshape(ng * hn, -1)], dim=0).contiguous()
-        self._qkv_b = torch.cat([b[:, :g].reshape(-1), b[:, g].reshape(-1), b[:, g + 1].reshape(-1)]).contiguous()
-        fc1 = self.mlp.linear_fc1.weight.data                      # cat(gate, up) -> rows (gate_i, up_i)
-        self._fc1_w = ops.interleave_gate_up(fc1[: self.ffn], fc1[self.ffn :])
-
-    def _fused_weights_current(self) -> bool:
-        """The re-ordered copies follow load_state_dict() / optimizer steps: every in-place update of a parameter bumps
-        its `_version`, and a re-assigned `.data` changes `data_ptr()`."""
-        ps = (self.self_attention.linear_qkv.weight, self.self_attention.linear_qkv.bias, self.mlp.linear_fc1.weight)
-        stamp = tuple((p._version, p.data_ptr()) for p in ps)
-        if self._qkv_w is None or stamp != self._fused_versions:
-            self._ungroup()
-            self._fused_versions = stamp
-        return True
+    def _decoder_layer(self) -> DecoderLayer:
+        """The inference layer on this module's parameters: Megatron's grouped QKV rows [ng, (np/ng + 2), hn, h] become
+        [all q | all k | all v] and fc1 = cat(gate, up) the interleaved SwiGLU operand.  The copies follow
+        load_state_dict() / optimizer steps / .to(): every in-place update of a parameter bumps its `_version`, and a
+        re-assigned `.data` or parameter changes `data_ptr()`."""
+        stamp = tuple((p._version, p.data_ptr()) for p in self.parameters())
+        if self._decoder is None or stamp != self._decoder_stamp:
+            self._decoder = None               # free the stale copies before the new ones are made
+            ng, hn, g = self.ng, self.hn, self.np // self.ng
+            a, m = self.self_attention, self.mlp
+            w = a.linear_qkv.weight.data.view(ng, g + 2, hn, -1)
+            b = a.linear_qkv.bias.data.view(ng, g + 2, hn)
+            fc1 = m.linear_fc1.weight.data
+            p = "model.layers.0."
+            hf = {p + "self_attn.o_proj.weight": a.linear_proj.weight.data,
+                  p + "mlp.gate_proj.weight": fc1[: self.ffn], p + "mlp.up_proj.weight": fc1[self.ffn :],
+                  p + "mlp.down_proj.weight": m.linear_fc2.weight.data,
+                  p + "input_layernorm.weight": a.linear_qkv.layer_norm_weight.data,
+                  p + "post_attention_layernorm.weight": m.linear_fc1.layer_norm_weight.data}
+            for name, rows in (("q_proj", slice(0, g)), ("k_proj", g), ("v_proj", g + 1)):
+                hf[p + f"self_attn.{name}.weight"] = w[:, rows].reshape(-1, w.shape[-1])
+                hf[p + f"self_attn.{name}.bias"] = b[:, rows].reshape(-1)
+            self._decoder, self._decoder_stamp = DecoderLayer(self._dims, hf, 0), stamp
+        return self._decoder
 
     def _cp(self, s: int, device):
-        """Context parallelism (zig-zag shards, training/utils.py:329-341): the layer receives this rank's rows only,
-        so attention must see the other ranks' K/V - `cp.CPContext` (fused in-kernel exchange forward, all-gather /
-        reduce-scatter backward).  None when context_parallel_size == 1."""
-        if self.cp_size <= 1:
-            return None
-        if megatron_packed_ends() is not None:
-            raise NotImplementedError("packed samples (--reset-attention-mask) under context parallelism are not supported")
-        if self._cp_ctx is None or self._cp_ctx.S != s * self.cp_size:
-            from ..cp import CPContext
-
-            group = self.cp_group
-            if group is None:
-                from megatron.core import parallel_state as mpu   # only reached inside a Megatron job
-
-                group = mpu.get_context_parallel_group()
-            self._cp_ctx = CPContext.shared(group, s * self.cp_size, self.np, self.ng, self.hn, device, fused_qkv=False)
+        self._cp_ctx = megatron_cp_context(self._cp_ctx, self.cp_size, s, self.np, self.ng, self.hn, device, self.cp_group)
         return self._cp_ctx
 
     def _rope(self, rotary_pos_emb):
@@ -150,30 +143,16 @@ class B200TransformerLayer(torch.nn.Module):
         s, b, h = hidden_states.shape
         if b != 1:
             raise NotImplementedError("micro-batch 1 (the reference's long-context setting)")
-        if torch.is_grad_enabled() and (hidden_states.requires_grad or any(p.requires_grad for p in self.parameters())):
+        if records_grad(hidden_states, *self.parameters()):
             return self._forward_train(hidden_states, rotary_pos_emb), context
-        self._fused_weights_current()
-        np_, ng, hn = self.np, self.ng, self.hn
-        x = hidden_states.reshape(s, h)
-        hcur = ops.rmsnorm(x, self.self_attention.linear_qkv.layer_norm_weight, self.eps)
-        qkv = ops.linear(hcur, self._qkv_w, self._qkv_b)
-        q = qkv[:, : np_ * hn].view(s, np_, hn)
-        k = qkv[:, np_ * hn : (np_ + ng) * hn].view(s, ng, hn)
-        v = qkv[:, (np_ + ng) * hn :].view(s, ng, hn)
-        if rotary_pos_emb is not None:
-            cos, sin = self._rope(rotary_pos_emb)
-            ops.rope(q, cos, sin, out=q)
-            ops.rope(k, cos, sin, out=k)
+        layer = self._decoder_layer()
+        cos, sin = (None, None) if rotary_pos_emb is None else self._rope(rotary_pos_emb)
         cp_ctx = self._cp(s, hidden_states.device)
         if cp_ctx is not None:
-            att = cp_ctx.attention_separate(q, k, v)                               # [s, np * hn]
+            attend = cp_ctx.attention_separate                                     # [s, np * hn]
         else:
-            att = ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True,
-                                    **ops.docs_kwargs(megatron_cu_seqlens(s, hidden_states.device)))
-        o = ops.linear(att.view(s, np_ * hn), self.self_attention.linear_proj.weight)
-        hcur, x = ops.rmsnorm(o, self.mlp.linear_fc1.layer_norm_weight, self.eps, residual=x)
-        a = ops.linear(hcur, self._fc1_w, act="swiglu")
-        d = ops.linear(a, self.mlp.linear_fc2.weight)
+            attend = partial(attention_step(cu_seqlens=megatron_cu_seqlens(s, hidden_states.device)), 0)
+        x, d = layer.forward(hidden_states.reshape(s, h), None, cos, sin, attend)
         out = ops.ls_residual(x, d)           # plain residual add (bias-dropout-add with p = 0, no bias)
         return out.view(s, b, h), context
 
@@ -188,7 +167,7 @@ class B200TransformerLayer(torch.nn.Module):
         s, b, h = hidden_states.shape
         np_, ng, hn = self.np, self.ng, self.hn
         g = np_ // ng
-        self._qkv_w = None                 # the re-ordered inference copies go stale once the parameters train
+        self._decoder = None               # the re-ordered inference copies go stale once the parameters train
         x = hidden_states.reshape(s, h)
         a = self.self_attention
         hcur = ops.rmsnorm_autograd(x, a.linear_qkv.layer_norm_weight, self.eps)

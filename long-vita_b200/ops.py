@@ -181,6 +181,40 @@ def _check_docs_call(b, sq, sk, causal, q_seg_len, q_seg_pos, kv_pos0):
 # ------------------------------------------------------------------------------------------------
 # attention
 # ------------------------------------------------------------------------------------------------
+def tma_view_ok(t: torch.Tensor) -> bool:
+    """The attention kernels load q / k / v / out (and the gradients) through TMA, in place: the head dimension must be
+    contiguous and every other stride a multiple of 8 elements (16 bytes)."""
+    return t.stride(-1) == 1 and all(s % 8 == 0 for s in t.stride()[:-1])
+
+
+def tma_view(t: torch.Tensor) -> torch.Tensor:
+    return t if tma_view_ok(t) else t.contiguous()
+
+
+def attn_params(q, k, v, out, lse=None, *, scale: Optional[float] = None, causal: bool, q_seg_len=None, q_seg_pos=None,
+                kv_pos0: int = 0) -> AttnParams:
+    """`lv_attn_params` of q [b, sq, hq, d], k / v [b, sk, hkv, d] and out [b, sq, hq, d] views (pointers and strides
+    are taken as they are) and lse [b, hq, sq] fp32 or None.  Defaults: scale 1/sqrt(d), one query segment of sq rows
+    whose mask is aligned to the last key (flash-attn >= 2.1)."""
+    b, sq, hq, d = q.shape
+    _, sk, hkv, _ = k.shape
+    p = AttnParams()
+    p.q, p.k, p.v, p.out = q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr()
+    p.lse = _ptr(lse)
+    p.batch, p.sq, p.sk, p.hq, p.hkv, p.d = b, sq, sk, hq, hkv, d
+    for name, t in (("q_strides", q), ("k_strides", k), ("v_strides", v), ("o_strides", out)):
+        arr = getattr(p, name)
+        arr[0], arr[1], arr[2] = t.stride(0), t.stride(1), t.stride(2)
+    p.scale = float(scale if scale is not None else 1.0 / math.sqrt(d))
+    p.causal = 1 if causal else 0
+    p.q_seg_len = int(q_seg_len if q_seg_len is not None else sq)
+    if q_seg_pos is None:
+        q_seg_pos = (sk - sq, 0)
+    p.q_seg_pos[0], p.q_seg_pos[1] = int(q_seg_pos[0]), int(q_seg_pos[1])
+    p.kv_pos0 = int(kv_pos0)
+    return p
+
+
 def attention_fwd(
     q: torch.Tensor,
     k: torch.Tensor,
@@ -213,36 +247,13 @@ def attention_fwd(
     if cu_seqlens is not None:
         _check_docs_call(b, sq, sk, causal, q_seg_len, q_seg_pos, kv_pos0)
         docs, host = _docs_arg(cu_seqlens, sk)
-
-    def ok(t):
-        return t.stride(3) == 1 and all(s % 8 == 0 for s in t.stride()[:3])
-
-    if not ok(qv):
-        qv = qv.contiguous()
-    if not ok(kv_):
-        kv_ = kv_.contiguous()
-    if not ok(vv):
-        vv = vv.contiguous()
+    qv, kv_, vv = tma_view(qv), tma_view(kv_), tma_view(vv)
     if out is None:
         # allocate in the caller's layout so the result is contiguous there
         out = torch.empty(q.shape, dtype=torch.bfloat16, device=q.device)
-    ov = out.permute(perm)
     lse = torch.empty((b, hq, sq), dtype=torch.float32, device=q.device) if return_lse else None
-
-    p = AttnParams()
-    p.q, p.k, p.v, p.out = qv.data_ptr(), kv_.data_ptr(), vv.data_ptr(), ov.data_ptr()
-    p.lse = _ptr(lse)
-    p.batch, p.sq, p.sk, p.hq, p.hkv, p.d = b, sq, sk, hq, hkv, d
-    for name, t in (("q_strides", qv), ("k_strides", kv_), ("v_strides", vv), ("o_strides", ov)):
-        arr = getattr(p, name)
-        arr[0], arr[1], arr[2] = t.stride(0), t.stride(1), t.stride(2)
-    p.scale = float(scale if scale is not None else 1.0 / math.sqrt(d))
-    p.causal = 1 if causal else 0
-    p.q_seg_len = int(q_seg_len if q_seg_len is not None else sq)
-    if q_seg_pos is None:
-        q_seg_pos = (sk - sq, 0)  # bottom-right aligned causal mask (flash-attn >= 2.1)
-    p.q_seg_pos[0], p.q_seg_pos[1] = int(q_seg_pos[0]), int(q_seg_pos[1])
-    p.kv_pos0 = int(kv_pos0)
+    p = attn_params(qv, kv_, vv, out.permute(perm), lse, scale=scale, causal=causal, q_seg_len=q_seg_len,
+                    q_seg_pos=q_seg_pos, kv_pos0=kv_pos0)
     ev0 = _TIMER.start() if _TIMER is not None else None
     if docs is not None:
         _lib.check(_lib.lib().lv_attn_docs_fwd(C.byref(p), C.byref(docs), _stream()), "lv_attn_docs_fwd")
@@ -259,24 +270,6 @@ def attention_fwd(
     return (out, lse) if return_lse else out
 
 
-def _fill_attn_params(p, qv, kv_, vv, ov, lse, scale, causal, q_seg_len, q_seg_pos, kv_pos0):
-    b, sq, hq, d = qv.shape
-    _, sk, hkv, _ = kv_.shape
-    p.q, p.k, p.v, p.out = qv.data_ptr(), kv_.data_ptr(), vv.data_ptr(), ov.data_ptr()
-    p.lse = _ptr(lse)
-    p.batch, p.sq, p.sk, p.hq, p.hkv, p.d = b, sq, sk, hq, hkv, d
-    for name, t in (("q_strides", qv), ("k_strides", kv_), ("v_strides", vv), ("o_strides", ov)):
-        arr = getattr(p, name)
-        arr[0], arr[1], arr[2] = t.stride(0), t.stride(1), t.stride(2)
-    p.scale = float(scale if scale is not None else 1.0 / math.sqrt(d))
-    p.causal = 1 if causal else 0
-    p.q_seg_len = int(q_seg_len if q_seg_len is not None else sq)
-    if q_seg_pos is None:
-        q_seg_pos = (sk - sq, 0)
-    p.q_seg_pos[0], p.q_seg_pos[1] = int(q_seg_pos[0]), int(q_seg_pos[1])
-    p.kv_pos0 = int(kv_pos0)
-
-
 def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[float] = None, q_seg_len=None,
                   q_seg_pos=None, kv_pos0: int = 0, cu_seqlens: Optional[torch.Tensor] = None,
                   dq: Optional[torch.Tensor] = None, dk: Optional[torch.Tensor] = None, dv: Optional[torch.Tensor] = None):
@@ -289,7 +282,7 @@ def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[flo
     if dq is not None:
         _need_cuda_bf16(dq, dk, dv)
         for t, ref in ((dq, q), (dk, k), (dv, v)):
-            if t.shape != ref.shape or t.stride(3) != 1 or any(s % 8 for s in t.stride()[:3]):
+            if t.shape != ref.shape or not tma_view_ok(t):
                 raise ValueError("attention_bwd: dq / dk / dv must have the shapes of q / k / v, a contiguous head dimension "
                                  "and strides that are multiples of 8 elements")
     _need_cuda_bf16(d_out, q, k, v, out)
@@ -298,18 +291,15 @@ def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[flo
     if cu_seqlens is not None:
         _check_docs_call(q.shape[0], q.shape[1], k.shape[1], causal, q_seg_len, q_seg_pos, kv_pos0)
         docs, _ = _docs_arg(cu_seqlens, k.shape[1])
-
-    def fix(t):
-        return t if (t.stride(3) == 1 and all(s % 8 == 0 for s in t.stride()[:3])) else t.contiguous()
-
-    q, k, v, out, d_out = fix(q), fix(k), fix(v), fix(out), fix(d_out)
+    q, k, v, out, d_out = tma_view(q), tma_view(k), tma_view(v), tma_view(out), tma_view(d_out)
     if dq is None:
         dq, dk, dv = torch.empty_like(q, memory_format=torch.contiguous_format), \
             torch.empty_like(k, memory_format=torch.contiguous_format), torch.empty_like(v, memory_format=torch.contiguous_format)
     b, sq, hq, _ = q.shape
     delta = torch.empty((b, hq, sq), dtype=torch.float32, device=q.device)
     p = AttnBwdParams()
-    _fill_attn_params(p.fwd, q, k, v, out, lse.contiguous(), scale, causal, q_seg_len, q_seg_pos, kv_pos0)
+    p.fwd = attn_params(q, k, v, out, lse.contiguous(), scale=scale, causal=causal, q_seg_len=q_seg_len,
+                        q_seg_pos=q_seg_pos, kv_pos0=kv_pos0)
     p.d_out, p.dq, p.dk, p.dv, p.delta_ws = d_out.data_ptr(), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), delta.data_ptr()
     for name, t in (("do_strides", d_out), ("dq_strides", dq), ("dk_strides", dk), ("dv_strides", dv)):
         arr = getattr(p, name)

@@ -1,6 +1,8 @@
 """GPU parity of the composed path: InternViT tower, projector, Qwen2 decoder layer (teacher-forced),
 and the whole LongVITAForCausalLM.forward on a tiny geometry that keeps the 14B head structure
 (GQA 5:1, head_dim 128 / 64, 448/14 patches) - against the CPU oracle on identical bf16 weights."""
+from functools import partial
+
 import pytest
 import torch
 
@@ -58,7 +60,7 @@ def test_decoder_layer_teacher_forced(setup):
     w32 = OM.cast_weights(w, torch.float32)
     ref = OM.decoder_layer(cfg, w32, 0, x.float(), cos.float(), sin.float())
     layer = M.DecoderLayer(cfg, wg, 0)
-    xg, delta = layer.forward(x.cuda(), None, cos.cuda(), sin.cuda(), {})
+    xg, delta = layer.forward(x.cuda(), None, cos.cuda(), sin.cuda(), partial(M.attention_step(), 0))
     out = xg.float() + delta.float()
     assert rel_fro(out, ref) < 4e-3, (rel_fro(out, ref), max_rel(out, ref))
 

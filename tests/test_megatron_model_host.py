@@ -538,14 +538,12 @@ def reference_glue_outputs(cfg, model):
     rotary.get_rotary_seq_len = lambda inference_params, decoder, decoder_input, config: decoder_input.shape[0]
 
     def decoder(hidden_states, attention_mask, inference_params, rotary_pos_emb, packed_seq_params):
-        from long_vita_b200 import ops
+        from long_vita_b200.hf.modeling import attention_step, run_layers
 
         f = rotary_pos_emb.reshape(rotary_pos_emb.shape[0], -1)
         cos, sin = torch.cos(f).to(torch.bfloat16), torch.sin(f).to(torch.bfloat16)
-        x, delta = hidden_states[:, 0], None
-        for layer in model.layers:
-            x, delta = layer.forward(x, delta, cos, sin, {})
-        h, _ = ops.rmsnorm(delta, model.final_layernorm, cfg.rms_norm_eps, residual=x)
+        h = run_layers(model.layers, hidden_states[:, 0], cos, sin, attention_step(), model.final_layernorm,
+                       cfg.rms_norm_eps)
         return h.unsqueeze(1)
 
     def output_layer(hidden_states, weight=None, logit_mask=None):
