@@ -6,6 +6,9 @@
 #include <cuda_bf16.h>
 #include <math.h>
 
+#include <iterator>
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace lv {
@@ -840,6 +843,36 @@ using namespace lv;
 
 static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
+// Row tiling of the norm kernels: TPR threads share a row (256 / TPR rows per CTA) and each holds VPT 16-byte vectors
+// of it.  A row of `cols` takes the first entry with cols / 8 <= max_nvec; the last entry takes every wider row.
+struct RowTiling {
+  int64_t max_nvec;
+  int tpr, vpt;
+};
+constexpr RowTiling NORM_TILING[] = {{32 * 4, 32, 4}, {128 * 4, 128, 4}, {128 * 5, 128, 5}, {INT64_MAX, 256, 8}};
+constexpr RowTiling LN_BWD_TILING[] = {{32 * 4, 32, 4}, {128 * 4, 128, 4}, {INT64_MAX, 256, 4}};
+
+// Calls launch(TPR, VPT), both std::integral_constant<int>, with the entry of TABLE that a row of `cols` takes.
+template <const auto& TABLE, size_t I = 0, class F>
+static void with_tiling(int64_t cols, F&& launch) {
+  if constexpr (I + 1 < std::size(TABLE)) {
+    if (cols / 8 > TABLE[I].max_nvec) return with_tiling<TABLE, I + 1>(cols, launch);
+  }
+  launch(std::integral_constant<int, TABLE[I].tpr>{}, std::integral_constant<int, TABLE[I].vpt>{});
+}
+
+// Rows of each fp32 partial buffer a norm backward writes: one per row slot of every CTA, ~2 CTAs per SM.
+template <const auto& TABLE>
+static int64_t bwd_partials(int64_t rows, int64_t cols) {
+  int64_t rpc = 0;
+  with_tiling<TABLE>(cols, [&](auto TPR, auto) { rpc = 256 / TPR; });
+  int64_t grid = (rows + rpc - 1) / rpc;
+  const int64_t cap = 2 * (int64_t)lv::sm_count();
+  if (grid > cap) grid = cap;
+  if (grid < 1) grid = 1;
+  return grid * rpc;
+}
+
 extern "C" {
 
 int lv_rmsnorm(const void* x, const void* residual, const void* w, void* y, void* sum_out, int64_t rows,
@@ -849,19 +882,10 @@ int lv_rmsnorm(const void* x, const void* residual, const void* w, void* y, void
   LV_CHECK_ARG(aligned16(x) && aligned16(w) && aligned16(y) && aligned16(residual) && aligned16(sum_out), "lv_rmsnorm: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  const int nvec = (int)(cols / 8);
-#define LAUNCH_RMS(TPR, VPT)                                                                                   \
-  rmsnorm_kernel<TPR, VPT><<<(unsigned)cdiv(rows, 256 / TPR), 256, 0, s>>>(BF(x), BF(residual), BF(w), BFM(y), \
-                                                                           BFM(sum_out), rows, (int)cols, eps)
-  if (nvec <= 32 * 4)
-    LAUNCH_RMS(32, 4);
-  else if (nvec <= 128 * 4)
-    LAUNCH_RMS(128, 4);
-  else if (nvec <= 128 * 5)
-    LAUNCH_RMS(128, 5);
-  else
-    LAUNCH_RMS(256, 8);
-#undef LAUNCH_RMS
+  with_tiling<NORM_TILING>(cols, [&](auto TPR, auto VPT) {
+    rmsnorm_kernel<TPR, VPT><<<(unsigned)cdiv(rows, 256 / TPR), 256, 0, s>>>(BF(x), BF(residual), BF(w), BFM(y),
+                                                                             BFM(sum_out), rows, (int)cols, eps);
+  });
   LV_CHECK_LAUNCH("rmsnorm_kernel");
   return LV_OK;
 }
@@ -873,18 +897,9 @@ int lv_layernorm(const void* x, const void* w, const void* b, void* y, int64_t r
   LV_CHECK_ARG(aligned16(x) && aligned16(w) && aligned16(y) && aligned16(b), "lv_layernorm: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
   cudaStream_t s = (cudaStream_t)stream;
-  const int nvec = (int)(cols / 8);
-#define LAUNCH_LN(TPR, VPT) \
-  layernorm_kernel<TPR, VPT><<<(unsigned)cdiv(rows, 256 / TPR), 256, 0, s>>>(BF(x), BF(w), BF(b), BFM(y), rows, (int)cols, eps)
-  if (nvec <= 32 * 4)
-    LAUNCH_LN(32, 4);
-  else if (nvec <= 128 * 4)
-    LAUNCH_LN(128, 4);
-  else if (nvec <= 128 * 5)
-    LAUNCH_LN(128, 5);
-  else
-    LAUNCH_LN(256, 8);
-#undef LAUNCH_LN
+  with_tiling<NORM_TILING>(cols, [&](auto TPR, auto VPT) {
+    layernorm_kernel<TPR, VPT><<<(unsigned)cdiv(rows, 256 / TPR), 256, 0, s>>>(BF(x), BF(w), BF(b), BFM(y), rows, (int)cols, eps);
+  });
   LV_CHECK_LAUNCH("layernorm_kernel");
   return LV_OK;
 }
@@ -1036,17 +1051,7 @@ int lv_attn_decode_merge(const void* o_part, const float* lse_part, void* out, f
   return LV_OK;
 }
 
-int64_t lv_rmsnorm_bwd_partials(int64_t rows, int64_t cols) {
-  // rows of the dw partial buffer the kernel writes: gridDim * rows-per-CTA (same TPR choice as the launch below)
-  const int64_t nvec = cols / 8;
-  const int tpr = nvec <= 32 * 4 ? 32 : (nvec <= 128 * 5 ? 128 : 256);
-  const int64_t rpc = 256 / tpr;
-  int64_t grid = (rows + rpc - 1) / rpc;
-  const int64_t cap = 2 * (int64_t)lv::sm_count();
-  if (grid > cap) grid = cap;
-  if (grid < 1) grid = 1;
-  return grid * rpc;
-}
+int64_t lv_rmsnorm_bwd_partials(int64_t rows, int64_t cols) { return bwd_partials<NORM_TILING>(rows, cols); }
 
 int lv_rmsnorm_bwd(const void* x, const void* w, const void* dy, const void* add_in, void* dx, float* dw_partials,
                    int64_t rows, int64_t cols, float eps, lv_stream_t stream) {
@@ -1060,19 +1065,10 @@ int lv_rmsnorm_bwd(const void* x, const void* w, const void* dy, const void* add
     LV_CHECK_CUDA(cudaMemsetAsync(dw_partials, 0, (size_t)parts * cols * 4, s));
     return LV_OK;
   }
-  const int nvec = (int)(cols / 8);
-#define LAUNCH_RMSB(TPR, VPT)                                                                                       \
-  rmsnorm_bwd_kernel<TPR, VPT><<<(unsigned)(parts / (256 / TPR)), 256, 0, s>>>(BF(x), BF(w), BF(dy), BF(add_in), BFM(dx), \
-                                                                                dw_partials, rows, (int)cols, eps)
-  if (nvec <= 32 * 4)
-    LAUNCH_RMSB(32, 4);
-  else if (nvec <= 128 * 4)
-    LAUNCH_RMSB(128, 4);
-  else if (nvec <= 128 * 5)
-    LAUNCH_RMSB(128, 5);
-  else
-    LAUNCH_RMSB(256, 8);
-#undef LAUNCH_RMSB
+  with_tiling<NORM_TILING>(cols, [&](auto TPR, auto VPT) {
+    rmsnorm_bwd_kernel<TPR, VPT><<<(unsigned)(parts / (256 / TPR)), 256, 0, s>>>(BF(x), BF(w), BF(dy), BF(add_in), BFM(dx),
+                                                                                  dw_partials, rows, (int)cols, eps);
+  });
   LV_CHECK_LAUNCH("rmsnorm_bwd_kernel");
   return LV_OK;
 }
@@ -1120,17 +1116,7 @@ int lv_ce_grad(const void* logits, int64_t ld, void* dlogits, int64_t ldd, const
   return LV_OK;
 }
 
-int64_t lv_layernorm_bwd_partials(int64_t rows, int64_t cols) {
-  // rows of each partial buffer the kernel writes: gridDim * rows-per-CTA (same TPR choice as the launch below)
-  const int64_t nvec = cols / 8;
-  const int tpr = nvec <= 32 * 4 ? 32 : (nvec <= 128 * 4 ? 128 : 256);
-  const int64_t rpc = 256 / tpr;
-  int64_t grid = (rows + rpc - 1) / rpc;
-  const int64_t cap = 2 * (int64_t)lv::sm_count();
-  if (grid > cap) grid = cap;
-  if (grid < 1) grid = 1;
-  return grid * rpc;
-}
+int64_t lv_layernorm_bwd_partials(int64_t rows, int64_t cols) { return bwd_partials<LN_BWD_TILING>(rows, cols); }
 
 int lv_layernorm_bwd(const void* x, const void* w, const void* dy, const void* add_in, void* dx, float* dw_partials,
                      float* db_partials, int64_t rows, int64_t cols, float eps, lv_stream_t stream) {
@@ -1147,17 +1133,10 @@ int lv_layernorm_bwd(const void* x, const void* w, const void* dy, const void* a
     LV_CHECK_CUDA(cudaMemsetAsync(db_partials, 0, (size_t)parts * cols * 4, s));
     return LV_OK;
   }
-  const int nvec = (int)(cols / 8);
-#define LAUNCH_LNB(TPR, VPT)                                                                                  \
-  layernorm_bwd_kernel<TPR, VPT><<<(unsigned)(parts / (256 / TPR)), 256, 0, s>>>(                             \
-      BF(x), BF(w), BF(dy), BF(add_in), BFM(dx), dw_partials, db_partials, rows, (int)cols, eps)
-  if (nvec <= 32 * 4)
-    LAUNCH_LNB(32, 4);
-  else if (nvec <= 128 * 4)
-    LAUNCH_LNB(128, 4);
-  else
-    LAUNCH_LNB(256, 4);
-#undef LAUNCH_LNB
+  with_tiling<LN_BWD_TILING>(cols, [&](auto TPR, auto VPT) {
+    layernorm_bwd_kernel<TPR, VPT><<<(unsigned)(parts / (256 / TPR)), 256, 0, s>>>(
+        BF(x), BF(w), BF(dy), BF(add_in), BFM(dx), dw_partials, db_partials, rows, (int)cols, eps);
+  });
   LV_CHECK_LAUNCH("layernorm_bwd_kernel");
   return LV_OK;
 }

@@ -608,82 +608,39 @@ def interleave_gate_up(gate_w: torch.Tensor, up_w: torch.Tensor) -> torch.Tensor
     return torch.stack([gate_w, up_w], dim=1).reshape(2 * gate_w.shape[0], gate_w.shape[1]).contiguous()
 
 
+class _SelectRowsFn(torch.autograd.Function):
+    """The rows of h [s, 1, c] that logit_mask [1, s] selects -> [M, c] (masked_select of the hidden rows,
+    long_vita_megatron/core/tensor_parallel/layers.py:402-409); the gradient goes back into zeros (masked_scatter,
+    :443-451).  Micro-batch 1, the reference's setting when logit_mask is used.  The row indices are computed by
+    torch (host-side index op)."""
+
+    @staticmethod
+    def forward(ctx, h, logit_mask):
+        s, b, c = h.shape
+        if b != 1:
+            raise NotImplementedError("logit-masked rows: micro-batch 1")
+        idx = logit_mask.reshape(-1).nonzero().view(-1)
+        ctx.save_for_backward(idx)
+        ctx.s = s
+        return row_gather(h.reshape(s, c), idx)
+
+    @staticmethod
+    def backward(ctx, d_sel):
+        (idx,) = ctx.saved_tensors
+        return row_scatter_zero(d_sel, idx, ctx.s).view(ctx.s, 1, -1), None
+
+
+def select_rows(h: torch.Tensor, logit_mask: torch.Tensor) -> torch.Tensor:
+    """Differentiable logit-mask row selection, h [s, 1, c] -> [M, c] (see _SelectRowsFn)."""
+    return _SelectRowsFn.apply(h, logit_mask)
+
+
 def masked_linear(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.Tensor, bias: Optional[torch.Tensor] = None):
-    """Logit-masked LM head forward: rows of h [s, b, c] selected by logit_mask [b, s] -> [M, b, vocab]
-    (LinearWithGradAccumulationAndAsyncCommunication.forward with logit_mask,
-    long_vita_megatron/core/tensor_parallel/layers.py:402-409).  b = 1 (the reference's setting when
-    logit_mask is used: micro-batch 1).  The row indices are computed by torch (host-side index op)."""
-    _need_cuda_bf16(h, weight, bias)
-    s, b, c = h.shape
-    if b != 1:
-        raise NotImplementedError("masked_linear: micro-batch 1")
-    idx = logit_mask.reshape(-1).nonzero().view(-1)
-    sel = row_gather(h.reshape(s, c), idx)
-    return linear(sel, weight, bias).view(idx.numel(), 1, weight.shape[0])
-
-
-def masked_linear_dgrad(grad_out: torch.Tensor, weight: torch.Tensor, logit_mask: torch.Tensor):
-    """dX of masked_linear: masked_scatter(zeros[s, b, c], dY @ W) (layers.py:443-451).  `weight` is
-    [vocab, c]; the GEMM needs its transpose as the [N, K] operand, materialised by the caller once
-    (weights are frozen in the reference's use of this path: linear_with_frozen_weight, :288-363)."""
-    _need_cuda_bf16(grad_out, weight)
-    m = grad_out.shape[0]
-    s = logit_mask.shape[-1]
-    wt = weight.t().contiguous()                      # [c, vocab] = the [N, K] operand of dY @ W
-    gi = linear(grad_out.reshape(m, -1), wt)          # [M, c]
-    idx = logit_mask.reshape(-1).nonzero().view(-1)
-    return row_scatter_zero(gi, idx, s).view(s, 1, -1)
-
-
-def masked_linear_wgrad(grad_out: torch.Tensor, h: torch.Tensor, logit_mask: torch.Tensor):
-    """dW of masked_linear: dY^T . masked_select(h) -> [vocab, c] (layers.py:451-456, 512-520: `grad_output.t()
-    .matmul(total_input)`).  Runs on the same wgmma GEMM with the contraction over the M selected rows: both
-    operands are transposed once ([vocab, M] and [c, M]; M is the number of answer tokens) and M is zero-padded
-    to a multiple of 8 (the GEMM's K granularity)."""
-    _need_cuda_bf16(grad_out, h)
-    s, b, c = h.shape
-    m = grad_out.shape[0]
-    vocab = grad_out.shape[-1]
-    if m == 0:
-        return torch.zeros((vocab, c), dtype=torch.bfloat16, device=h.device)
-    idx = logit_mask.reshape(-1).nonzero().view(-1)
-    sel = row_gather(h.reshape(s, c), idx)                              # [M, c]
-    mp = (m + 7) // 8 * 8
-    gt = torch.zeros((vocab, mp), dtype=torch.bfloat16, device=h.device)
-    gt[:, :m] = grad_out.reshape(m, vocab).t()
-    st = torch.zeros((c, mp), dtype=torch.bfloat16, device=h.device)
-    st[:, :m] = sel.t()
-    return linear(gt, st)                                               # [vocab, c]
-
-
-class _MaskedLinearFn(torch.autograd.Function):
-    """LinearWithGradAccumulationAndAsyncCommunication with `logit_mask` (layers.py:371-456) for tp = 1,
-    no sequence parallelism, no gradient-accumulation fusion: forward = gather + GEMM, backward =
-    dX = masked_scatter(zeros, dY W) and (when the weight trains) dW = dY^T sel."""
-
-    @staticmethod
-    def forward(ctx, h, weight, logit_mask):
-        ctx.save_for_backward(h, weight, logit_mask)
-        return masked_linear(h, weight, logit_mask)
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        h, weight, logit_mask = ctx.saved_tensors
-        grad_out = grad_out.contiguous()
-        gh = gw = None
-        if ctx.needs_input_grad[0]:
-            if grad_out.shape[0] == 0:
-                gh = torch.zeros_like(h)
-            else:
-                gh = masked_linear_dgrad(grad_out, weight, logit_mask)
-        if ctx.needs_input_grad[1]:
-            gw = masked_linear_wgrad(grad_out, h, logit_mask)
-        return gh, gw, None
-
-
-def masked_linear_autograd(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.Tensor):
-    """Differentiable logit-masked LM head (SURVEY.md 8a-12)."""
-    return _MaskedLinearFn.apply(h, weight, logit_mask)
+    """Logit-masked LM head, differentiable: rows of h [s, 1, c] selected by logit_mask [1, s] -> [M, 1, vocab]
+    (LinearWithGradAccumulationAndAsyncCommunication with logit_mask, layers.py:371-456, for tp = 1, no sequence
+    parallelism, no gradient-accumulation fusion).  Under no_grad it is the gather and the GEMM, nothing recorded."""
+    sel = select_rows(h, logit_mask)
+    return linear_autograd(sel, weight, bias).view(sel.shape[0], 1, weight.shape[0])
 
 
 # ------------------------------------------------------------------------------------------------
@@ -757,45 +714,32 @@ def lm_head_ce_bwd(sel: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor
     dloss = dloss.contiguous().float()
     chunks = _ce_chunks(V, vocab_chunk)
     buf = torch.empty((M, chunks[0][1] - chunks[0][0]), dtype=torch.bfloat16, device=dev)
-    mp = (M + 7) // 8 * 8
-    if need_dw:
-        st = torch.zeros((c, mp), dtype=torch.bfloat16, device=dev)        # sel^T, contraction dim padded to 8
-        st[:, :M] = sel.t()
+    st = _kmajor(sel) if need_dw else None
     for v0, v1 in chunks:
         n = v1 - v0
         lg = ce_grad(linear(sel, weight[v0:v1], out=buf[:, :n]), labels, lse, dloss, v0)
         if need_dsel:
-            wt = weight[v0:v1].t().contiguous()                             # [c, n] = the [N, K] operand of d_logits @ W
-            dsel += linear(lg, wt).float()
+            dsel += linear(lg, _kmajor(weight[v0:v1])).float()
         if need_dw:
-            gt = torch.zeros((n, mp), dtype=torch.bfloat16, device=dev)
-            gt[:, :M] = lg.t()
-            linear(gt, st, out=dw[v0:v1])
+            linear(_kmajor(lg), st, out=dw[v0:v1])
     return (None if dsel is None else dsel.to(torch.bfloat16)), dw
 
 
-class _MaskedLMHeadCEFn(torch.autograd.Function):
+class _LMHeadCEFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, h, weight, logit_mask, labels, vocab_chunk):
-        s, b, c = h.shape
-        if b != 1:
-            raise NotImplementedError("masked_lm_head_ce: micro-batch 1")
-        idx = logit_mask.reshape(-1).nonzero().view(-1)
-        sel = row_gather(h.reshape(s, c), idx)
-        loss, lse = lm_head_ce_fwd(sel, weight, labels.reshape(-1), vocab_chunk)
-        ctx.save_for_backward(sel, weight, idx, labels.reshape(-1), lse)
-        ctx.s, ctx.vocab_chunk = s, vocab_chunk
+    def forward(ctx, sel, weight, labels, vocab_chunk):
+        labels = labels.reshape(-1)
+        loss, lse = lm_head_ce_fwd(sel, weight, labels, vocab_chunk)
+        ctx.save_for_backward(sel, weight, labels, lse)
+        ctx.vocab_chunk = vocab_chunk
         return loss.view(1, -1)
 
     @staticmethod
     def backward(ctx, dloss):
-        sel, weight, idx, labels, lse = ctx.saved_tensors
+        sel, weight, labels, lse = ctx.saved_tensors
         dsel, dw = lm_head_ce_bwd(sel, weight, labels, lse, dloss.reshape(-1), ctx.needs_input_grad[0], ctx.needs_input_grad[1],
                                   ctx.vocab_chunk)
-        gh = None
-        if dsel is not None:
-            gh = row_scatter_zero(dsel, idx, ctx.s).view(ctx.s, 1, -1)
-        return gh, dw, None, None, None
+        return dsel, dw, None, None
 
 
 def masked_lm_head_ce(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.Tensor, labels: torch.Tensor,
@@ -804,7 +748,7 @@ def masked_lm_head_ce(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.T
     :339 output_layer, :379-382 masked_select of the labels done by the caller, :412 per-token loss): h [s, 1, c],
     weight [vocab, c], logit_mask [1, s] bool, labels [1, M] (the M selected label ids) -> loss [1, M] fp32.  The
     [M, vocab] logits are never materialised (1M tokens x 152 064 would be 318 GB in bf16)."""
-    return _MaskedLMHeadCEFn.apply(h, weight, logit_mask, labels, vocab_chunk)
+    return _LMHeadCEFn.apply(select_rows(h, logit_mask), weight, labels, vocab_chunk)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -897,8 +841,7 @@ def rope_autograd(x, cos, sin):
 
 class _LinearFn(torch.autograd.Function):
     """y = x W^T + b on the wgmma GEMM; dX = dY W and dW = dY^T X reuse the same kernel on operands transposed once
-    per call (the [N, K] operand of each product must be K-contiguous); the token count is zero-padded to a multiple
-    of 8 for the weight gradient (the GEMM's K granularity)."""
+    per call (_kmajor)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):
@@ -914,7 +857,7 @@ class _LinearFn(torch.autograd.Function):
         x2 = x.reshape(-1, k_in)
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
-            dx = linear(dy2, weight.t().contiguous()).view(x.shape)          # [T, K] = dY [T, N] . (W^T)[K, N]^T
+            dx = linear(dy2, _kmajor(weight)).view(x.shape)                  # [T, K] = dY [T, N] . (W^T)[K, N]^T
         if ctx.needs_input_grad[1]:
             dw = linear_wgrad(dy2, x2)
         if ctx.has_bias and ctx.needs_input_grad[2]:
@@ -922,17 +865,24 @@ class _LinearFn(torch.autograd.Function):
         return dx, dw, db
 
 
+def _kmajor(t: torch.Tensor) -> torch.Tensor:
+    """[T, X] -> [X, T'], the K-contiguous operand of a GEMM product that contracts over T (lv_gemm_bias_act takes
+    [N, K] operands with K a multiple of 8).  T' is T rounded up to a multiple of 8; the padding columns are zero, so
+    they add exact zeros to every dot product."""
+    rows, cols = t.shape
+    if rows % 8 == 0:
+        return t.t().contiguous()
+    out = torch.zeros((cols, (rows + 7) // 8 * 8), dtype=t.dtype, device=t.device)
+    out[:, :rows] = t.t()
+    return out
+
+
 def linear_wgrad(dy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
-    """dW [N, K] = dY^T [N, T] . X [T, K] on the wgmma GEMM: both operands are transposed once so that the token
-    dimension T is the contraction, zero-padded to a multiple of 8 (the GEMM's K granularity)."""
-    t, n_out = dy2.shape
-    k_in = x2.shape[1]
-    tp = (t + 7) // 8 * 8
-    dyt = torch.zeros((n_out, tp), dtype=dy2.dtype, device=dy2.device)
-    dyt[:, :t] = dy2.t()
-    xt = torch.zeros((k_in, tp), dtype=x2.dtype, device=x2.device)
-    xt[:, :t] = x2.t()
-    return linear(dyt, xt)                                                   # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
+    """dW [N, K] = dY^T [N, T] . X [T, K] on the wgmma GEMM, the token dimension T being the contraction.  Without
+    tokens (a context-parallel rank that owns no answer token) dW is zero and no GEMM runs."""
+    if dy2.shape[0] == 0:
+        return torch.zeros((dy2.shape[1], x2.shape[1]), dtype=dy2.dtype, device=dy2.device)
+    return linear(_kmajor(dy2), _kmajor(x2))                                 # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
 
 
 def linear_autograd(x, weight, bias=None):

@@ -183,7 +183,7 @@ SUBSTITUTES = {
     "row_scatter_zero": _row_scatter_zero,
     "linear": _linear,
     "patch_embed": _patch_embed,
-    # composite wrappers (masked_linear, masked_linear_dgrad) keep their own host logic and only lose
+    # composite wrappers (masked_linear, masked_lm_head_ce) keep their own host logic and only lose
     # the "must be a CUDA tensor" guard
     "_need_cuda_bf16": lambda *ts: None,
     "_need_cuda": lambda t, dtype: None,

@@ -37,7 +37,8 @@ def test_rmsnorm_fused_residual(L):
     assert rel_fro(y, ref) < 1e-3 and mismatch_fraction(y, ref) < 0.01
 
 
-@pytest.mark.parametrize("rows,cols,eps", [(1025 * 2, 1024, 1e-6), (256, 4096, 1e-5), (7, 1152, 1e-6)])
+@pytest.mark.parametrize("rows,cols,eps", [(1025 * 2, 1024, 1e-6), (256, 4096, 1e-5), (7, 1152, 1e-6), (37, 5120, 1e-6),
+                                          (3, 8192, 1e-6)])
 def test_layernorm(L, rows, cols, eps):
     g = seeded(3)
     x = randn_bf16((rows, cols), g)
@@ -163,7 +164,7 @@ def test_row_gather_scatter_bit_exact(L):
 
 def test_rmsnorm_backward(L):
     g = seeded(31)
-    for rows, cols in ((300, 5120), (77, 640), (1000, 1024)):
+    for rows, cols in ((300, 5120), (77, 640), (1000, 1024), (129, 2048), (33, 8192)):
         x, dy = randn_bf16((rows, cols), g, 2.0), randn_bf16((rows, cols), g)
         w = (1 + 0.1 * torch.randn(cols, generator=g)).to(torch.bfloat16)
         add = randn_bf16((rows, cols), g)

@@ -85,12 +85,14 @@ def test_logit_masked_lm_head_forward_and_dgrad(L):
     w = randn_bf16((vocab, c), g, 0.05)
     mask = torch.rand(1, s, generator=g) < 0.05
     mask[0, -1] = True
-    out = L.masked_linear(h.cuda(), w.cuda(), mask.cuda())
+    hg = h.cuda().requires_grad_(True)
+    out = L.masked_linear(hg, w.cuda(), mask.cuda())
     ref = O.masked_linear_fwd(h.float(), w.float(), mask)
     assert out.shape == ref.shape
     assert rel_fro(out, ref.to(torch.bfloat16)) < 1e-3          # vs the oracle rounded once to bf16, like the other GEMM tests
     go = randn_bf16(tuple(ref.shape), g)
-    gx = L.masked_linear_dgrad(go.cuda(), w.cuda(), mask.cuda())
+    out.backward(go.cuda())
+    gx = hg.grad
     gx_ref, _ = O.masked_linear_bwd(go.float(), h.float(), w.float(), mask)
     assert gx.shape == (s, 1, c)
     assert rel_fro(gx, gx_ref.to(torch.bfloat16)) < 1e-3

@@ -161,7 +161,7 @@ def test_masked_lm_head_autograd(lib_built):
     mask[0, [5, 6, 77, 150, 299]] = True
     dy = randn_bf16((5, 1, vocab), g)
     hg, wg = h.cuda().requires_grad_(True), w.cuda().requires_grad_(True)
-    out = ops.masked_linear_autograd(hg, wg, mask.cuda())
+    out = ops.masked_linear(hg, wg, mask.cuda())
     out.backward(dy.cuda())
     ref_out = O.masked_linear_fwd(h.float(), w.float(), mask)
     gx, gw = O.masked_linear_bwd(dy.float(), h.float(), w.float(), mask)

@@ -366,8 +366,8 @@ def test_embedding_modes_equal_the_references_own_embedding(tiny):
 
 
 def test_masked_lm_head_forward_and_dgrad_equal_the_references_own_function():
-    """ops.masked_linear / masked_linear_dgrad (gather -> GEMM, GEMM -> scatter-with-zeros; kernels replaced by the
-    oracle) against committed outputs of the reference's own autograd function (layers.py:365-534)."""
+    """ops.masked_linear forward and input gradient (gather -> GEMM, GEMM -> scatter-with-zeros; kernels replaced by
+    the oracle) against committed outputs of the reference's own autograd function (layers.py:365-534)."""
     import os
     import sys
 
@@ -379,8 +379,10 @@ def test_masked_lm_head_forward_and_dgrad_equal_the_references_own_function():
     h, w, mask, dy = masked_linear_golden_inputs()
     bf = torch.bfloat16
     with oracle_ops() as ops:
-        out = ops.masked_linear(h.to(bf), w.to(bf), mask)
-        dx = ops.masked_linear_dgrad(dy.to(bf), w.to(bf), mask)
+        hb = h.to(bf).requires_grad_(True)
+        out = ops.masked_linear(hb, w.to(bf), mask)
+        out.backward(dy.to(bf))
+        dx = hb.grad
     assert out.shape == gold["out"].shape and rel_fro(out, gold["out"]) < 8e-3      # bf16 inputs vs the fp32 fixture
     assert dx.shape == gold["dx"].shape and rel_fro(dx, gold["dx"]) < 8e-3
     assert torch.equal(dx[:, 0].float().abs().sum(-1) == 0, gold["dx"][:, 0].abs().sum(-1) == 0)   # same zero rows
@@ -629,9 +631,9 @@ def test_masked_lm_head_autograd_matches_reference_formulas():
     mask[0, [3, 4, 17, 30, 39]] = True                          # M = 5: exercises the zero padding to 8
     dy = torch.randn(5, 1, vocab, generator=g).to(torch.bfloat16)
     with oracle_ops() as ops:
-        out = ops.masked_linear_autograd(h, w, mask)
+        out = ops.masked_linear(h, w, mask)
         out.backward(dy)
-        empty = ops.masked_linear_autograd(h.detach().requires_grad_(True), w.detach(), torch.zeros(1, s, dtype=torch.bool))
+        empty = ops.masked_linear(h.detach().requires_grad_(True), w.detach(), torch.zeros(1, s, dtype=torch.bool))
         assert empty.shape == (0, 1, vocab)
     ref_out = O.masked_linear_fwd(h.detach().float(), w.detach().float(), mask)
     gx, gw = O.masked_linear_bwd(dy.float(), h.detach().float(), w.detach().float(), mask)
