@@ -107,6 +107,25 @@ def test_backward_and_gemm_argument_errors(lib_built):
     assert h.lv_attn_bwd_ws_bytes(1, 40, 16384) == 40 * 16384 * 4
     b = AttnBwdParams()
     assert h.lv_attn_bwd(ctypes.byref(b), None) == -1 and b"required" in h.lv_last_error()
+    # the backward takes the forward's size limits; each case fails validation before any pointer is used
+    for kw, msg in ((dict(sq=1 << 30, q_seg_len=1 << 30), b"sequence too long"),
+                    (dict(sk=1 << 30), b"sequence too long"),
+                    (dict(sq=(1 << 30) - 1, q_seg_len=(1 << 30) - 1, batch=256), b"too many work items"),     # dQ pass
+                    (dict(sq=128, q_seg_len=128, sk=1 << 29, hq=8, hkv=8, batch=64), b"too many work items"),  # dK/dV pass
+                    (dict(q_seg_len=100), b"bad query segmentation"),
+                    (dict(d=96), b"head_dim 96 not supported")):
+        b = AttnBwdParams()
+        b.fwd = _attn_params(**kw)
+        b.fwd.lse = 0x1000
+        b.d_out = b.dq = b.dk = b.dv = b.delta_ws = 0x1000
+        assert h.lv_attn_bwd(ctypes.byref(b), None) == -1 and msg in h.lv_last_error(), (kw, h.lv_last_error())
+    b = AttnBwdParams()
+    b.fwd = _attn_params()
+    b.fwd.lse = 0x1000
+    b.d_out = b.dq = b.dk = b.dv = b.delta_ws = 0x1000
+    b.fwd.sq, b.fwd.q_seg_len, b.fwd.batch = 256, 256, 1 << 23   # 2^23 * 8 heads * 2 tiles = 2^27 items: within limits
+    b.dq_strides[0] = 12                                         # ... so the stride check is what refuses it
+    assert h.lv_attn_bwd(ctypes.byref(b), None) == -1 and b"multiples of 8" in h.lv_last_error()
     assert h.lv_gemm_bias_act(1, 1, None, 1, 4, 24, 8, 8, 8, 24, 3, None) == -1 and b"SwiGLU" in h.lv_last_error()
     assert h.lv_gemm_bias_act(1, 1, None, 1, 4, 16, 8, 8, 8, 16, 7, None) == -1 and b"unknown activation" in h.lv_last_error()
 

@@ -19,6 +19,7 @@ import pytest
 import torch
 
 from oracle import ops as O
+from tests.attn_grad_ref import _sample_rows
 from tests.util import rel_fro
 
 pytestmark = pytest.mark.gpu
@@ -42,21 +43,6 @@ def _device_inputs(S, hq, hkv, d, seed, sq=None):
     k = torch.randn((1, S, hkv, d), generator=g, device="cuda", dtype=torch.float32).to(torch.bfloat16)
     v = torch.randn((1, S, hkv, d), generator=g, device="cuda", dtype=torch.float32).to(torch.bfloat16)
     return q, k, v
-
-
-def _sample_rows(n_rows, local_len, seed, boundaries=(128, 256)):
-    """Local row indices: ends, both sides of 128- / 256-row tile boundaries, random rows."""
-    rows = {0, 1, local_len - 1, local_len - 2, local_len // 2 - 1, local_len // 2}
-    for b in boundaries:
-        for m in (1, 7, local_len // b // 2, local_len // b - 1):
-            for off in (-1, 0):
-                r = m * b + off
-                if 0 <= r < local_len:
-                    rows.add(r)
-    g = torch.Generator().manual_seed(seed)
-    while len(rows) < n_rows:
-        rows.add(int(torch.randint(0, local_len, (1,), generator=g)))
-    return torch.tensor(sorted(rows), dtype=torch.int64)
 
 
 def _check_rows(out, lse, q, k, v, rows, q_pos_of_row):
