@@ -313,6 +313,18 @@ int lv_attn_decode_merge(const void* o_part, const float* lse_part, void* out, f
 int lv_gemm_bias_act(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N,
                      int64_t K, int64_t lda, int64_t ldw, int64_t ldc, int32_t act, lv_stream_t stream);
 
+/* lv_gemm_bias_act with a layout flag per operand, for the backward products dX = dY . W and dW = dY^T . X, which
+ * contract over a dimension that is not contiguous in memory.  a_mn_major = 0: A is [M, K] (row stride lda);
+ * 1: A is stored [K, M] with M contiguous (A^T, row stride lda >= M).  w_mn_major likewise: W [N, K] or stored
+ * [K, N] (ldw >= N).  An MN-major operand needs no padding: its contraction extent K may be any value >= 1 (tails
+ * are zero-filled); K must be a multiple of 8 only while an operand is K-major.  All leading dimensions are multiples
+ * of 8 and A, W, C 16-byte aligned.  Epilogues (bias, act) are those of lv_gemm_bias_act; results equal
+ * lv_gemm_bias_act on transposed copies of the MN-major operands, bit for bit.  With both flags 0 the call is
+ * lv_gemm_bias_act. */
+int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K,
+               int64_t lda, int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, int32_t act,
+               lv_stream_t stream);
+
 /* Patch embedding of 14x14 non-overlapping patches (Conv2d(3, C, k=14, s=14),
  * modeling_intern_vit.py:79-81,98; intern_vit_model.py:139-145,203) + class token + learned
  * position embedding (modeling_intern_vit.py:100-107):
@@ -330,8 +342,8 @@ int lv_patch_embed(const void* images, const void* W, const void* bias, const vo
 
 /* The im2col step of lv_patch_embed on its own: col bf16 [n * (img/ps)^2, kpad], row p of image i = the patch's
  * 3*ps*ps pixels in (channel, y, x) order, zero-padded to kpad (a multiple of 8, >= 3*ps*ps).  With it the conv weight
- * gradient is one lv_gemm_bias_act call: dW[C, kpad] = dP^T . col, both operands transposed so that the token
- * dimension is the contraction. */
+ * gradient is one lv_gemm_ex call: dW[C, kpad] = dP^T . col, both operands MN-major (read in place) so that the
+ * token dimension is the contraction. */
 int lv_patch_im2col(const void* images, void* col, int64_t n, int64_t img, int64_t ps, int64_t kpad, lv_stream_t stream);
 
 /* Cross-entropy over vocabulary CHUNKS, fused with the logit-masked LM head (SURVEY.md 8f-3): replaces

@@ -8,6 +8,7 @@
 //                   activation, bf16 pack, swizzled st.shared, TMA store (clips the M / N tails) - while the
 //                   producer already fills the ring for the next tile
 // Tiles are rasterised in groups of M-blocks so the concurrently resident tiles share A and W panels in L2.
+// Either operand may also be MN-major (stored transposed, lv_gemm_ex): the backward products read dY, X and W in place.
 //
 // Replaces torch.matmul / te.Linear at long_vita_megatron/core/tensor_parallel/layers.py:270,409 and
 // the nn.Linear calls of modeling_intern_vit.py:131,141,190-191 / resampler_projector.py:19-23.
@@ -46,6 +47,12 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
   nb = r / gsz;
 }
 
+// A_MN / W_MN select the layout of each operand in global memory.  K-major (false): A[M][K] / W[N][K], one TMA box of
+// 64 k-columns x 128 (256) rows per tile.  MN-major (true): A stored [K][M] / W stored [K][N] with the M / N index
+// contiguous - the transposed operands of the backward products dX = dY W and dW = dY^T X - loaded as boxes of
+// 64 contiguous M / N elements (128 B) x 64 k-rows, two per A tile and four per W tile, each 8 KB box holding 8-k-row
+// groups of 1024 B; wgmma reads them with its transpose bit set.  Stage sizes, ring and barriers are the same.
+template <bool A_MN, bool W_MN>
 __global__ void __launch_bounds__(G_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmC, const __nv_bfloat16* __restrict__ bias, int M, int N,
@@ -88,8 +95,20 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full[stage], G_A_BYTES + G_B_BYTES);
-          tma_load_2d(sA + stage * G_A_BYTES, &tmA, &full[stage], kb * G_BK, mb * G_BM, kEvictNormal);
-          tma_load_2d(sB + stage * G_B_BYTES, &tmB, &full[stage], kb * G_BK, nb * G_BN, kEvictNormal);
+          if constexpr (A_MN) {
+#pragma unroll
+            for (int j = 0; j < G_BM / 64; ++j)
+              tma_load_2d(sA + stage * G_A_BYTES + j * 8192, &tmA, &full[stage], mb * G_BM + j * 64, kb * G_BK, kEvictNormal);
+          } else {
+            tma_load_2d(sA + stage * G_A_BYTES, &tmA, &full[stage], kb * G_BK, mb * G_BM, kEvictNormal);
+          }
+          if constexpr (W_MN) {
+#pragma unroll
+            for (int j = 0; j < G_BN / 64; ++j)
+              tma_load_2d(sB + stage * G_B_BYTES + j * 8192, &tmB, &full[stage], nb * G_BN + j * 64, kb * G_BK, kEvictNormal);
+          } else {
+            tma_load_2d(sB + stage * G_B_BYTES, &tmB, &full[stage], kb * G_BK, nb * G_BN, kEvictNormal);
+          }
           if (++stage == G_STAGES) {
             stage = 0;
             phase ^= 1;
@@ -106,8 +125,13 @@ __global__ void __launch_bounds__(G_THREADS, 1)
     const int r_lo = warp * 16 + (lane >> 2);       // accumulator rows r_lo and r_lo + 8 (of 64)
     const int cq = 2 * (lane & 3);                  // first of the two columns of each 8-column group
     uint8_t* stg_base = sC + cw * 2 * G_C_BYTES;
-    const uint64_t adesc0 = make_smem_desc(smem_u32(sA) + cw * 8192, 16, 1024);
-    const uint64_t bdesc0 = make_smem_desc(smem_u32(sB), 16, 1024);
+    // K-major: 128 B rows of 64 k, 8-row groups 1024 B apart, a k16 step is +32 B.  MN-major: 8-k-row groups 1024 B
+    // apart, the next 64 M / N elements one 8 KB box (LBO) away, a k16 step is 16 rows = +2048 B.  A consumer's 64 rows
+    // start 8 KB into the A tile in both layouts.
+    constexpr uint32_t a_lbo = A_MN ? 8192 : 16, b_lbo = W_MN ? 8192 : 16;
+    const uint64_t adesc0 = make_smem_desc(smem_u32(sA) + cw * 8192, a_lbo, 1024);
+    const uint64_t bdesc0 = make_smem_desc(smem_u32(sB), b_lbo, 1024);
+    constexpr int a_kstep = A_MN ? 2048 >> 4 : 32 >> 4, b_kstep = W_MN ? 2048 >> 4 : 32 >> 4;
     int stage = 0;
     uint32_t phase = 0;
     uint32_t chunk_counter = 0;
@@ -122,7 +146,8 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         const uint64_t adesc = adesc0 + (uint64_t)((stage * G_A_BYTES) >> 4);
         const uint64_t bdesc = bdesc0 + (uint64_t)((stage * G_B_BYTES) >> 4);
 #pragma unroll
-        for (int kk = 0; kk < G_BK / 16; ++kk) wgmma_ss_n256(acc, adesc + 2 * kk, bdesc + 2 * kk, (kb | kk) != 0 ? 1u : 0u);
+        for (int kk = 0; kk < G_BK / 16; ++kk)
+          wgmma_ss_n256<A_MN, W_MN>(acc, adesc + a_kstep * kk, bdesc + b_kstep * kk, (kb | kk) != 0 ? 1u : 0u);
         wgmma_commit();
         // the k-block before this one has retired: its ring slot may be refilled
         wgmma_wait<1>();
@@ -377,34 +402,36 @@ static int launch_gemv(const void* A, const void* W, const void* bias, void* C, 
   return LV_OK;
 }
 
+// TMA map of one GEMM operand with `rows` M (or N) indices: K-major [rows][K] in boxes of 64 k x `rows_box`, MN-major
+// [K][rows] in boxes of 64 rows x 64 k (see gemm_bf16_kernel).  Out-of-range rows and k are zero-filled.
+static int encode_operand(CUtensorMap* m, const void* p, int64_t rows, int64_t K, int64_t ld, bool mn_major,
+                          uint32_t rows_box) {
+  const uint64_t dims[2] = {(uint64_t)(mn_major ? rows : K), (uint64_t)(mn_major ? K : rows)};
+  const uint64_t str[2] = {2, (uint64_t)ld * 2};
+  const uint32_t box[2] = {mn_major ? 64u : (uint32_t)G_BK, mn_major ? (uint32_t)G_BK : rows_box};
+  return encode_tmap_bf16(m, p, 2, dims, str, box, true);
+}
+
+template <bool A_MN, bool W_MN>
 static int launch_gemm(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K,
                        int64_t lda, int64_t ldw, int64_t ldc, int act, cudaStream_t s) {
   CUtensorMap tmA, tmB, tmC;
-  {
-    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
-    const uint64_t str[2] = {2, (uint64_t)lda * 2};
-    const uint32_t box[2] = {G_BK, G_BM};
-    int r = encode_tmap_bf16(&tmA, A, 2, dims, str, box, true);
-    if (r) return r;
-  }
-  {
-    const uint64_t dims[2] = {(uint64_t)K, (uint64_t)N};
-    const uint64_t str[2] = {2, (uint64_t)ldw * 2};
-    const uint32_t box[2] = {G_BK, G_BN};
-    int r = encode_tmap_bf16(&tmB, W, 2, dims, str, box, true);
-    if (r) return r;
-  }
+  int r = encode_operand(&tmA, A, M, K, lda, A_MN, G_BM);
+  if (r) return r;
+  r = encode_operand(&tmB, W, N, K, ldw, W_MN, G_BN);
+  if (r) return r;
   {
     const uint64_t dims[2] = {(uint64_t)(act == 3 ? N / 2 : N), (uint64_t)M};
     const uint64_t str[2] = {2, (uint64_t)ldc * 2};
     const uint32_t box[2] = {64, 64};
-    int r = encode_tmap_bf16(&tmC, C, 2, dims, str, box, true);
+    r = encode_tmap_bf16(&tmC, C, 2, dims, str, box, true);
     if (r) return r;
   }
-  static PerDeviceOnce attr_once;
+  auto* const kernel = gemm_bf16_kernel<A_MN, W_MN>;
+  static PerDeviceOnce attr_once;  // one per instantiation
   int attr_dev;
   if (attr_once.needed(&attr_dev)) {
-    LV_CHECK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
+    LV_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, G_SMEM));
     attr_once.done(attr_dev);
   }
   const int64_t tiles = ((M + G_BM - 1) / G_BM) * ((N + G_BN - 1) / G_BN);
@@ -414,8 +441,8 @@ static int launch_gemm(const void* A, const void* W, const void* bias, void* C, 
   // sized so that the A panel takes ~16 MB of the 50 MB L2, but never fewer than 8 M-blocks.
   int gm = (int)((16ll << 20) / (256 * K));
   gm = gm < 8 ? 8 : (gm > 64 ? 64 : gm);
-  gemm_bf16_kernel<<<grid, G_THREADS, G_SMEM, s>>>(tmA, tmB, tmC, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M,
-                                                   (int)N, (int)K, act, gm);
+  kernel<<<grid, G_THREADS, G_SMEM, s>>>(tmA, tmB, tmC, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M, (int)N,
+                                         (int)K, act, gm);
   LV_CHECK_LAUNCH("gemm_bf16_kernel");
   return LV_OK;
 }
@@ -443,7 +470,39 @@ int lv_gemm_bias_act(const void* A, const void* W, const void* bias, void* C, in
   if (M <= 4 && gemv_enabled() && (N + G_BN - 1) / G_BN < sm_count() && (reinterpret_cast<uintptr_t>(A) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(W) & 15) == 0)
     return launch_gemv(A, W, bias, C, M, N, K, lda, ldw, ldc, act, (cudaStream_t)stream);
-  return launch_gemm(A, W, bias, C, M, N, K, lda, ldw, ldc, act, (cudaStream_t)stream);
+  return launch_gemm<false, false>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, (cudaStream_t)stream);
+}
+
+int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+               int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, int32_t act, lv_stream_t stream) {
+  LV_CHECK_ARG(A && W && C, "lv_gemm_ex: null pointer");
+  LV_CHECK_ARG((a_mn_major == 0 || a_mn_major == 1) && (w_mn_major == 0 || w_mn_major == 1),
+               "lv_gemm_ex: a_mn_major=%d and w_mn_major=%d must be 0 or 1", a_mn_major, w_mn_major);
+  LV_CHECK_ARG(M >= 0 && N > 0 && K > 0, "lv_gemm_ex: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
+  LV_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "lv_gemm_ex: dimension too large");
+  LV_CHECK_ARG(N % 8 == 0, "lv_gemm_ex: N=%lld must be a multiple of 8", (long long)N);
+  LV_CHECK_ARG(K % 8 == 0 || (a_mn_major && w_mn_major),
+               "lv_gemm_ex: K=%lld must be a multiple of 8 while an operand is K-major", (long long)K);
+  LV_CHECK_ARG(act >= 0 && act <= 3, "lv_gemm_ex: unknown activation %d", act);
+  LV_CHECK_ARG(lda % 8 == 0 && lda >= (a_mn_major ? M : K),
+               "lv_gemm_ex: lda=%lld must be a multiple of 8 and >= %s=%lld", (long long)lda, a_mn_major ? "M" : "K",
+               (long long)(a_mn_major ? M : K));
+  LV_CHECK_ARG(ldw % 8 == 0 && ldw >= (w_mn_major ? N : K),
+               "lv_gemm_ex: ldw=%lld must be a multiple of 8 and >= %s=%lld", (long long)ldw, w_mn_major ? "N" : "K",
+               (long long)(w_mn_major ? N : K));
+  LV_CHECK_ARG(ldc % 8 == 0 && ldc >= (act == 3 ? N / 2 : N), "lv_gemm_ex: ldc=%lld must be a multiple of 8 and >= the row length",
+               (long long)ldc);
+  LV_CHECK_ARG(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(C)) & 15) == 0,
+               "lv_gemm_ex: A, W and C must be 16-byte aligned");
+  LV_CHECK_ARG(act != 3 || (N % 16 == 0 && bias == nullptr), "lv_gemm_ex: fused SwiGLU needs N %% 16 == 0 and no bias");
+  if (!a_mn_major && !w_mn_major) return lv_gemm_bias_act(A, W, bias, C, M, N, K, lda, ldw, ldc, act, stream);
+  if (M == 0) return LV_OK;
+  LV_BIND_DEVICE(A);
+  // No GEMV for an MN-major operand: its rows are not contiguous along K; the tensor-core kernel is right for any M.
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (a_mn_major && w_mn_major) return launch_gemm<true, true>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
+  if (a_mn_major) return launch_gemm<true, false>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
+  return launch_gemm<false, true>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
 }
 
 int64_t lv_patch_embed_ws_bytes(int64_t n, int64_t img, int64_t ps, int64_t C) {
@@ -467,7 +526,7 @@ int lv_patch_embed(const void* images, const void* W, const void* bias, const vo
   im2col_patch_kernel<<<(unsigned)(n * P), 128, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(images), col, n, (int)img,
                                                        (int)ps, (int)kpad);
   LV_CHECK_LAUNCH("im2col_patch_kernel");
-  int r = launch_gemm(col, W, bias, tmp, n * P, C, kpad, kpad, kpad, C, 0, s);
+  int r = launch_gemm<false, false>(col, W, bias, tmp, n * P, C, kpad, kpad, kpad, C, 0, s);
   if (r) return r;
   add_cls_pos_kernel<<<(unsigned)(n * (P + (cls != nullptr ? 1 : 0))), 128, 0, s>>>(tmp, reinterpret_cast<const __nv_bfloat16*>(cls),
                                                            reinterpret_cast<const __nv_bfloat16*>(pos),

@@ -212,8 +212,9 @@ def register_b200_patches(patches_manager=None, vision_model: bool = False) -> N
 
     `vision_model=True` also builds the vision side (InternViT-300M + projector) as `B200VisionModel`, forward and
     backward on the fused kernels (`b200_gpt_vl_model_init_wrapper`).  It is opt-in: the provider refuses
-    configurations it does not implement (tensor parallelism > 1, recompute, vision context parallelism, other towers),
-    and with the whole tower trained its backward is currently slower than the stock modules (DESIGN.md §8)."""
+    configurations it does not implement (tensor parallelism > 1, recompute, vision context parallelism, other towers).
+    With the whole tower trained a step is still slower than the stock modules: 477 ms against 389 ms for eager bf16
+    PyTorch at 64 frames on one H100 80GB HBM3 at 700 W (DESIGN.md §8)."""
     if patches_manager is None:
         from long_vita_megatron.patch_utils import MindSpeedPatchesManager as patches_manager  # noqa: N813
     patches_manager.register_patch(

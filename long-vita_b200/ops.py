@@ -574,16 +574,27 @@ def row_scatter_zero(x: torch.Tensor, idx: torch.Tensor, n_rows_out: int):
 _ACT = {None: 0, "none": 0, "gelu": 1, "gelu_tanh": 2, "swiglu": 3}
 
 
+def _mn_major(t: torch.Tensor) -> bool:
+    """A 2-D transposed view (t.t() of a [K, rows] row-major tensor) that the GEMM reads in place as an MN-major
+    operand: rows contiguous, a column stride that is a multiple of 8 elements, a 16-byte aligned start."""
+    return t.dim() == 2 and t.stride(0) == 1 and t.stride(1) % 8 == 0 and t.stride(1) >= t.shape[0] \
+        and t.data_ptr() % 16 == 0
+
+
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, act: Optional[str] = None,
            out: Optional[torch.Tensor] = None):
-    """act(x @ weight.T + bias); weight is [N, K] (nn.Linear layout)."""
+    """act(x @ weight.T + bias); weight is [N, K] (nn.Linear layout).  Either operand may also be a 2-D transposed
+    view (stride(0) == 1, stride(1) a multiple of 8, e.g. t.t() of a contiguous [K, X]): the kernel reads it in place
+    (lv_gemm_ex) instead of a contiguous copy.  Any other layout is copied to a contiguous tensor first."""
     _need_cuda_bf16(x, weight, bias)
     K = x.shape[-1]
     N = weight.shape[0]
     x2 = x.reshape(-1, K)
-    if x2.stride(1) != 1 or x2.stride(0) % 8 != 0:
+    a_mn = x2.stride(1) != 1 and _mn_major(x2)
+    if not a_mn and (x2.stride(1) != 1 or x2.stride(0) % 8 != 0):
         x2 = x2.contiguous()
-    if weight.stride(1) != 1:
+    w_mn = weight.stride(1) != 1 and _mn_major(weight)
+    if not w_mn and weight.stride(1) != 1:
         weight = weight.contiguous()
     M = x2.shape[0]
     n_out = N // 2 if act == "swiglu" else N      # fused SwiGLU: weight rows interleaved (gate_i, up_i)
@@ -592,11 +603,19 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
     if M == 0:      # e.g. a context-parallel rank that owns no answer token (empty logit mask)
         return out.view(*x.shape[:-1], n_out)
     ev0 = _TIMER.start() if _TIMER is not None else None
-    _lib.check(
-        _lib.lib().lv_gemm_bias_act(x2.data_ptr(), weight.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K, x2.stride(0),
-                                    weight.stride(0), out.stride(0), _ACT[act], _stream()),
-        "lv_gemm_bias_act",
-    )
+    if a_mn or w_mn:
+        _lib.check(
+            _lib.lib().lv_gemm_ex(x2.data_ptr(), weight.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K,
+                                  x2.stride(1) if a_mn else x2.stride(0), weight.stride(1) if w_mn else weight.stride(0),
+                                  out.stride(0), int(a_mn), int(w_mn), _ACT[act], _stream()),
+            "lv_gemm_ex",
+        )
+    else:
+        _lib.check(
+            _lib.lib().lv_gemm_bias_act(x2.data_ptr(), weight.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K,
+                                        x2.stride(0), weight.stride(0), out.stride(0), _ACT[act], _stream()),
+            "lv_gemm_bias_act",
+        )
     if ev0 is not None:
         _TIMER.stop("gemm_bf16", 2.0 * M * N * K, ev0)
     return out.view(*x.shape[:-1], n_out)
@@ -714,14 +733,13 @@ def lm_head_ce_bwd(sel: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor
     dloss = dloss.contiguous().float()
     chunks = _ce_chunks(V, vocab_chunk)
     buf = torch.empty((M, chunks[0][1] - chunks[0][0]), dtype=torch.bfloat16, device=dev)
-    st = _kmajor(sel) if need_dw else None
     for v0, v1 in chunks:
         n = v1 - v0
         lg = ce_grad(linear(sel, weight[v0:v1], out=buf[:, :n]), labels, lse, dloss, v0)
         if need_dsel:
-            dsel += linear(lg, _kmajor(weight[v0:v1])).float()
+            dsel += linear(lg, weight[v0:v1].t()).float()           # the weight chunk read in place, MN-major
         if need_dw:
-            linear(_kmajor(lg), st, out=dw[v0:v1])
+            linear(lg.t(), sel.t(), out=dw[v0:v1])                  # both MN-major, the M rows are the contraction
     return (None if dsel is None else dsel.to(torch.bfloat16)), dw
 
 
@@ -840,8 +858,8 @@ def rope_autograd(x, cos, sin):
 
 
 class _LinearFn(torch.autograd.Function):
-    """y = x W^T + b on the wgmma GEMM; dX = dY W and dW = dY^T X reuse the same kernel on operands transposed once
-    per call (_kmajor)."""
+    """y = x W^T + b on the wgmma GEMM; dX = dY W and dW = dY^T X reuse the same kernel, which reads the transposed
+    operands (W^T, dY^T, X^T) in place as MN-major views."""
 
     @staticmethod
     def forward(ctx, x, weight, bias):
@@ -857,7 +875,7 @@ class _LinearFn(torch.autograd.Function):
         x2 = x.reshape(-1, k_in)
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
-            dx = linear(dy2, _kmajor(weight)).view(x.shape)                  # [T, K] = dY [T, N] . (W^T)[K, N]^T
+            dx = linear(dy2, weight.t()).view(x.shape)                       # [T, K] = dY [T, N] . (W^T)[K, N]^T
         if ctx.needs_input_grad[1]:
             dw = linear_wgrad(dy2, x2)
         if ctx.has_bias and ctx.needs_input_grad[2]:
@@ -865,24 +883,15 @@ class _LinearFn(torch.autograd.Function):
         return dx, dw, db
 
 
-def _kmajor(t: torch.Tensor) -> torch.Tensor:
-    """[T, X] -> [X, T'], the K-contiguous operand of a GEMM product that contracts over T (lv_gemm_bias_act takes
-    [N, K] operands with K a multiple of 8).  T' is T rounded up to a multiple of 8; the padding columns are zero, so
-    they add exact zeros to every dot product."""
-    rows, cols = t.shape
-    if rows % 8 == 0:
-        return t.t().contiguous()
-    out = torch.zeros((cols, (rows + 7) // 8 * 8), dtype=t.dtype, device=t.device)
-    out[:, :rows] = t.t()
-    return out
-
-
 def linear_wgrad(dy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
-    """dW [N, K] = dY^T [N, T] . X [T, K] on the wgmma GEMM, the token dimension T being the contraction.  Without
-    tokens (a context-parallel rank that owns no answer token) dW is zero and no GEMM runs."""
+    """dW [N, K] = dY^T [N, T] . X [T, K] on the wgmma GEMM, the token dimension T being the contraction: dY^T and X^T
+    are read in place as MN-major operands, so T may be any length.  Without tokens (a context-parallel rank that
+    owns no answer token) dW is zero and no GEMM runs."""
     if dy2.shape[0] == 0:
         return torch.zeros((dy2.shape[1], x2.shape[1]), dtype=dy2.dtype, device=dy2.device)
-    return linear(_kmajor(dy2), _kmajor(x2))                                 # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
+    dy2, x2 = (t if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0 else t.contiguous()
+               for t in (dy2, x2))
+    return linear(dy2.t(), x2.t())                                           # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
 
 
 def linear_autograd(x, weight, bias=None):
