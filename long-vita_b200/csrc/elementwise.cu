@@ -877,7 +877,7 @@ extern "C" {
 
 int lv_rmsnorm(const void* x, const void* residual, const void* w, void* y, void* sum_out, int64_t rows,
                int64_t cols, float eps, lv_stream_t stream) {
-  LV_CHECK_ARG(x && w && y, "lv_rmsnorm: null pointer");
+  LV_CHECK_ARG(w && (rows == 0 || (x && y)), "lv_rmsnorm: null pointer");  // an empty tensor may have no storage
   LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0 && cols <= 16384, "lv_rmsnorm: cols=%lld must be a multiple of 8 and <= 16384", (long long)cols);
   LV_CHECK_ARG(aligned16(x) && aligned16(w) && aligned16(y) && aligned16(residual) && aligned16(sum_out), "lv_rmsnorm: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
@@ -892,7 +892,7 @@ int lv_rmsnorm(const void* x, const void* residual, const void* w, void* y, void
 
 int lv_layernorm(const void* x, const void* w, const void* b, void* y, int64_t rows, int64_t cols, float eps,
                  lv_stream_t stream) {
-  LV_CHECK_ARG(x && w && y, "lv_layernorm: null pointer");
+  LV_CHECK_ARG(w && (rows == 0 || (x && y)), "lv_layernorm: null pointer");
   LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0 && cols <= 16384, "lv_layernorm: cols=%lld must be a multiple of 8 and <= 16384", (long long)cols);
   LV_CHECK_ARG(aligned16(x) && aligned16(w) && aligned16(y) && aligned16(b), "lv_layernorm: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
@@ -906,7 +906,7 @@ int lv_layernorm(const void* x, const void* w, const void* b, void* y, int64_t r
 
 int lv_rope_table(const int64_t* pos, const float* inv_freq, void* cos_out, void* sin_out, int64_t n, int64_t dim,
                   lv_stream_t stream) {
-  LV_CHECK_ARG(pos && inv_freq && cos_out && sin_out, "lv_rope_table: null pointer");
+  LV_CHECK_ARG(inv_freq && (n == 0 || (pos && cos_out && sin_out)), "lv_rope_table: null pointer");
   LV_CHECK_ARG(n >= 0 && dim > 0 && dim % 2 == 0, "lv_rope_table: bad dim %lld", (long long)dim);
   if (n == 0) return LV_OK;
   const int64_t total = n * (dim / 2);
@@ -919,7 +919,7 @@ int lv_rope_table(const int64_t* pos, const float* inv_freq, void* cos_out, void
 int lv_rope(const void* x, void* out, const void* cos_t, const void* sin_t, int64_t n_tok, int64_t heads, int64_t dim,
             int64_t x_tok_stride, int64_t x_head_stride, int64_t o_tok_stride, int64_t o_head_stride,
             lv_stream_t stream) {
-  LV_CHECK_ARG(x && out && cos_t && sin_t, "lv_rope: null pointer");
+  LV_CHECK_ARG(n_tok == 0 || heads == 0 || (x && out && cos_t && sin_t), "lv_rope: null pointer");
   LV_CHECK_ARG(dim > 0 && dim % 16 == 0, "lv_rope: dim=%lld must be a multiple of 16", (long long)dim);
   LV_CHECK_ARG(x_tok_stride % 8 == 0 && x_head_stride % 8 == 0 && o_tok_stride % 8 == 0 && o_head_stride % 8 == 0,
                "lv_rope: strides must be multiples of 8 elements");
@@ -943,7 +943,7 @@ int lv_rope(const void* x, void* out, const void* cos_t, const void* sin_t, int6
 }
 
 int lv_swiglu(const void* gate_up, void* out, int64_t rows, int64_t inter, lv_stream_t stream) {
-  LV_CHECK_ARG(gate_up && out, "lv_swiglu: null pointer");
+  LV_CHECK_ARG(rows == 0 || (gate_up && out), "lv_swiglu: null pointer");
   LV_CHECK_ARG(inter > 0 && inter % 8 == 0, "lv_swiglu: inter=%lld must be a multiple of 8", (long long)inter);
   LV_CHECK_ARG(aligned16(gate_up) && aligned16(out), "lv_swiglu: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
@@ -955,7 +955,7 @@ int lv_swiglu(const void* gate_up, void* out, int64_t rows, int64_t inter, lv_st
 
 int lv_bias_gelu(const void* x, const void* bias, void* y, int64_t rows, int64_t cols, int32_t approx,
                  lv_stream_t stream) {
-  LV_CHECK_ARG(x && y, "lv_bias_gelu: null pointer");
+  LV_CHECK_ARG(rows == 0 || (x && y), "lv_bias_gelu: null pointer");
   LV_CHECK_ARG(cols > 0 && cols % 8 == 0, "lv_bias_gelu: cols=%lld must be a multiple of 8", (long long)cols);
   LV_CHECK_ARG(aligned16(x) && aligned16(y) && aligned16(bias), "lv_bias_gelu: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
@@ -968,7 +968,7 @@ int lv_bias_gelu(const void* x, const void* bias, void* y, int64_t rows, int64_t
 
 int lv_ls_residual(const void* x, const void* y, const void* bias, const void* ls, void* out, int64_t rows,
                    int64_t cols, lv_stream_t stream) {
-  LV_CHECK_ARG(x && y && out, "lv_ls_residual: null pointer");
+  LV_CHECK_ARG(rows == 0 || (x && y && out), "lv_ls_residual: null pointer");
   LV_CHECK_ARG(cols > 0 && cols % 8 == 0, "lv_ls_residual: cols=%lld must be a multiple of 8", (long long)cols);
   LV_CHECK_ARG(aligned16(x) && aligned16(y) && aligned16(out) && aligned16(bias) && aligned16(ls), "lv_ls_residual: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
@@ -1055,10 +1055,10 @@ int64_t lv_rmsnorm_bwd_partials(int64_t rows, int64_t cols) { return bwd_partial
 
 int lv_rmsnorm_bwd(const void* x, const void* w, const void* dy, const void* add_in, void* dx, float* dw_partials,
                    int64_t rows, int64_t cols, float eps, lv_stream_t stream) {
-  LV_CHECK_ARG(x && w && dy && dx && dw_partials, "lv_rmsnorm_bwd: null pointer");
+  LV_CHECK_ARG(w && dw_partials && (rows == 0 || (x && dy && dx)), "lv_rmsnorm_bwd: null pointer");
   LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0 && cols <= 16384, "lv_rmsnorm_bwd: cols=%lld must be a multiple of 8 and <= 16384", (long long)cols);
   LV_CHECK_ARG(aligned16(x) && aligned16(w) && aligned16(dy) && aligned16(dx) && aligned16(add_in), "lv_rmsnorm_bwd: pointers must be 16-byte aligned");
-  LV_BIND_DEVICE(x);
+  LV_BIND_DEVICE(dw_partials);  // the partial buffer exists (and is zeroed) even with zero rows
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t parts = lv_rmsnorm_bwd_partials(rows, cols);
   if (rows == 0) {
@@ -1074,7 +1074,7 @@ int lv_rmsnorm_bwd(const void* x, const void* w, const void* dy, const void* add
 }
 
 int lv_swiglu_bwd(const void* gate_up, const void* dh, void* d_gate_up, int64_t rows, int64_t inter, lv_stream_t stream) {
-  LV_CHECK_ARG(gate_up && dh && d_gate_up, "lv_swiglu_bwd: null pointer");
+  LV_CHECK_ARG(rows == 0 || (gate_up && dh && d_gate_up), "lv_swiglu_bwd: null pointer");
   LV_CHECK_ARG(inter > 0 && inter % 8 == 0, "lv_swiglu_bwd: inter=%lld must be a multiple of 8", (long long)inter);
   LV_CHECK_ARG(aligned16(gate_up) && aligned16(dh) && aligned16(d_gate_up), "lv_swiglu_bwd: pointers must be 16-byte aligned");
   if (rows == 0) return LV_OK;
@@ -1120,12 +1120,12 @@ int64_t lv_layernorm_bwd_partials(int64_t rows, int64_t cols) { return bwd_parti
 
 int lv_layernorm_bwd(const void* x, const void* w, const void* dy, const void* add_in, void* dx, float* dw_partials,
                      float* db_partials, int64_t rows, int64_t cols, float eps, lv_stream_t stream) {
-  LV_CHECK_ARG(x && w && dy && dw_partials && db_partials, "lv_layernorm_bwd: null pointer");
+  LV_CHECK_ARG(w && dw_partials && db_partials && (rows == 0 || (x && dy)), "lv_layernorm_bwd: null pointer");
   LV_CHECK_ARG(dx != nullptr || add_in == nullptr, "lv_layernorm_bwd: add_in needs dx");
   LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0 && cols <= 8192, "lv_layernorm_bwd: cols=%lld must be a multiple of 8 and <= 8192", (long long)cols);
   LV_CHECK_ARG(aligned16(x) && aligned16(w) && aligned16(dy) && aligned16(dx) && aligned16(add_in) && aligned16(dw_partials) &&
                    aligned16(db_partials), "lv_layernorm_bwd: pointers must be 16-byte aligned");
-  LV_BIND_DEVICE(x);
+  LV_BIND_DEVICE(dw_partials);  // the partial buffer exists (and is zeroed) even with zero rows
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t parts = lv_layernorm_bwd_partials(rows, cols);
   if (rows == 0) {
@@ -1142,7 +1142,7 @@ int lv_layernorm_bwd(const void* x, const void* w, const void* dy, const void* a
 }
 
 int lv_gelu_bwd(const void* pre, const void* dy, void* dx, int64_t rows, int64_t cols, int32_t approx, lv_stream_t stream) {
-  LV_CHECK_ARG(pre && dy && dx, "lv_gelu_bwd: null pointer");
+  LV_CHECK_ARG(rows == 0 || (pre && dy && dx), "lv_gelu_bwd: null pointer");
   LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0, "lv_gelu_bwd: cols=%lld must be a multiple of 8", (long long)cols);
   LV_CHECK_ARG(approx == 0 || approx == 1, "lv_gelu_bwd: approx=%d must be 0 (erf) or 1 (tanh)", approx);
   LV_CHECK_ARG(aligned16(pre) && aligned16(dy) && aligned16(dx), "lv_gelu_bwd: pointers must be 16-byte aligned");
@@ -1167,11 +1167,11 @@ int64_t lv_ls_residual_bwd_partials(int64_t rows, int64_t cols) {
 
 int lv_ls_residual_bwd(const void* dout, const void* y, const void* ls, void* dy, float* dls_partials, int64_t rows,
                        int64_t cols, lv_stream_t stream) {
-  LV_CHECK_ARG(dout && y && ls && dy && dls_partials, "lv_ls_residual_bwd: null pointer");
+  LV_CHECK_ARG(ls && dls_partials && (rows == 0 || (dout && y && dy)), "lv_ls_residual_bwd: null pointer");
   LV_CHECK_ARG(rows >= 0 && cols > 0 && cols % 8 == 0, "lv_ls_residual_bwd: cols=%lld must be a multiple of 8", (long long)cols);
   LV_CHECK_ARG(aligned16(dout) && aligned16(y) && aligned16(ls) && aligned16(dy) && aligned16(dls_partials),
                "lv_ls_residual_bwd: pointers must be 16-byte aligned");
-  LV_BIND_DEVICE(dout);
+  LV_BIND_DEVICE(dls_partials);  // the partial buffer exists (and is zeroed) even with zero rows
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t gy = lv_ls_residual_bwd_partials(rows, cols);
   if (rows == 0) {
