@@ -71,7 +71,7 @@ typedef struct lv_attn_params {
   int64_t k_strides[3];
   int64_t v_strides[3];
   int64_t o_strides[3];
-  float scale;            /* softmax scale, e.g. 1/sqrt(d) */
+  float scale;            /* softmax scale, e.g. 1/sqrt(d); finite and > 0, else LV_EINVAL */
   int32_t causal;         /* 0 / 1 */
   int64_t q_seg_len;      /* rows per query segment (sq if one segment); multiple of 128 if < sq */
   int64_t q_seg_pos[2];   /* global position of the first row of each query segment */

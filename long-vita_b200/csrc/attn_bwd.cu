@@ -507,6 +507,7 @@ static int check_bwd_params(const lv_attn_bwd_params* a) {
   LV_CHECK_ARG(a->d_out && a->dq && a->dk && a->dv && a->delta_ws, "lv_attn_bwd: null gradient / workspace pointer");
   LV_CHECK_ARG(f->d == 64 || f->d == 128, "lv_attn_bwd: head_dim %lld not supported (64, 128)", (long long)f->d);
   LV_CHECK_ARG(f->batch > 0 && f->sq > 0 && f->sk > 0 && f->hq > 0 && f->hkv > 0 && f->hq % f->hkv == 0, "lv_attn_bwd: bad shape");
+  LV_CHECK_ARG(f->scale > 0.f && isfinite(f->scale), "lv_attn_bwd: scale %g must be finite and > 0", (double)f->scale);
   // launch_bwd hands sizes, row indices and work-item counts to the kernels as int
   LV_CHECK_ARG(f->sq < (1ll << 30) && f->sk < (1ll << 30), "lv_attn_bwd: sequence too long");
   LV_CHECK_ARG(f->batch * f->hq * ((f->sq + 127) / 128) < (1ll << 31) && f->batch * f->hkv * ((f->sk + 127) / 128) < (1ll << 31),

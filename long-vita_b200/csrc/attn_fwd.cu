@@ -735,6 +735,8 @@ static int check_attn_params(const lv_attn_params* a) {
   LV_CHECK_ARG(a->d == 64 || a->d == 128, "lv_attn_fwd: head_dim %lld not supported (64, 128)", (long long)a->d);
   LV_CHECK_ARG(a->batch > 0 && a->sq > 0 && a->sk > 0 && a->hq > 0 && a->hkv > 0, "lv_attn_fwd: empty shape");
   LV_CHECK_ARG(a->hq % a->hkv == 0, "lv_attn_fwd: hq=%lld is not a multiple of hkv=%lld", (long long)a->hq, (long long)a->hkv);
+  // masked scores are -inf before s * scale_log2 - m: a zero scale makes them NaN, a negative one gives them p = +inf
+  LV_CHECK_ARG(a->scale > 0.f && isfinite(a->scale), "lv_attn_fwd: scale %g must be finite and > 0", (double)a->scale);
   LV_CHECK_ARG(a->sq < (1ll << 30) && a->sk < (1ll << 30), "lv_attn_fwd: sequence too long");
   LV_CHECK_ARG(a->batch * a->hq * ((a->sq + 127) / 128) < (1ll << 31), "lv_attn_fwd: too many work items");
   LV_CHECK_ARG(a->q_seg_len > 0 && a->q_seg_len <= a->sq, "lv_attn_fwd: q_seg_len=%lld out of range", (long long)a->q_seg_len);

@@ -86,6 +86,10 @@ def _attn_params(**kw):
     (dict(q=None), b"null tensor pointer"),
     (dict(q_seg_len=300), b"out of range"),
     (dict(q_seg_len=100), b"q_seg_len % 128 == 0"),
+    (dict(scale=0.0), b"must be finite and > 0"),
+    (dict(scale=-0.1), b"must be finite and > 0"),
+    (dict(scale=float("nan")), b"must be finite and > 0"),
+    (dict(scale=float("inf")), b"must be finite and > 0"),
 ])
 def test_attention_argument_errors_have_the_documented_code_and_text(lib_built, kw, msg):
     """INTEGRATION.md section 4: every entry point returns a negative LV_E* code and sets lv_last_error()."""
@@ -97,6 +101,18 @@ def test_attention_argument_errors_have_the_documented_code_and_text(lib_built, 
     assert rc == -1 and msg in h.lv_last_error(), h.lv_last_error()
     with pytest.raises(RuntimeError, match="lv_attn_fwd failed"):
         _lib.check(rc, "lv_attn_fwd")
+    if "scale" in kw:
+        # the document-masked and context-parallel forwards and the backward refuse the same scales
+        from long_vita_b200._lib import AttnBwdParams, AttnDocs, CpParams
+
+        assert h.lv_attn_docs_fwd(ctypes.byref(p), ctypes.byref(AttnDocs()), None) == -1 and msg in h.lv_last_error()
+        assert h.lv_attn_cp_fwd(ctypes.byref(p), ctypes.byref(CpParams()), None) == -1 and msg in h.lv_last_error()
+        b = AttnBwdParams()
+        b.fwd = p
+        b.fwd.lse = 0x1000
+        b.d_out = b.dq = b.dk = b.dv = b.delta_ws = 0x1000
+        assert h.lv_attn_bwd(ctypes.byref(b), None) == -1 and msg in h.lv_last_error()
+        assert h.lv_attn_docs_bwd(ctypes.byref(b), ctypes.byref(AttnDocs()), None) == -1 and msg in h.lv_last_error()
 
 
 def test_backward_and_gemm_argument_errors(lib_built):
