@@ -325,6 +325,16 @@ int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t 
                int64_t lda, int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, int32_t act,
                lv_stream_t stream);
 
+/* Weight-gradient accumulation into an fp32 master gradient (Megatron's gradient_accumulation_fusion, the
+ * `main_grad` of layers.py:486-518): C[M, N] += A . W^T in fp32, with the operands, layouts, mainloop and k-order of
+ * lv_gemm_ex, so the accumulator added is exactly the value lv_gemm_ex rounds to bf16.  Each element becomes one IEEE
+ * fp32 round-to-nearest add prior + acc (subnormals kept), deterministic.  Only a_mn_major = w_mn_major = 1 is built
+ * (dW = dY^T . X with dY and X read in place); K may be any value >= 0 (K = 0 or M = 0: no launch).  C is fp32 with
+ * row stride ldc (a multiple of 4, >= N), N a multiple of 4, lda / ldw multiples of 8, A, W, C 16-byte aligned;
+ * columns and rows outside [M, N] are not touched. */
+int lv_gemm_wgrad_acc_f32(const void* A, const void* W, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                          int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, lv_stream_t stream);
+
 /* Patch embedding of 14x14 non-overlapping patches (Conv2d(3, C, k=14, s=14),
  * modeling_intern_vit.py:79-81,98; intern_vit_model.py:139-145,203) + class token + learned
  * position embedding (modeling_intern_vit.py:100-107):

@@ -109,6 +109,7 @@ SIGNATURES = {
     "lv_gemm_bias_act": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_ptr]),
     "lv_gemm_ex": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_i32, c_i32,
                            c_ptr]),
+    "lv_gemm_wgrad_acc_f32": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_i32, c_ptr]),
     "lv_patch_embed_ws_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i64]),
     "lv_patch_embed": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr]),
 }

@@ -15,6 +15,7 @@
 #include <cuda_bf16.h>
 #include <math.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "ptx.cuh"
@@ -26,6 +27,7 @@ constexpr int G_A_BYTES = G_BM * G_BK * 2;          // 16 KB
 constexpr int G_B_BYTES = G_BN * G_BK * 2;          // 32 KB
 constexpr int G_C_BYTES = 64 * 64 * 2;              // 8 KB staging per 64 x 64 output chunk (two per consumer)
 constexpr int G_THREADS = 384;
+constexpr int G_ACC_PREFETCH_KB = 8;                // accumulate epilogue: L2 prefetch of accC this many k-blocks early
 constexpr int G_SMEM = G_STAGES * (G_A_BYTES + G_B_BYTES) + 4 * G_C_BYTES + 256 + 1024;  // + barriers + align slack
 
 __device__ __forceinline__ float act_apply(float t, int act) {
@@ -52,11 +54,16 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
 // contiguous - the transposed operands of the backward products dX = dY W and dW = dY^T X - loaded as boxes of
 // 64 contiguous M / N elements (128 B) x 64 k-rows, two per A tile and four per W tile, each 8 KB box holding 8-k-row
 // groups of 1024 B; wgmma reads them with its transpose bit set.  Stage sizes, ring and barriers are the same.
-template <bool A_MN, bool W_MN>
+//
+// ACC selects the gradient-accumulation epilogue (lv_gemm_wgrad_acc_f32): accC[M, N] (fp32, row stride ldc) +=
+// the fp32 accumulator, with no bias, activation or bf16 rounding; tmC, bias and act are unused.  Mainloop, ring,
+// rasterisation and k-order are those of the bf16 epilogue, so the accumulator is the value whose bf16 rounding
+// that epilogue stores.
+template <bool A_MN, bool W_MN, bool ACC = false>
 __global__ void __launch_bounds__(G_THREADS, 1)
     gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ CUtensorMap tmC, const __nv_bfloat16* __restrict__ bias, int M, int N,
-                     int K, int act, int gm) {
+                     int K, int act, int gm, float* accC, long long ldc) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
@@ -74,7 +81,7 @@ __global__ void __launch_bounds__(G_THREADS, 1)
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmC);
+    if constexpr (!ACC) tma_prefetch_desc(&tmC);
     for (int i = 0; i < G_STAGES; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 2);
@@ -149,6 +156,19 @@ __global__ void __launch_bounds__(G_THREADS, 1)
         for (int kk = 0; kk < G_BK / 16; ++kk)
           wgmma_ss_n256<A_MN, W_MN>(acc, adesc + a_kstep * kk, bdesc + b_kstep * kk, (kb | kk) != 0 ? 1u : 0u);
         wgmma_commit();
+        if constexpr (ACC) {
+          // G_ACC_PREFETCH_KB k-blocks before the epilogue, pull this consumer's 64 x 256 fp32 block of accC into L2
+          // (one 128-byte line per thread and step, 8 lines per 1 KB row): the epilogue's reads then hit L2 instead of
+          // waiting on DRAM while the tensor cores idle
+          if (kb == (num_kb > G_ACC_PREFETCH_KB ? num_kb - G_ACC_PREFETCH_KB : 0)) {
+            const int prow = mb * G_BM + cw * 64 + (wg_tid >> 1);
+#pragma unroll
+            for (int l = 0; l < 4; ++l) {
+              const int pcol = nb * G_BN + ((wg_tid & 1) * 4 + l) * 32;
+              if (prow < M && pcol < N) asm volatile("prefetch.global.L2 [%0];" ::"l"(accC + prow * ldc + pcol));
+            }
+          }
+        }
         // the k-block before this one has retired: its ring slot may be refilled
         wgmma_wait<1>();
         wgmma_keep(acc);
@@ -164,6 +184,45 @@ __global__ void __launch_bounds__(G_THREADS, 1)
       if (wg_tid == 0) mbar_arrive(&empty[prev_stage]);
 
       // ------------------------------- epilogue -----------------------------------
+      if constexpr (ACC) {
+        // accC += acc as a plain read-add-write from registers, not a TMA reduce-add: cp.reduce.async.bulk .add.f32
+        // flushes subnormal inputs and results to zero, while add.rn.f32 (no .ftz) is one IEEE-754 round-to-nearest-
+        // even add that keeps subnormals, so every element becomes exactly prior + acc, as torch computes it.  Each
+        // element has one writer per launch (deterministic).  A quad's two-column pairs span 8 consecutive fp32 = one
+        // full 32-byte sector per row, so the 8-byte accesses waste no DRAM traffic; the staging buffers are unused.
+        // Per 64-column chunk, the 16 loads are issued before the adds and stores.
+        const int row0 = mb * G_BM + cw * 64 + r_lo;
+#pragma unroll
+        for (int c = 0; c < G_BN / 64; ++c) {
+          float2 prior[16];
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int col = nb * G_BN + 64 * c + 8 * jj + cq;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row0 + 8 * h;
+              prior[2 * jj + h] = make_float2(0.f, 0.f);
+              if (row < M && col < N) prior[2 * jj + h] = *reinterpret_cast<const float2*>(accC + row * ldc + col);
+            }
+          }
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = c * 8 + jj;
+            const int col = nb * G_BN + 64 * c + 8 * jj + cq;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = row0 + 8 * h;
+              if (row < M && col < N) {
+                float2 v = prior[2 * jj + h];
+                asm("add.rn.f32 %0, %0, %1;" : "+f"(v.x) : "f"(acc[4 * j + 2 * h]));
+                asm("add.rn.f32 %0, %0, %1;" : "+f"(v.y) : "f"(acc[4 * j + 2 * h + 1]));
+                *reinterpret_cast<float2*>(accC + row * ldc + col) = v;
+              }
+            }
+          }
+        }
+        continue;
+      }
       // Output chunks of 64 x 64: staged (128-byte swizzle, the layout of the TMA map) and stored with TMA.  The
       // chunk loops are unrolled so that every accumulator index is a compile-time constant (registers, not stack).
       auto stage_begin = [&]() -> uint8_t* {
@@ -412,7 +471,8 @@ static int encode_operand(CUtensorMap* m, const void* p, int64_t rows, int64_t K
   return encode_tmap_bf16(m, p, 2, dims, str, box, true);
 }
 
-template <bool A_MN, bool W_MN>
+// ACC: C is fp32 and accumulated into (gemm_bf16_kernel); bias and act must be null / 0.
+template <bool A_MN, bool W_MN, bool ACC = false>
 static int launch_gemm(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K,
                        int64_t lda, int64_t ldw, int64_t ldc, int act, cudaStream_t s) {
   CUtensorMap tmA, tmB, tmC;
@@ -420,14 +480,16 @@ static int launch_gemm(const void* A, const void* W, const void* bias, void* C, 
   if (r) return r;
   r = encode_operand(&tmB, W, N, K, ldw, W_MN, G_BN);
   if (r) return r;
-  {
+  if constexpr (ACC) {
+    memset(&tmC, 0, sizeof(tmC));
+  } else {
     const uint64_t dims[2] = {(uint64_t)(act == 3 ? N / 2 : N), (uint64_t)M};
     const uint64_t str[2] = {2, (uint64_t)ldc * 2};
     const uint32_t box[2] = {64, 64};
     r = encode_tmap_bf16(&tmC, C, 2, dims, str, box, true);
     if (r) return r;
   }
-  auto* const kernel = gemm_bf16_kernel<A_MN, W_MN>;
+  auto* const kernel = gemm_bf16_kernel<A_MN, W_MN, ACC>;
   static PerDeviceOnce attr_once;  // one per instantiation
   int attr_dev;
   if (attr_once.needed(&attr_dev)) {
@@ -442,7 +504,8 @@ static int launch_gemm(const void* A, const void* W, const void* bias, void* C, 
   int gm = (int)((16ll << 20) / (256 * K));
   gm = gm < 8 ? 8 : (gm > 64 ? 64 : gm);
   kernel<<<grid, G_THREADS, G_SMEM, s>>>(tmA, tmB, tmC, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M, (int)N,
-                                         (int)K, act, gm);
+                                         (int)K, act, gm, ACC ? reinterpret_cast<float*>(C) : nullptr,
+                                         ACC ? (long long)ldc : 0ll);
   LV_CHECK_LAUNCH("gemm_bf16_kernel");
   return LV_OK;
 }
@@ -503,6 +566,30 @@ int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t 
   if (a_mn_major && w_mn_major) return launch_gemm<true, true>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
   if (a_mn_major) return launch_gemm<true, false>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
   return launch_gemm<false, true>(A, W, bias, C, M, N, K, lda, ldw, ldc, act, s);
+}
+
+int lv_gemm_wgrad_acc_f32(const void* A, const void* W, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
+                          int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, lv_stream_t stream) {
+  LV_CHECK_ARG(A && W && C, "lv_gemm_wgrad_acc_f32: null pointer");
+  LV_CHECK_ARG((a_mn_major == 0 || a_mn_major == 1) && (w_mn_major == 0 || w_mn_major == 1),
+               "lv_gemm_wgrad_acc_f32: a_mn_major=%d and w_mn_major=%d must be 0 or 1", a_mn_major, w_mn_major);
+  LV_CHECK_ARG(a_mn_major && w_mn_major,
+               "lv_gemm_wgrad_acc_f32: only MN-major A and W are built (dW = dY^T . X with dY and X read in place)");
+  LV_CHECK_ARG(M >= 0 && N > 0 && K >= 0, "lv_gemm_wgrad_acc_f32: bad shape M=%lld N=%lld K=%lld", (long long)M,
+               (long long)N, (long long)K);
+  LV_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "lv_gemm_wgrad_acc_f32: dimension too large");
+  LV_CHECK_ARG(N % 4 == 0, "lv_gemm_wgrad_acc_f32: N=%lld must be a multiple of 4", (long long)N);
+  LV_CHECK_ARG(lda % 8 == 0 && lda >= M, "lv_gemm_wgrad_acc_f32: lda=%lld must be a multiple of 8 and >= M=%lld",
+               (long long)lda, (long long)M);
+  LV_CHECK_ARG(ldw % 8 == 0 && ldw >= N, "lv_gemm_wgrad_acc_f32: ldw=%lld must be a multiple of 8 and >= N=%lld",
+               (long long)ldw, (long long)N);
+  LV_CHECK_ARG(ldc % 4 == 0 && ldc >= N, "lv_gemm_wgrad_acc_f32: ldc=%lld must be a multiple of 4 and >= N=%lld",
+               (long long)ldc, (long long)N);
+  LV_CHECK_ARG(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(C)) & 15) == 0,
+               "lv_gemm_wgrad_acc_f32: A, W and C must be 16-byte aligned");
+  if (M == 0 || K == 0) return LV_OK;      // nothing to add
+  LV_BIND_DEVICE(A);
+  return launch_gemm<true, true, true>(A, W, nullptr, C, M, N, K, lda, ldw, ldc, 0, (cudaStream_t)stream);
 }
 
 int64_t lv_patch_embed_ws_bytes(int64_t n, int64_t img, int64_t ps, int64_t C) {

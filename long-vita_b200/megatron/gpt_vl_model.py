@@ -48,7 +48,8 @@ from .checkpoint import mcore_to_hf
 class B200GPTVLModel:
     def __init__(self, cfg: LongVITAConfig, state_dict: Dict[str, torch.Tensor], *, pre_process: bool = True,
                  post_process: bool = True, cp=None, is_instruction_dataset: bool = False,
-                 output_multiplier_scale: Optional[float] = None, output_logit_softcapping: Optional[float] = None):
+                 output_multiplier_scale: Optional[float] = None, output_logit_softcapping: Optional[float] = None,
+                 gradient_accumulation_fusion: bool = False):
         if not (pre_process and post_process):
             raise NotImplementedError("pipeline parallelism is not built (14B bf16 fits one 80 GB H100: pp = 1)")
         self.config = cfg
@@ -57,6 +58,9 @@ class B200GPTVLModel:
         self.is_instruction_dataset = is_instruction_dataset
         self.output_multiplier_scale = output_multiplier_scale
         self.output_logit_softcapping = output_logit_softcapping
+        # Megatron's config.gradient_accumulation_fusion for the output layer: when output_weight requires grad, its
+        # gradient is added to output_weight.main_grad (fp32) inside the GEMM (ops.masked_lm_head_ce / masked_linear)
+        self.gradient_accumulation_fusion = bool(gradient_accumulation_fusion)
         w = mcore_to_hf(state_dict, cfg)
         self.word_embeddings = w["model.embed_tokens.weight"]
         self.final_layernorm = w["model.norm.weight"]
@@ -198,7 +202,8 @@ class B200GPTVLModel:
                 last = mask.reshape(-1).nonzero().view(-1)[-1:]
                 keep.view(-1)[last] = False
                 mask, lab = keep, lab[:, 1:].contiguous()
-            loss = ops.masked_lm_head_ce(hidden_states, self.output_weight, mask, lab)
+            loss = ops.masked_lm_head_ce(hidden_states, self.output_weight, mask, lab,
+                                         accumulate_wgrad=self.gradient_accumulation_fusion)
             if loss.sum().isnan():
                 rank = torch.distributed.get_rank() if torch.distributed.is_initialized() else 0
                 raise ValueError(f"Rank {rank}: found NaN in local forward logits calculation. "
@@ -207,7 +212,8 @@ class B200GPTVLModel:
 
         # output layer (ColumnParallelLinear with logit_mask, layers.py:402-409, 825-904)
         if logit_mask is not None:
-            logits = ops.masked_linear(hidden_states, self.output_weight, logit_mask.to(hidden_states.device))
+            logits = ops.masked_linear(hidden_states, self.output_weight, logit_mask.to(hidden_states.device),
+                                       accumulate_wgrad=self.gradient_accumulation_fusion)
         else:
             logits = ops.linear(hidden_states.view(s, -1), self.output_weight).view(s, 1, -1)
         if self.output_multiplier_scale:

@@ -163,15 +163,19 @@ class B200TransformerLayer(torch.nn.Module):
         (RMSNorm / SwiGLU / RoPE backward kernels, `lv_attn_bwd`, and the wgmma GEMM for dX and dW).  It works on the
         Megatron parameter layouts directly (grouped QKV rows, fc1 = cat(gate, up)), so gradients land on the
         parameters Megatron's optimizer owns; the fused-epilogue / in-place shortcuts of the inference path are not
-        used here (the un-fused gate|up activation is what the SwiGLU backward needs)."""
+        used here (the un-fused gate|up activation is what the SwiGLU backward needs).
+
+        `config.gradient_accumulation_fusion` (absent: off) adds the four weight gradients to each weight's fp32
+        `main_grad` inside the GEMM, as Megatron's linears do (ops.linear_autograd, accumulate_wgrad)."""
         s, b, h = hidden_states.shape
         np_, ng, hn = self.np, self.ng, self.hn
         g = np_ // ng
         self._decoder = None               # the re-ordered inference copies go stale once the parameters train
+        fuse = bool(getattr(self.config, "gradient_accumulation_fusion", False))
         x = hidden_states.reshape(s, h)
         a = self.self_attention
         hcur = ops.rmsnorm_autograd(x, a.linear_qkv.layer_norm_weight, self.eps)
-        qkv = ops.linear_autograd(hcur, a.linear_qkv.weight, a.linear_qkv.bias).view(s, ng, g + 2, hn)
+        qkv = ops.linear_autograd(hcur, a.linear_qkv.weight, a.linear_qkv.bias, fuse).view(s, ng, g + 2, hn)
         q = qkv[:, :, :g].reshape(s, np_, hn)
         k = qkv[:, :, g].contiguous()
         v = qkv[:, :, g + 1].contiguous()
@@ -187,10 +191,10 @@ class B200TransformerLayer(torch.nn.Module):
         else:
             att = ops.attention(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True,
                                 **ops.docs_kwargs(megatron_cu_seqlens(s, hidden_states.device)))    # [1, s, np, hn]
-        o = ops.linear_autograd(att.reshape(s, np_ * hn), a.linear_proj.weight)
+        o = ops.linear_autograd(att.reshape(s, np_ * hn), a.linear_proj.weight, None, fuse)
         hcur, x = ops.rmsnorm_autograd(o, self.mlp.linear_fc1.layer_norm_weight, self.eps, residual=x)
-        gate_up = ops.linear_autograd(hcur, self.mlp.linear_fc1.weight)                         # cat(gate, up)
-        d = ops.linear_autograd(ops.swiglu_autograd(gate_up), self.mlp.linear_fc2.weight)
+        gate_up = ops.linear_autograd(hcur, self.mlp.linear_fc1.weight, None, fuse)             # cat(gate, up)
+        d = ops.linear_autograd(ops.swiglu_autograd(gate_up), self.mlp.linear_fc2.weight, None, fuse)
         return (x + d).view(s, b, h)
 
 

@@ -25,7 +25,9 @@ the bf16 pre-activation (Megatron's MLP applies the activation after the linear 
 
 `vision_model_freeze` / `vision_projector_freeze` run the tower / the projector under `no_grad`, as the reference does
 (:485-520).  Recompute and vision context parallelism are refused (NotImplementedError); no shipped 14B script sets
-them.  The flags are read once, at construction.
+them.  `gradient_accumulation_fusion` (`--no-gradient-accumulation-fusion` unset) adds every weight gradient of the
+tower and the projector, the patch-embedding conv weight included, to the weight's fp32 `main_grad` inside the GEMM.
+The flags are read once, at construction.
 """
 from __future__ import annotations
 
@@ -48,7 +50,8 @@ class B200VisionModel(torch.nn.Module):
     def __init__(self, hidden_size: int, vision: Optional[VisionConfig] = None, *, vision_model_freeze: bool = False,
                  vision_projector_freeze: bool = False, vision_model_recompute: bool = False,
                  vision_projector_recompute: bool = False, vision_context_parallel: bool = False,
-                 layernorm_epsilon: Optional[float] = None, params_dtype=torch.bfloat16, device=None):
+                 layernorm_epsilon: Optional[float] = None, params_dtype=torch.bfloat16, device=None,
+                 gradient_accumulation_fusion: bool = False):
         super().__init__()
         if vision_model_recompute or vision_projector_recompute:
             raise NotImplementedError("B200VisionModel: --vision-model-recompute / --vision-projector-recompute are not "
@@ -59,6 +62,7 @@ class B200VisionModel(torch.nn.Module):
         self.vcfg = v
         self.vision_model_freeze = bool(vision_model_freeze)
         self.vision_projector_freeze = bool(vision_projector_freeze)
+        self.gradient_accumulation_fusion = bool(gradient_accumulation_fusion)
         self.eps = v.layer_norm_eps if layernorm_epsilon is None else float(layernorm_epsilon)
         self.pre_proj_eps = v.pre_proj_ln_eps
         C, F, ps = v.hidden_size, v.intermediate_size, v.patch_size
@@ -115,21 +119,22 @@ class B200VisionModel(torch.nn.Module):
     def _vit(self, images: torch.Tensor) -> torch.Tensor:
         v, vit = self.vcfg, self.vit
         H, D = v.num_attention_heads, v.head_dim
+        fuse = self.gradient_accumulation_fusion
         x = ops.patch_embed_autograd(images, vit.conv1.weight, vit.conv1.bias, vit.class_token,
-                                     vit.position_embeddings.weight, v.patch_size)             # [n, S, C]
+                                     vit.position_embeddings.weight, v.patch_size, fuse)       # [n, S, C]
         n, S, C = x.shape
         x = x.view(n * S, C)
         for L in vit.decoder.layers:
             a, m = L.self_attention, L.mlp
             h, x = ops.layernorm_autograd(x, L.input_layernorm.weight, L.input_layernorm.bias, self.eps, passthrough=True)
-            qkv = ops.linear_autograd(h, a.linear_qkv.weight, a.linear_qkv.bias)            # [n*S, H*3*D]
+            qkv = ops.linear_autograd(h, a.linear_qkv.weight, a.linear_qkv.bias, fuse)      # [n*S, H*3*D]
             att = ops.vit_attention(qkv.view(n, S, 3 * C), H, D ** -0.5)
-            o = ops.linear_autograd(att.view(n * S, C), a.linear_proj.weight, a.linear_proj.bias)
+            o = ops.linear_autograd(att.view(n * S, C), a.linear_proj.weight, a.linear_proj.bias, fuse)
             x = ops.ls_residual_autograd(x, o, L.ls1)
             h, x = ops.layernorm_autograd(x, L.pre_mlp_layernorm.weight, L.pre_mlp_layernorm.bias, self.eps,
                                           passthrough=True)
-            f = ops.gelu_autograd(ops.linear_autograd(h, m.linear_fc1.weight, m.linear_fc1.bias))
-            f = ops.linear_autograd(f, m.linear_fc2.weight, m.linear_fc2.bias)
+            f = ops.gelu_autograd(ops.linear_autograd(h, m.linear_fc1.weight, m.linear_fc1.bias, fuse))
+            f = ops.linear_autograd(f, m.linear_fc2.weight, m.linear_fc2.bias, fuse)
             x = ops.ls_residual_autograd(x, f, L.ls2)
         return x.view(n, S, C)
 
@@ -138,8 +143,9 @@ class B200VisionModel(torch.nn.Module):
         enc = self.vision_projection.encoder
         y = ops.layernorm_autograd(x.reshape(n * t, c4), self.pre_proj_layernorm.weight, self.pre_proj_layernorm.bias,
                                    self.pre_proj_eps)
-        y = ops.gelu_autograd(ops.linear_autograd(y, enc.linear_fc1.weight))
-        y = ops.linear_autograd(y, enc.linear_fc2.weight)
+        fuse = self.gradient_accumulation_fusion
+        y = ops.gelu_autograd(ops.linear_autograd(y, enc.linear_fc1.weight, None, fuse))
+        y = ops.linear_autograd(y, enc.linear_fc2.weight, None, fuse)
         return y.view(n, t, -1)
 
     def forward_once(self, images: torch.Tensor) -> torch.Tensor:
@@ -222,6 +228,7 @@ def b200_vision_model_provider(config, *external_args, args=None, load_checkpoin
         vision_context_parallel=bool(_arg(args, "vision_context_parallel", False)),
         layernorm_epsilon=float(_arg(args, "norm_epsilon", v.layer_norm_eps)),
         params_dtype=getattr(config, "params_dtype", None) or torch.bfloat16,
+        gradient_accumulation_fusion=bool(_arg(args, "gradient_accumulation_fusion", False)),
     )
     if vit_load is not None:
         load_checkpoint([model.vit], None, None, load_arg="vit_load", args=_vit_args(args, v))

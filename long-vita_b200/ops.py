@@ -654,12 +654,14 @@ def select_rows(h: torch.Tensor, logit_mask: torch.Tensor) -> torch.Tensor:
     return _SelectRowsFn.apply(h, logit_mask)
 
 
-def masked_linear(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.Tensor, bias: Optional[torch.Tensor] = None):
+def masked_linear(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.Tensor, bias: Optional[torch.Tensor] = None,
+                  accumulate_wgrad: bool = False):
     """Logit-masked LM head, differentiable: rows of h [s, 1, c] selected by logit_mask [1, s] -> [M, 1, vocab]
-    (LinearWithGradAccumulationAndAsyncCommunication with logit_mask, layers.py:371-456, for tp = 1, no sequence
-    parallelism, no gradient-accumulation fusion).  Under no_grad it is the gather and the GEMM, nothing recorded."""
+    (LinearWithGradAccumulationAndAsyncCommunication with logit_mask, layers.py:371-518, for tp = 1, no sequence
+    parallelism; accumulate_wgrad is its gradient_accumulation_fusion, see linear_autograd).  Under no_grad it is the
+    gather and the GEMM, nothing recorded."""
     sel = select_rows(h, logit_mask)
-    return linear_autograd(sel, weight, bias).view(sel.shape[0], 1, weight.shape[0])
+    return linear_autograd(sel, weight, bias, accumulate_wgrad).view(sel.shape[0], 1, weight.shape[0])
 
 
 # ------------------------------------------------------------------------------------------------
@@ -715,16 +717,19 @@ def lm_head_ce_fwd(sel: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor
 
 
 def lm_head_ce_bwd(sel: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor, lse: torch.Tensor, dloss: torch.Tensor,
-                   need_dsel: bool = True, need_dw: bool = False, vocab_chunk: int = 16384):
+                   need_dsel: bool = True, need_dw: bool = False, vocab_chunk: int = 16384,
+                   main_grad: Optional[torch.Tensor] = None):
     """Backward of lm_head_ce_fwd, chunk by chunk: the chunk's logits are recomputed (one GEMM), turned into
     d_logits = (softmax - onehot) * dloss in place (`lv_ce_grad`), and contracted by the same wgmma GEMM:
     d_sel += d_logits @ W[chunk] (fp32 accumulation across chunks), dW[chunk] = d_logits^T @ sel
-    (layers.py:443-456, 512-520).  Returns (d_sel [M, c] bf16 or None, dW [vocab, c] bf16 or None)."""
+    (layers.py:443-456, 512-520).  Returns (d_sel [M, c] bf16 or None, dW [vocab, c] bf16 or None).  With need_dw and
+    an fp32 `main_grad` [vocab, c], each chunk's dW is added to its row slice main_grad[chunk] instead
+    (linear_wgrad_accumulate) and dW is None."""
     M, c = sel.shape
     V = weight.shape[0]
     dev = sel.device
     dsel = torch.zeros((M, c), dtype=torch.float32, device=dev) if need_dsel else None
-    dw = torch.empty((V, c), dtype=torch.bfloat16, device=dev) if need_dw else None
+    dw = torch.empty((V, c), dtype=torch.bfloat16, device=dev) if need_dw and main_grad is None else None
     if M == 0:
         if dw is not None:
             dw.zero_()
@@ -738,34 +743,44 @@ def lm_head_ce_bwd(sel: torch.Tensor, weight: torch.Tensor, labels: torch.Tensor
         lg = ce_grad(linear(sel, weight[v0:v1], out=buf[:, :n]), labels, lse, dloss, v0)
         if need_dsel:
             dsel += linear(lg, weight[v0:v1].t()).float()           # the weight chunk read in place, MN-major
-        if need_dw:
+        if need_dw and main_grad is not None:
+            linear_wgrad_accumulate(lg, sel, main_grad[v0:v1])
+        elif need_dw:
             linear(lg.t(), sel.t(), out=dw[v0:v1])                  # both MN-major, the M rows are the contraction
     return (None if dsel is None else dsel.to(torch.bfloat16)), dw
 
 
 class _LMHeadCEFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, sel, weight, labels, vocab_chunk):
+    def forward(ctx, sel, weight, labels, vocab_chunk, accumulate_wgrad=False):
         labels = labels.reshape(-1)
         loss, lse = lm_head_ce_fwd(sel, weight, labels, vocab_chunk)
         ctx.save_for_backward(sel, weight, labels, lse)
-        ctx.vocab_chunk = vocab_chunk
+        ctx.vocab_chunk, ctx.accumulate_wgrad = vocab_chunk, accumulate_wgrad
         return loss.view(1, -1)
 
     @staticmethod
     def backward(ctx, dloss):
         sel, weight, labels, lse = ctx.saved_tensors
-        dsel, dw = lm_head_ce_bwd(sel, weight, labels, lse, dloss.reshape(-1), ctx.needs_input_grad[0], ctx.needs_input_grad[1],
-                                  ctx.vocab_chunk)
-        return dsel, dw, None, None
+        if not (ctx.accumulate_wgrad and ctx.needs_input_grad[1]):
+            dsel, dw = lm_head_ce_bwd(sel, weight, labels, lse, dloss.reshape(-1), ctx.needs_input_grad[0],
+                                      ctx.needs_input_grad[1], ctx.vocab_chunk)
+            return dsel, dw, None, None, None
+        main_grad = fused_wgrad_main_grad(weight)
+        dsel, _ = lm_head_ce_bwd(sel, weight, labels, lse, dloss.reshape(-1), ctx.needs_input_grad[0], True,
+                                 ctx.vocab_chunk, main_grad=main_grad)
+        return dsel, fused_wgrad_dummy(weight, main_grad, sel.dtype), None, None, None
 
 
 def masked_lm_head_ce(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.Tensor, labels: torch.Tensor,
-                      vocab_chunk: int = 16384) -> torch.Tensor:
+                      vocab_chunk: int = 16384, accumulate_wgrad: bool = False) -> torch.Tensor:
     """GPTVLModel's training tail in one differentiable op (gpt_vl_model.py:325-339 masked_select of the hidden rows,
     :339 output_layer, :379-382 masked_select of the labels done by the caller, :412 per-token loss): h [s, 1, c],
     weight [vocab, c], logit_mask [1, s] bool, labels [1, M] (the M selected label ids) -> loss [1, M] fp32.  The
-    [M, vocab] logits are never materialised (1M tokens x 152 064 would be 318 GB in bf16)."""
+    [M, vocab] logits are never materialised (1M tokens x 152 064 would be 318 GB in bf16).  accumulate_wgrad: the
+    weight gradient goes to weight.main_grad, vocabulary chunk by chunk (see linear_autograd)."""
+    if accumulate_wgrad:
+        return _LMHeadCEFn.apply(select_rows(h, logit_mask), weight, labels, vocab_chunk, True)
     return _LMHeadCEFn.apply(select_rows(h, logit_mask), weight, labels, vocab_chunk)
 
 
@@ -859,12 +874,14 @@ def rope_autograd(x, cos, sin):
 
 class _LinearFn(torch.autograd.Function):
     """y = x W^T + b on the wgmma GEMM; dX = dY W and dW = dY^T X reuse the same kernel, which reads the transposed
-    operands (W^T, dY^T, X^T) in place as MN-major views."""
+    operands (W^T, dY^T, X^T) in place as MN-major views.  With accumulate_wgrad, dW is added to weight.main_grad in
+    fp32 instead (gradient-accumulation fusion, see fused_wgrad_main_grad)."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias):
+    def forward(ctx, x, weight, bias, accumulate_wgrad=False):
         ctx.save_for_backward(x, weight)
         ctx.has_bias = bias is not None
+        ctx.accumulate_wgrad = accumulate_wgrad
         return linear(x, weight, bias)
 
     @staticmethod
@@ -877,10 +894,22 @@ class _LinearFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = linear(dy2, weight.t()).view(x.shape)                       # [T, K] = dY [T, N] . (W^T)[K, N]^T
         if ctx.needs_input_grad[1]:
-            dw = linear_wgrad(dy2, x2)
+            if ctx.accumulate_wgrad:
+                main_grad = fused_wgrad_main_grad(weight)
+                linear_wgrad_accumulate(dy2, x2, main_grad)
+                dw = fused_wgrad_dummy(weight, main_grad, dy2.dtype)
+            else:
+                dw = linear_wgrad(dy2, x2)
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = dy2.float().sum(dim=0).to(dy2.dtype)
-        return dx, dw, db
+        return dx, dw, db, None
+
+
+def _wgrad_operands(dy2: torch.Tensor, x2: torch.Tensor):
+    """dY [T, N] and X [T, K] as the GEMM reads them transposed in place (MN-major): unit column stride, a row stride
+    that is a multiple of 8 elements, a 16-byte aligned start; any other layout is copied to a contiguous tensor."""
+    return tuple(t if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0 else t.contiguous()
+                 for t in (dy2, x2))
 
 
 def linear_wgrad(dy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
@@ -889,12 +918,66 @@ def linear_wgrad(dy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
     owns no answer token) dW is zero and no GEMM runs."""
     if dy2.shape[0] == 0:
         return torch.zeros((dy2.shape[1], x2.shape[1]), dtype=dy2.dtype, device=dy2.device)
-    dy2, x2 = (t if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0 else t.contiguous()
-               for t in (dy2, x2))
+    dy2, x2 = _wgrad_operands(dy2, x2)
     return linear(dy2.t(), x2.t())                                           # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
 
 
-def linear_autograd(x, weight, bias=None):
+def linear_wgrad_accumulate(dy2: torch.Tensor, x2: torch.Tensor, main_grad: torch.Tensor) -> torch.Tensor:
+    """main_grad [N, K] fp32 += dY^T [N, T] . X [T, K], in place (`lv_gemm_wgrad_acc_f32`): the product of linear_wgrad
+    with the same operands and k-order, added to main_grad in fp32 without a bf16 rounding.  main_grad may be a view
+    (a row slice, or the first K columns of a wider tensor): unit column stride, a row stride that is a multiple of 4,
+    16-byte aligned; elements outside it are not touched.  Without tokens nothing is launched.  Returns main_grad."""
+    _need_cuda_bf16(dy2, x2)
+    _need_cuda(main_grad, torch.float32)
+    n_out, k_in = dy2.shape[1], x2.shape[1]
+    if tuple(main_grad.shape) != (n_out, k_in):
+        raise RuntimeError(f"linear_wgrad_accumulate: main_grad is {tuple(main_grad.shape)}, the weight gradient is "
+                           f"[{n_out}, {k_in}]")
+    if main_grad.stride(1) != 1 or main_grad.stride(0) % 4 != 0 or main_grad.data_ptr() % 16 != 0:
+        raise RuntimeError(f"linear_wgrad_accumulate: main_grad (strides {main_grad.stride()}) must have unit column "
+                           "stride, a row stride that is a multiple of 4 and a 16-byte aligned start")
+    T = dy2.shape[0]
+    if T == 0:
+        return main_grad
+    dy2, x2 = _wgrad_operands(dy2, x2)
+    ev0 = _TIMER.start() if _TIMER is not None else None
+    _lib.check(_lib.lib().lv_gemm_wgrad_acc_f32(dy2.data_ptr(), x2.data_ptr(), main_grad.data_ptr(), n_out, k_in, T,
+                                                dy2.stride(0), x2.stride(0), main_grad.stride(0), 1, 1, _stream()),
+               "lv_gemm_wgrad_acc_f32")
+    if ev0 is not None:
+        _TIMER.stop("gemm_bf16", 2.0 * n_out * k_in * T, ev0)
+    return main_grad
+
+
+def fused_wgrad_main_grad(weight: torch.Tensor) -> torch.Tensor:
+    """The fp32 `main_grad` a weight gradient is accumulated into under Megatron's gradient_accumulation_fusion
+    (long_vita_megatron/core/tensor_parallel/layers.py:486-497; Megatron's DDP wrapper allocates it)."""
+    main_grad = getattr(weight, "main_grad", None)
+    if main_grad is None:
+        raise RuntimeError(f"gradient_accumulation_fusion: the trainable weight of shape {tuple(weight.shape)} has no "
+                           "`main_grad` to accumulate into (it is allocated by Megatron's DistributedDataParallel)")
+    if main_grad.dtype != torch.float32:
+        raise NotImplementedError(f"gradient_accumulation_fusion: main_grad is {main_grad.dtype}; only an fp32 "
+                                  "main_grad is supported (Megatron's with --bf16)")
+    return main_grad
+
+
+def fused_wgrad_dummy(weight: torch.Tensor, main_grad: torch.Tensor, dtype: torch.dtype) -> Optional[torch.Tensor]:
+    """The gradient returned for a weight whose gradient went to main_grad (layers.py:499-518): None when the weight has
+    no `grad_added_to_main_grad` attribute; otherwise a main_grad-shaped tensor - zeros with `zero_out_wgrad`, else
+    uninitialised - and grad_added_to_main_grad is set."""
+    if not hasattr(weight, "grad_added_to_main_grad"):
+        return None
+    make = torch.zeros if getattr(weight, "zero_out_wgrad", False) else torch.empty
+    weight.grad_added_to_main_grad = True
+    return make(main_grad.shape, dtype=dtype, device=main_grad.device)
+
+
+def linear_autograd(x, weight, bias=None, accumulate_wgrad: bool = False):
+    """Differentiable linear (see _LinearFn).  accumulate_wgrad: the weight gradient is added to weight.main_grad
+    (fp32) and the returned gradient follows fused_wgrad_dummy; the bias gradient is unchanged."""
+    if accumulate_wgrad:
+        return _LinearFn.apply(x, weight, bias, True)
     return _LinearFn.apply(x, weight, bias)
 
 
@@ -1094,16 +1177,17 @@ class _PatchEmbedFn(torch.autograd.Function):
     the conv weight gradient is dW[C, Kpad] = dP^T . col on the wgmma GEMM, with the padding columns dropped."""
 
     @staticmethod
-    def forward(ctx, images, conv_w, conv_b, cls, pos, patch):
+    def forward(ctx, images, conv_w, conv_b, cls, pos, patch, accumulate_wgrad=False):
         w_pad = pad_patch_weight(conv_w)
-        ctx.save_for_backward(images)
+        ctx.save_for_backward(images, conv_w if accumulate_wgrad else None)
         ctx.patch, ctx.kpad, ctx.w_shape = patch, w_pad.shape[1], conv_w.shape
         ctx.cls_shape, ctx.pos_shape = cls.shape, pos.shape
+        ctx.accumulate_wgrad = accumulate_wgrad
         return patch_embed(images, w_pad, conv_b, cls.reshape(-1), pos, patch)
 
     @staticmethod
     def backward(ctx, dout):
-        (images,) = ctx.saved_tensors
+        images, conv_w = ctx.saved_tensors
         n, s, c = dout.shape
         d = dout.contiguous()
         dw = db = dcls = dpos = None
@@ -1111,20 +1195,29 @@ class _PatchEmbedFn(torch.autograd.Function):
         if ctx.needs_input_grad[1]:
             col = patch_im2col(images, ctx.patch, ctx.kpad)
             k = ctx.w_shape[1] * ctx.w_shape[2] * ctx.w_shape[3]
-            dw = linear_wgrad(dp, col)[:, :k].reshape(ctx.w_shape)
+            if ctx.accumulate_wgrad:
+                # only the k real im2col columns: the padding columns of the [C, kpad] product never reach main_grad
+                main_grad = fused_wgrad_main_grad(conv_w)
+                linear_wgrad_accumulate(dp, col[:, :k], main_grad.view(ctx.w_shape[0], k))
+                dw = fused_wgrad_dummy(conv_w, main_grad, d.dtype)
+            else:
+                dw = linear_wgrad(dp, col)[:, :k].reshape(ctx.w_shape)
         if ctx.needs_input_grad[2]:
             db = dp.float().sum(dim=0).to(d.dtype)
         if ctx.needs_input_grad[3]:
             dcls = d[:, 0].float().sum(dim=0).to(d.dtype).reshape(ctx.cls_shape)
         if ctx.needs_input_grad[4]:
             dpos = d.float().sum(dim=0).to(d.dtype).reshape(ctx.pos_shape)
-        return None, dw, db, dcls, dpos, None
+        return None, dw, db, dcls, dpos, None, None
 
 
-def patch_embed_autograd(images, conv_w, conv_b, cls, pos, patch: int):
+def patch_embed_autograd(images, conv_w, conv_b, cls, pos, patch: int, accumulate_wgrad: bool = False):
     """Differentiable InternViT embedding: images [n, 3, S, S], conv_w [C, 3, patch, patch], conv_b [C], cls (C
     elements, e.g. [1, 1, C]), pos [1 + (S/patch)^2, C] -> [n, 1 + (S/patch)^2, C].  Gradients: conv weight, conv bias,
-    class token (sum over frames of row 0), position embedding (sum over frames); none for the images."""
+    class token (sum over frames of row 0), position embedding (sum over frames); none for the images.
+    accumulate_wgrad: the conv weight gradient goes to conv_w.main_grad (see linear_autograd)."""
+    if accumulate_wgrad:
+        return _PatchEmbedFn.apply(images, conv_w, conv_b, cls, pos, patch, True)
     return _PatchEmbedFn.apply(images, conv_w, conv_b, cls, pos, patch)
 
 
