@@ -514,18 +514,48 @@ static int launch_gemm(const void* A, const void* W, const void* bias, void* C, 
 
 using namespace lv;
 
+// The argument checks of the three GEMM entry points; `fn` names the entry point in lv_last_error.  a_mn / w_mn are the
+// operand layouts (0, 0 for lv_gemm_bias_act); acc is the fp32 accumulation of lv_gemm_wgrad_acc_f32 (MN-major A and W
+// only, K may be 0, N and ldc multiples of 4 fp32 elements, no bias or activation); `aligned` requires 16-byte aligned
+// A, W and C (lv_gemm_bias_act does not: its GEMV path takes any C).
+static int check_gemm_args(const char* fn, const void* A, const void* W, const void* bias, const void* C, int64_t M,
+                           int64_t N, int64_t K, int64_t lda, int64_t ldw, int64_t ldc, int32_t a_mn, int32_t w_mn,
+                           int32_t act, bool acc, bool aligned) {
+  LV_CHECK_ARG(A && W && C, "%s: null pointer", fn);
+  LV_CHECK_ARG((a_mn == 0 || a_mn == 1) && (w_mn == 0 || w_mn == 1), "%s: a_mn_major=%d and w_mn_major=%d must be 0 or 1",
+               fn, a_mn, w_mn);
+  LV_CHECK_ARG(!acc || (a_mn && w_mn), "%s: only MN-major A and W are built (dW = dY^T . X with dY and X read in place)",
+               fn);
+  LV_CHECK_ARG(M >= 0 && N > 0 && (acc ? K >= 0 : K > 0), "%s: bad shape M=%lld N=%lld K=%lld", fn, (long long)M,
+               (long long)N, (long long)K);
+  LV_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "%s: dimension too large", fn);
+  const int nq = acc ? 4 : 8;  // N and ldc in elements of C: 16 bytes of fp32 or of bf16
+  if (a_mn && w_mn)
+    LV_CHECK_ARG(N % nq == 0, "%s: N=%lld must be a multiple of %d", fn, (long long)N, nq);
+  else
+    LV_CHECK_ARG(K % 8 == 0 && N % 8 == 0, "%s: K=%lld and N=%lld must be multiples of 8 while an operand is K-major", fn,
+                 (long long)K, (long long)N);
+  LV_CHECK_ARG(act >= 0 && act <= 3, "%s: unknown activation %d", fn, act);
+  LV_CHECK_ARG(lda % 8 == 0 && lda >= (a_mn ? M : K), "%s: lda=%lld must be a multiple of 8 and >= %s=%lld", fn,
+               (long long)lda, a_mn ? "M" : "K", (long long)(a_mn ? M : K));
+  LV_CHECK_ARG(ldw % 8 == 0 && ldw >= (w_mn ? N : K), "%s: ldw=%lld must be a multiple of 8 and >= %s=%lld", fn,
+               (long long)ldw, w_mn ? "N" : "K", (long long)(w_mn ? N : K));
+  const int64_t row = act == 3 ? N / 2 : N;
+  LV_CHECK_ARG(ldc % nq == 0 && ldc >= row, "%s: ldc=%lld must be a multiple of %d and >= the row length %lld", fn,
+               (long long)ldc, nq, (long long)row);
+  LV_CHECK_ARG(!aligned || ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W) |
+                             reinterpret_cast<uintptr_t>(C)) & 15) == 0,
+               "%s: A, W and C must be 16-byte aligned", fn);
+  LV_CHECK_ARG(act != 3 || (N % 16 == 0 && bias == nullptr), "%s: fused SwiGLU needs N %% 16 == 0 and no bias", fn);
+  return LV_OK;
+}
+
 extern "C" {
 
 int lv_gemm_bias_act(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K,
                      int64_t lda, int64_t ldw, int64_t ldc, int32_t act, lv_stream_t stream) {
-  LV_CHECK_ARG(A && W && C, "lv_gemm_bias_act: null pointer");
-  LV_CHECK_ARG(M >= 0 && N > 0 && K > 0, "lv_gemm_bias_act: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
-  LV_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "lv_gemm_bias_act: dimension too large");
-  LV_CHECK_ARG(K % 8 == 0 && N % 8 == 0, "lv_gemm_bias_act: K=%lld and N=%lld must be multiples of 8", (long long)K, (long long)N);
-  LV_CHECK_ARG(act >= 0 && act <= 3, "lv_gemm_bias_act: unknown activation %d", act);
-  LV_CHECK_ARG(lda >= K && ldw >= K && ldc >= (act == 3 ? N / 2 : N) && lda % 8 == 0 && ldw % 8 == 0 && ldc % 8 == 0,
-               "lv_gemm_bias_act: leading dimensions must be >= the row length and multiples of 8");
-  LV_CHECK_ARG(act != 3 || (N % 16 == 0 && bias == nullptr), "lv_gemm_bias_act: fused SwiGLU needs N %% 16 == 0 and no bias");
+  int r = check_gemm_args("lv_gemm_bias_act", A, W, bias, C, M, N, K, lda, ldw, ldc, 0, 0, act, false, false);
+  if (r) return r;
   if (M == 0) return LV_OK;
   LV_BIND_DEVICE(A);
   // Weight-stream GEMV for decode-sized M - unless the tensor-core kernel already has a tile for every SM (the LM head:
@@ -538,26 +568,8 @@ int lv_gemm_bias_act(const void* A, const void* W, const void* bias, void* C, in
 
 int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, int32_t act, lv_stream_t stream) {
-  LV_CHECK_ARG(A && W && C, "lv_gemm_ex: null pointer");
-  LV_CHECK_ARG((a_mn_major == 0 || a_mn_major == 1) && (w_mn_major == 0 || w_mn_major == 1),
-               "lv_gemm_ex: a_mn_major=%d and w_mn_major=%d must be 0 or 1", a_mn_major, w_mn_major);
-  LV_CHECK_ARG(M >= 0 && N > 0 && K > 0, "lv_gemm_ex: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
-  LV_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "lv_gemm_ex: dimension too large");
-  LV_CHECK_ARG(N % 8 == 0, "lv_gemm_ex: N=%lld must be a multiple of 8", (long long)N);
-  LV_CHECK_ARG(K % 8 == 0 || (a_mn_major && w_mn_major),
-               "lv_gemm_ex: K=%lld must be a multiple of 8 while an operand is K-major", (long long)K);
-  LV_CHECK_ARG(act >= 0 && act <= 3, "lv_gemm_ex: unknown activation %d", act);
-  LV_CHECK_ARG(lda % 8 == 0 && lda >= (a_mn_major ? M : K),
-               "lv_gemm_ex: lda=%lld must be a multiple of 8 and >= %s=%lld", (long long)lda, a_mn_major ? "M" : "K",
-               (long long)(a_mn_major ? M : K));
-  LV_CHECK_ARG(ldw % 8 == 0 && ldw >= (w_mn_major ? N : K),
-               "lv_gemm_ex: ldw=%lld must be a multiple of 8 and >= %s=%lld", (long long)ldw, w_mn_major ? "N" : "K",
-               (long long)(w_mn_major ? N : K));
-  LV_CHECK_ARG(ldc % 8 == 0 && ldc >= (act == 3 ? N / 2 : N), "lv_gemm_ex: ldc=%lld must be a multiple of 8 and >= the row length",
-               (long long)ldc);
-  LV_CHECK_ARG(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(C)) & 15) == 0,
-               "lv_gemm_ex: A, W and C must be 16-byte aligned");
-  LV_CHECK_ARG(act != 3 || (N % 16 == 0 && bias == nullptr), "lv_gemm_ex: fused SwiGLU needs N %% 16 == 0 and no bias");
+  int r = check_gemm_args("lv_gemm_ex", A, W, bias, C, M, N, K, lda, ldw, ldc, a_mn_major, w_mn_major, act, false, true);
+  if (r) return r;
   if (!a_mn_major && !w_mn_major) return lv_gemm_bias_act(A, W, bias, C, M, N, K, lda, ldw, ldc, act, stream);
   if (M == 0) return LV_OK;
   LV_BIND_DEVICE(A);
@@ -570,23 +582,9 @@ int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t 
 
 int lv_gemm_wgrad_acc_f32(const void* A, const void* W, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                           int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, lv_stream_t stream) {
-  LV_CHECK_ARG(A && W && C, "lv_gemm_wgrad_acc_f32: null pointer");
-  LV_CHECK_ARG((a_mn_major == 0 || a_mn_major == 1) && (w_mn_major == 0 || w_mn_major == 1),
-               "lv_gemm_wgrad_acc_f32: a_mn_major=%d and w_mn_major=%d must be 0 or 1", a_mn_major, w_mn_major);
-  LV_CHECK_ARG(a_mn_major && w_mn_major,
-               "lv_gemm_wgrad_acc_f32: only MN-major A and W are built (dW = dY^T . X with dY and X read in place)");
-  LV_CHECK_ARG(M >= 0 && N > 0 && K >= 0, "lv_gemm_wgrad_acc_f32: bad shape M=%lld N=%lld K=%lld", (long long)M,
-               (long long)N, (long long)K);
-  LV_CHECK_ARG(M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31), "lv_gemm_wgrad_acc_f32: dimension too large");
-  LV_CHECK_ARG(N % 4 == 0, "lv_gemm_wgrad_acc_f32: N=%lld must be a multiple of 4", (long long)N);
-  LV_CHECK_ARG(lda % 8 == 0 && lda >= M, "lv_gemm_wgrad_acc_f32: lda=%lld must be a multiple of 8 and >= M=%lld",
-               (long long)lda, (long long)M);
-  LV_CHECK_ARG(ldw % 8 == 0 && ldw >= N, "lv_gemm_wgrad_acc_f32: ldw=%lld must be a multiple of 8 and >= N=%lld",
-               (long long)ldw, (long long)N);
-  LV_CHECK_ARG(ldc % 4 == 0 && ldc >= N, "lv_gemm_wgrad_acc_f32: ldc=%lld must be a multiple of 4 and >= N=%lld",
-               (long long)ldc, (long long)N);
-  LV_CHECK_ARG(((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(C)) & 15) == 0,
-               "lv_gemm_wgrad_acc_f32: A, W and C must be 16-byte aligned");
+  int r = check_gemm_args("lv_gemm_wgrad_acc_f32", A, W, nullptr, C, M, N, K, lda, ldw, ldc, a_mn_major, w_mn_major, 0,
+                          true, true);
+  if (r) return r;
   if (M == 0 || K == 0) return LV_OK;      // nothing to add
   LV_BIND_DEVICE(A);
   return launch_gemm<true, true, true>(A, W, nullptr, C, M, N, K, lda, ldw, ldc, 0, (cudaStream_t)stream);

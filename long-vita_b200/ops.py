@@ -1,8 +1,11 @@
 """Operator layer: PyTorch tensors in / out, arithmetic in liblvb200.so through the C ABI.
 
-PyTorch is used for device memory, streams and autograd plumbing only.  Every function validates
-that its tensors are CUDA bf16 (or the stated integer / float type) and raises RuntimeError when
-the extension is missing or a call fails - there is no eager fallback.
+PyTorch is used for device memory, streams and autograd plumbing only.  The C side cannot see tensor extents, so each
+wrapper hands its tensors over as the kernel reads them - row matrices (`_rows`, `_like`), per-column parameters
+(`_param`), index / label / statistics vectors (`_vec`), GEMM operands (`_gemm_operand`) - and a shape, length or dtype
+mismatch raises ValueError naming the wrapper and the argument before anything is launched.  Tensors must be CUDA bf16
+(or the stated integer / float type); RuntimeError is raised otherwise, when the extension is missing or when a call
+fails - there is no eager fallback.
 """
 from __future__ import annotations
 
@@ -37,6 +40,42 @@ def _need_cuda_bf16(*ts: Optional[torch.Tensor]) -> None:
 def _need_cuda(t: torch.Tensor, dtype: torch.dtype) -> None:
     if not t.is_cuda or t.dtype != dtype:
         raise RuntimeError(f"expected CUDA {dtype} tensor, got {t.device} {t.dtype}")
+
+
+def _call(name: str, *args) -> None:
+    """Call the C entry point `name` with `args` and the current stream; RuntimeError if it fails."""
+    _lib.check(getattr(_lib.lib(), name)(*args, _stream()), name)
+
+
+def _rows(t: torch.Tensor, cols: int) -> torch.Tensor:
+    """t [..., cols] as the contiguous row matrix [-1, cols] a kernel reads (copied only when it is not contiguous)."""
+    return t.reshape(-1, cols).contiguous()
+
+
+def _like(op: str, name: str, t: torch.Tensor, shape) -> torch.Tensor:
+    """A companion operand (a residual, a gradient) as the contiguous [rows, cols] `shape` of the primary's rows."""
+    if t.numel() != shape[0] * shape[1]:
+        raise ValueError(f"{op}: {name} {tuple(t.shape)} does not hold the {shape[0]} rows of {shape[1]} it is read as")
+    return (t if t.shape == shape else t.reshape(shape)).contiguous()
+
+
+def _param(op: str, name: str, t: Optional[torch.Tensor], n: int) -> Optional[torch.Tensor]:
+    """None, or t as the n contiguous elements a kernel reads (a per-column weight, bias or layer scale, a class token,
+    a position table)."""
+    if t is not None and t.numel() != n:
+        raise ValueError(f"{op}: {name} {tuple(t.shape)} has {t.numel()} elements, the kernel reads {n}")
+    return None if t is None else t.contiguous()
+
+
+def _vec(op: str, name: str, t: torch.Tensor, dtype: torch.dtype, n: Optional[int] = None,
+         inplace: bool = False) -> torch.Tensor:
+    """An index, label or row-statistics tensor as the contiguous CUDA vector of `dtype` (and `n` elements, if given) a
+    kernel reads; one the kernel writes (`inplace`) must already be contiguous."""
+    if t.dtype != dtype or (n is not None and t.numel() != n) or (inplace and not t.is_contiguous()):
+        want = f"{'a contiguous ' if inplace else ''}{dtype}{'' if n is None else f' of {n} elements'}"
+        raise ValueError(f"{op}: {name} must be {want}, got {t.dtype} {tuple(t.shape)}")
+    _need_cuda(t, dtype)
+    return t.contiguous().view(-1)
 
 
 class KernelTimer:
@@ -256,9 +295,9 @@ def attention_fwd(
                     q_seg_pos=q_seg_pos, kv_pos0=kv_pos0)
     ev0 = _TIMER.start() if _TIMER is not None else None
     if docs is not None:
-        _lib.check(_lib.lib().lv_attn_docs_fwd(C.byref(p), C.byref(docs), _stream()), "lv_attn_docs_fwd")
+        _call("lv_attn_docs_fwd", C.byref(p), C.byref(docs))
     else:
-        _lib.check(_lib.lib().lv_attn_fwd(C.byref(p), _stream()), "lv_attn_fwd")
+        _call("lv_attn_fwd", C.byref(p))
     if ev0 is not None:
         if docs is not None:
             fl = _docs_flops(host, hq, d)
@@ -287,6 +326,8 @@ def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[flo
                                  "and strides that are multiples of 8 elements")
     _need_cuda_bf16(d_out, q, k, v, out)
     _need_cuda(lse, torch.float32)
+    if tuple(lse.shape) != (q.shape[0], q.shape[2], q.shape[1]):
+        raise ValueError(f"attention_bwd: lse {tuple(lse.shape)} is not [b, hq, sq] of q {tuple(q.shape)}")
     docs = None
     if cu_seqlens is not None:
         _check_docs_call(q.shape[0], q.shape[1], k.shape[1], causal, q_seg_len, q_seg_pos, kv_pos0)
@@ -305,9 +346,9 @@ def attention_bwd(d_out, q, k, v, out, lse, *, causal: bool, scale: Optional[flo
         arr = getattr(p, name)
         arr[0], arr[1], arr[2] = t.stride(0), t.stride(1), t.stride(2)
     if docs is not None:
-        _lib.check(_lib.lib().lv_attn_docs_bwd(C.byref(p), C.byref(docs), _stream()), "lv_attn_docs_bwd")
+        _call("lv_attn_docs_bwd", C.byref(p), C.byref(docs))
     else:
-        _lib.check(_lib.lib().lv_attn_bwd(C.byref(p), _stream()), "lv_attn_bwd")
+        _call("lv_attn_bwd", C.byref(p))
     return dq, dk, dv
 
 
@@ -385,13 +426,11 @@ def decode_merge(o_part: torch.Tensor, lse_part: torch.Tensor, return_lse: bool 
     """o_part [n, G, hkv, d] bf16, lse_part [n, hkv, G] fp32 -> out [hq, d] (head h = kvh * G + g) and the
     merged log-sum-exp [hq]: out = sum_s exp(lse_s - LSE) o_s (lv_attn_decode_merge)."""
     _need_cuda_bf16(o_part)
-    _need_cuda(lse_part, torch.float32)
     n, G, hkv, d = o_part.shape
-    o_part, lse_part = o_part.contiguous(), lse_part.contiguous()
+    o_part, lse_part = o_part.contiguous(), _vec("decode_merge", "lse_part", lse_part, torch.float32, n * hkv * G)
     out = torch.empty((hkv * G, d), dtype=torch.bfloat16, device=o_part.device)
     lse = torch.empty((hkv * G,), dtype=torch.float32, device=o_part.device) if return_lse else None
-    _lib.check(_lib.lib().lv_attn_decode_merge(o_part.data_ptr(), lse_part.data_ptr(), out.data_ptr(), _ptr(lse), n, G, hkv, d,
-                                               _stream()), "lv_attn_decode_merge")
+    _call("lv_attn_decode_merge", o_part.data_ptr(), lse_part.data_ptr(), out.data_ptr(), _ptr(lse), n, G, hkv, d)
     return (out, lse) if return_lse else out
 
 
@@ -401,94 +440,69 @@ def decode_merge(o_part: torch.Tensor, lse_part: torch.Tensor, return_lse: bool 
 def rmsnorm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, residual: Optional[torch.Tensor] = None):
     """RMSNorm over the last dim.  With `residual`, returns (norm(x + residual), x + residual)."""
     _need_cuda_bf16(x, weight, residual)
-    x2 = x.reshape(-1, x.shape[-1])
-    if not x2.is_contiguous():
-        x2 = x2.contiguous()
+    cols = x.shape[-1]
+    x2 = _rows(x, cols)
+    res2 = None if residual is None else _like("rmsnorm", "residual", residual, x2.shape)
+    weight = _param("rmsnorm", "weight", weight, cols)
     y = torch.empty_like(x2)
-    res2 = None
-    s = None
-    if residual is not None:
-        res2 = residual.reshape(-1, x.shape[-1]).contiguous()
-        s = torch.empty_like(x2)
-    _lib.check(
-        _lib.lib().lv_rmsnorm(x2.data_ptr(), _ptr(res2), weight.data_ptr(), y.data_ptr(), _ptr(s), x2.shape[0],
-                              x2.shape[1], float(eps), _stream()),
-        "lv_rmsnorm",
-    )
-    if residual is not None:
-        return y.view(x.shape), s.view(x.shape)
-    return y.view(x.shape)
+    s = None if residual is None else torch.empty_like(x2)
+    _call("lv_rmsnorm", x2.data_ptr(), _ptr(res2), weight.data_ptr(), y.data_ptr(), _ptr(s), x2.shape[0], cols, float(eps))
+    return y.view(x.shape) if s is None else (y.view(x.shape), s.view(x.shape))
 
 
 def layernorm(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], eps: float = 1e-6):
     _need_cuda_bf16(x, weight, bias)
-    x2 = x.reshape(-1, x.shape[-1])
-    if not x2.is_contiguous():
-        x2 = x2.contiguous()
+    cols = x.shape[-1]
+    x2 = _rows(x, cols)
+    weight, bias = _param("layernorm", "weight", weight, cols), _param("layernorm", "bias", bias, cols)
     y = torch.empty_like(x2)
-    _lib.check(
-        _lib.lib().lv_layernorm(x2.data_ptr(), weight.data_ptr(), _ptr(bias), y.data_ptr(), x2.shape[0], x2.shape[1],
-                                float(eps), _stream()),
-        "lv_layernorm",
-    )
+    _call("lv_layernorm", x2.data_ptr(), weight.data_ptr(), _ptr(bias), y.data_ptr(), x2.shape[0], cols, float(eps))
     return y.view(x.shape)
 
 
 def rope_table(pos: torch.Tensor, inv_freq: torch.Tensor):
     """cos, sin tables (bf16 [n, 2 * len(inv_freq)]) for int64 positions `pos` [n]."""
-    _need_cuda(pos, torch.int64)
-    _need_cuda(inv_freq, torch.float32)
-    pos = pos.contiguous().view(-1)
+    pos, inv_freq = _vec("rope_table", "pos", pos, torch.int64), _vec("rope_table", "inv_freq", inv_freq, torch.float32)
     dim = 2 * inv_freq.numel()
     cos = torch.empty((pos.numel(), dim), dtype=torch.bfloat16, device=pos.device)
     sin = torch.empty_like(cos)
-    _lib.check(
-        _lib.lib().lv_rope_table(pos.data_ptr(), inv_freq.contiguous().data_ptr(), cos.data_ptr(), sin.data_ptr(),
-                                 pos.numel(), dim, _stream()),
-        "lv_rope_table",
-    )
+    _call("lv_rope_table", pos.data_ptr(), inv_freq.data_ptr(), cos.data_ptr(), sin.data_ptr(), pos.numel(), dim)
     return cos, sin
 
 
 def rope(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, out: Optional[torch.Tensor] = None):
-    """Rotate-half RoPE of x[n_tok, heads, dim] (a strided view is fine); returns a new tensor or
-    writes `out` (which may be x itself)."""
+    """Rotate-half RoPE of x[n_tok, heads, dim] (a strided view is fine) with cos / sin [n_tok, dim]; returns a new
+    tensor or writes `out` (which may be x itself)."""
     _need_cuda_bf16(x, cos, sin)
-    assert x.dim() == 3 and x.stride(2) == 1
+    if x.dim() != 3 or x.stride(2) != 1:
+        raise ValueError(f"rope: x {tuple(x.shape)} must be [n_tok, heads, dim] with a contiguous last dimension")
     n_tok, heads, dim = x.shape
+    cos, sin = _like("rope", "cos", cos, (n_tok, dim)), _like("rope", "sin", sin, (n_tok, dim))
     if out is None:
         out = torch.empty((n_tok, heads, dim), dtype=torch.bfloat16, device=x.device)
-    assert out.stride(2) == 1
-    _lib.check(
-        _lib.lib().lv_rope(x.data_ptr(), out.data_ptr(), cos.data_ptr(), sin.data_ptr(), n_tok, heads, dim, x.stride(0),
-                           x.stride(1), out.stride(0), out.stride(1), _stream()),
-        "lv_rope",
-    )
+    elif out.shape != x.shape or out.stride(2) != 1:
+        raise ValueError(f"rope: out {tuple(out.shape)} must have x's shape and a contiguous last dimension")
+    _call("lv_rope", x.data_ptr(), out.data_ptr(), cos.data_ptr(), sin.data_ptr(), n_tok, heads, dim, x.stride(0),
+          x.stride(1), out.stride(0), out.stride(1))
     return out
 
 
 def swiglu(gate_up: torch.Tensor):
     _need_cuda_bf16(gate_up)
     inter = gate_up.shape[-1] // 2
-    g2 = gate_up.reshape(-1, 2 * inter)
-    if not g2.is_contiguous():
-        g2 = g2.contiguous()
+    g2 = _rows(gate_up, 2 * inter)
     out = torch.empty((g2.shape[0], inter), dtype=torch.bfloat16, device=gate_up.device)
-    _lib.check(_lib.lib().lv_swiglu(g2.data_ptr(), out.data_ptr(), g2.shape[0], inter, _stream()), "lv_swiglu")
+    _call("lv_swiglu", g2.data_ptr(), out.data_ptr(), g2.shape[0], inter)
     return out.view(*gate_up.shape[:-1], inter)
 
 
 def bias_gelu(x: torch.Tensor, bias: Optional[torch.Tensor] = None, approximate: str = "none"):
     _need_cuda_bf16(x, bias)
-    x2 = x.reshape(-1, x.shape[-1])
-    if not x2.is_contiguous():
-        x2 = x2.contiguous()
+    cols = x.shape[-1]
+    x2 = _rows(x, cols)
+    bias = _param("bias_gelu", "bias", bias, cols)
     y = torch.empty_like(x2)
-    _lib.check(
-        _lib.lib().lv_bias_gelu(x2.data_ptr(), _ptr(bias), y.data_ptr(), x2.shape[0], x2.shape[1],
-                                1 if approximate == "tanh" else 0, _stream()),
-        "lv_bias_gelu",
-    )
+    _call("lv_bias_gelu", x2.data_ptr(), _ptr(bias), y.data_ptr(), x2.shape[0], cols, 1 if approximate == "tanh" else 0)
     return y.view(x.shape)
 
 
@@ -496,75 +510,61 @@ def ls_residual(x: torch.Tensor, y: torch.Tensor, ls: Optional[torch.Tensor] = N
                 bias: Optional[torch.Tensor] = None):
     """x + (y + bias) * ls (layer-scale residual); ls / bias optional."""
     _need_cuda_bf16(x, y, ls, bias)
-    x2 = x.reshape(-1, x.shape[-1]).contiguous()
-    y2 = y.reshape(-1, x.shape[-1]).contiguous()
+    cols = x.shape[-1]
+    x2 = _rows(x, cols)
+    y2 = _like("ls_residual", "y", y, x2.shape)
+    ls, bias = _param("ls_residual", "ls", ls, cols), _param("ls_residual", "bias", bias, cols)
     out = torch.empty_like(x2)
-    _lib.check(
-        _lib.lib().lv_ls_residual(x2.data_ptr(), y2.data_ptr(), _ptr(bias), _ptr(ls), out.data_ptr(), x2.shape[0],
-                                  x2.shape[1], _stream()),
-        "lv_ls_residual",
-    )
+    _call("lv_ls_residual", x2.data_ptr(), y2.data_ptr(), _ptr(bias), _ptr(ls), out.data_ptr(), x2.shape[0], cols)
     return out.view(x.shape)
 
 
 def pixel_shuffle(x: torch.Tensor, hw: int, has_cls: bool):
     """[n, (1 +) hw*hw, c] -> [n, (hw/2)^2, 4c]."""
     _need_cuda_bf16(x)
+    if x.dim() != 3 or x.shape[1] != hw * hw + (1 if has_cls else 0):
+        raise ValueError(f"pixel_shuffle: x {tuple(x.shape)} is not [n, (1 +) {hw}*{hw}, c]")
     x = x.contiguous()
     n, _, c = x.shape
     out = torch.empty((n, (hw // 2) ** 2, 4 * c), dtype=torch.bfloat16, device=x.device)
-    _lib.check(_lib.lib().lv_pixel_shuffle(x.data_ptr(), out.data_ptr(), n, hw, c, 1 if has_cls else 0, _stream()),
-               "lv_pixel_shuffle")
+    _call("lv_pixel_shuffle", x.data_ptr(), out.data_ptr(), n, hw, c, 1 if has_cls else 0)
     return out
 
 
 def embed_scatter(ids: torch.Tensor, table: torch.Tensor, feat: Optional[torch.Tensor] = None,
                   dst_idx: Optional[torch.Tensor] = None, src_idx: Optional[torch.Tensor] = None):
     """out[t] = table[ids[t]]; out[dst_idx[i]] = feat[src_idx[i]] (src_idx None => i)."""
-    _need_cuda(ids, torch.int64)
     _need_cuda_bf16(table, feat)
-    ids = ids.contiguous().view(-1)
+    ids = _vec("embed_scatter", "ids", ids, torch.int64)
     n_tok, hidden = ids.numel(), table.shape[1]
     out = torch.empty((n_tok, hidden), dtype=torch.bfloat16, device=table.device)
     n_sc = 0
     if feat is not None:
-        feat = feat.reshape(-1, hidden).contiguous()
-        dst_idx = dst_idx.contiguous().view(-1)
-        _need_cuda(dst_idx, torch.int64)
+        feat = _rows(feat, hidden)
+        dst_idx = _vec("embed_scatter", "dst_idx", dst_idx, torch.int64)
         n_sc = dst_idx.numel()
         if src_idx is not None:
-            src_idx = src_idx.contiguous().view(-1)
-            _need_cuda(src_idx, torch.int64)
-    _lib.check(
-        _lib.lib().lv_embed_scatter(ids.data_ptr(), table.data_ptr(), table.shape[0], _ptr(feat), _ptr(src_idx),
-                                    _ptr(dst_idx), n_sc, out.data_ptr(), n_tok, hidden, _stream()),
-        "lv_embed_scatter",
-    )
+            src_idx = _vec("embed_scatter", "src_idx", src_idx, torch.int64, n_sc)
+    _call("lv_embed_scatter", ids.data_ptr(), table.data_ptr(), table.shape[0], _ptr(feat), _ptr(src_idx), _ptr(dst_idx),
+          n_sc, out.data_ptr(), n_tok, hidden)
     return out
 
 
 def row_gather(x: torch.Tensor, idx: torch.Tensor):
     _need_cuda_bf16(x)
-    _need_cuda(idx, torch.int64)
     x = x.contiguous()
-    idx = idx.contiguous().view(-1)
+    idx = _vec("row_gather", "idx", idx, torch.int64)
     out = torch.empty((idx.numel(), x.shape[1]), dtype=torch.bfloat16, device=x.device)
-    _lib.check(_lib.lib().lv_row_gather(x.data_ptr(), idx.data_ptr(), out.data_ptr(), idx.numel(), x.shape[1], _stream()),
-               "lv_row_gather")
+    _call("lv_row_gather", x.data_ptr(), idx.data_ptr(), out.data_ptr(), idx.numel(), x.shape[1])
     return out
 
 
 def row_scatter_zero(x: torch.Tensor, idx: torch.Tensor, n_rows_out: int):
     _need_cuda_bf16(x)
-    _need_cuda(idx, torch.int64)
     x = x.contiguous()
-    idx = idx.contiguous().view(-1)
+    idx = _vec("row_scatter_zero", "idx", idx, torch.int64)
     out = torch.empty((n_rows_out, x.shape[1]), dtype=torch.bfloat16, device=x.device)
-    _lib.check(
-        _lib.lib().lv_row_scatter_zero(x.data_ptr(), idx.data_ptr(), out.data_ptr(), idx.numel(), n_rows_out, x.shape[1],
-                                       _stream()),
-        "lv_row_scatter_zero",
-    )
+    _call("lv_row_scatter_zero", x.data_ptr(), idx.data_ptr(), out.data_ptr(), idx.numel(), n_rows_out, x.shape[1])
     return out
 
 
@@ -574,11 +574,19 @@ def row_scatter_zero(x: torch.Tensor, idx: torch.Tensor, n_rows_out: int):
 _ACT = {None: 0, "none": 0, "gelu": 1, "gelu_tanh": 2, "swiglu": 3}
 
 
-def _mn_major(t: torch.Tensor) -> bool:
-    """A 2-D transposed view (t.t() of a [K, rows] row-major tensor) that the GEMM reads in place as an MN-major
-    operand: rows contiguous, a column stride that is a multiple of 8 elements, a 16-byte aligned start."""
-    return t.dim() == 2 and t.stride(0) == 1 and t.stride(1) % 8 == 0 and t.stride(1) >= t.shape[0] \
-        and t.data_ptr() % 16 == 0
+def _gemm_operand(t: torch.Tensor, mn_ok: bool = True) -> Tuple[torch.Tensor, bool, int]:
+    """How the wgmma GEMM reads the 2-D operand t [rows, K]: (tensor, mn_major, leading dimension).  K-major in place
+    when K is contiguous, the row stride a multiple of 8 elements and >= K (no overlapping rows) and the start 16-byte
+    aligned; else, unless mn_ok is False, MN-major in place under the same conditions with the two dimensions swapped
+    (t.t() of such a [K, rows] tensor); else a contiguous K-major copy."""
+    (rows, K), (s0, s1) = t.shape, t.stride()
+    aligned = t.data_ptr() % 16 == 0
+    if s1 == 1 and s0 % 8 == 0 and s0 >= K and aligned:
+        return t, False, s0
+    if mn_ok and s0 == 1 and s1 % 8 == 0 and s1 >= rows and aligned:
+        return t, True, s1
+    t = t.clone(memory_format=torch.contiguous_format)
+    return t, False, t.stride(0)
 
 
 def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, act: Optional[str] = None,
@@ -588,14 +596,12 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
     (lv_gemm_ex) instead of a contiguous copy.  Any other layout is copied to a contiguous tensor first."""
     _need_cuda_bf16(x, weight, bias)
     K = x.shape[-1]
+    if weight.dim() != 2 or weight.shape[1] != K:
+        raise ValueError(f"linear: weight {tuple(weight.shape)} is not [N, K={K}]")
     N = weight.shape[0]
-    x2 = x.reshape(-1, K)
-    a_mn = x2.stride(1) != 1 and _mn_major(x2)
-    if not a_mn and (x2.stride(1) != 1 or x2.stride(0) % 8 != 0):
-        x2 = x2.contiguous()
-    w_mn = weight.stride(1) != 1 and _mn_major(weight)
-    if not w_mn and weight.stride(1) != 1:
-        weight = weight.contiguous()
+    bias = _param("linear", "bias", bias, N)
+    x2, a_mn, lda = _gemm_operand(x.reshape(-1, K))
+    weight, w_mn, ldw = _gemm_operand(weight)
     M = x2.shape[0]
     n_out = N // 2 if act == "swiglu" else N      # fused SwiGLU: weight rows interleaved (gate_i, up_i)
     if out is None:
@@ -604,18 +610,11 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
         return out.view(*x.shape[:-1], n_out)
     ev0 = _TIMER.start() if _TIMER is not None else None
     if a_mn or w_mn:
-        _lib.check(
-            _lib.lib().lv_gemm_ex(x2.data_ptr(), weight.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K,
-                                  x2.stride(1) if a_mn else x2.stride(0), weight.stride(1) if w_mn else weight.stride(0),
-                                  out.stride(0), int(a_mn), int(w_mn), _ACT[act], _stream()),
-            "lv_gemm_ex",
-        )
-    else:
-        _lib.check(
-            _lib.lib().lv_gemm_bias_act(x2.data_ptr(), weight.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K,
-                                        x2.stride(0), weight.stride(0), out.stride(0), _ACT[act], _stream()),
-            "lv_gemm_bias_act",
-        )
+        _call("lv_gemm_ex", x2.data_ptr(), weight.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K, lda, ldw, out.stride(0),
+              int(a_mn), int(w_mn), _ACT[act])
+    else:       # the entry point whose decode-sized GEMV path also takes an unaligned `out`
+        _call("lv_gemm_bias_act", x2.data_ptr(), weight.data_ptr(), _ptr(bias), out.data_ptr(), M, N, K, lda, ldw,
+              out.stride(0), _ACT[act])
     if ev0 is not None:
         _TIMER.stop("gemm_bf16", 2.0 * M * N * K, ev0)
     return out.view(*x.shape[:-1], n_out)
@@ -678,16 +677,21 @@ def ce_accumulate(logits: torch.Tensor, labels: torch.Tensor, run_max: torch.Ten
     fp32 row statistics (in place): max, sum of exp(. - max), and the target logit where labels fall in the chunk."""
     _need_cuda_bf16(logits)
     M, n = logits.shape
-    _lib.check(_lib.lib().lv_ce_accumulate(logits.data_ptr(), logits.stride(0), labels.data_ptr(), run_max.data_ptr(),
-                                           run_sum.data_ptr(), tgt.data_ptr(), M, n, col0, _stream()), "lv_ce_accumulate")
+    labels = _vec("ce_accumulate", "labels", labels, torch.int64, M)
+    run_max, run_sum, tgt = (_vec("ce_accumulate", name, t, torch.float32, M, inplace=True)
+                             for name, t in (("run_max", run_max), ("run_sum", run_sum), ("tgt", tgt)))
+    _call("lv_ce_accumulate", logits.data_ptr(), logits.stride(0), labels.data_ptr(), run_max.data_ptr(), run_sum.data_ptr(),
+          tgt.data_ptr(), M, n, col0)
 
 
 def ce_grad(logits: torch.Tensor, labels: torch.Tensor, lse: torch.Tensor, dloss: torch.Tensor, col0: int) -> torch.Tensor:
     """In place: logits[M, n] (a vocabulary chunk) -> d_logits = (exp(logits - lse) - onehot) * dloss (bf16)."""
     _need_cuda_bf16(logits)
     M, n = logits.shape
-    _lib.check(_lib.lib().lv_ce_grad(logits.data_ptr(), logits.stride(0), logits.data_ptr(), logits.stride(0), labels.data_ptr(),
-                                     lse.data_ptr(), dloss.data_ptr(), M, n, col0, _stream()), "lv_ce_grad")
+    labels = _vec("ce_grad", "labels", labels, torch.int64, M)
+    lse, dloss = _vec("ce_grad", "lse", lse, torch.float32, M), _vec("ce_grad", "dloss", dloss, torch.float32, M)
+    _call("lv_ce_grad", logits.data_ptr(), logits.stride(0), logits.data_ptr(), logits.stride(0), labels.data_ptr(),
+          lse.data_ptr(), dloss.data_ptr(), M, n, col0)
     return logits
 
 
@@ -779,9 +783,7 @@ def masked_lm_head_ce(h: torch.Tensor, weight: torch.Tensor, logit_mask: torch.T
     weight [vocab, c], logit_mask [1, s] bool, labels [1, M] (the M selected label ids) -> loss [1, M] fp32.  The
     [M, vocab] logits are never materialised (1M tokens x 152 064 would be 318 GB in bf16).  accumulate_wgrad: the
     weight gradient goes to weight.main_grad, vocabulary chunk by chunk (see linear_autograd)."""
-    if accumulate_wgrad:
-        return _LMHeadCEFn.apply(select_rows(h, logit_mask), weight, labels, vocab_chunk, True)
-    return _LMHeadCEFn.apply(select_rows(h, logit_mask), weight, labels, vocab_chunk)
+    return _LMHeadCEFn.apply(select_rows(h, logit_mask), weight, labels, vocab_chunk, accumulate_wgrad)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -792,24 +794,26 @@ def rmsnorm_bwd(x: torch.Tensor, weight: torch.Tensor, dy: torch.Tensor, eps: fl
     """Gradients of rmsnorm(x, weight): returns (dx [+ add_in], dweight).  `x` is the tensor that was normalised."""
     _need_cuda_bf16(x, weight, dy, add_in)
     cols = x.shape[-1]
-    x2, dy2 = x.reshape(-1, cols).contiguous(), dy.reshape(-1, cols).contiguous()
-    a2 = None if add_in is None else add_in.reshape(-1, cols).contiguous()
+    x2 = _rows(x, cols)
+    dy2 = _like("rmsnorm_bwd", "dy", dy, x2.shape)
+    a2 = None if add_in is None else _like("rmsnorm_bwd", "add_in", add_in, x2.shape)
+    weight = _param("rmsnorm_bwd", "weight", weight, cols)
     rows = x2.shape[0]
     parts = int(_lib.lib().lv_rmsnorm_bwd_partials(rows, cols))
     dw_part = torch.empty((parts, cols), dtype=torch.float32, device=x.device)
     dx = torch.empty_like(x2)
-    _lib.check(_lib.lib().lv_rmsnorm_bwd(x2.data_ptr(), weight.data_ptr(), dy2.data_ptr(), _ptr(a2), dx.data_ptr(),
-                                         dw_part.data_ptr(), rows, cols, float(eps), _stream()), "lv_rmsnorm_bwd")
+    _call("lv_rmsnorm_bwd", x2.data_ptr(), weight.data_ptr(), dy2.data_ptr(), _ptr(a2), dx.data_ptr(), dw_part.data_ptr(),
+          rows, cols, float(eps))
     return dx.view(x.shape), dw_part.sum(dim=0).to(torch.bfloat16)
 
 
 def swiglu_bwd(gate_up: torch.Tensor, dh: torch.Tensor):
     _need_cuda_bf16(gate_up, dh)
     inter = gate_up.shape[-1] // 2
-    g2, d2 = gate_up.reshape(-1, 2 * inter).contiguous(), dh.reshape(-1, inter).contiguous()
+    g2 = _rows(gate_up, 2 * inter)
+    d2 = _like("swiglu_bwd", "dh", dh, (g2.shape[0], inter))
     out = torch.empty_like(g2)
-    _lib.check(_lib.lib().lv_swiglu_bwd(g2.data_ptr(), d2.data_ptr(), out.data_ptr(), g2.shape[0], inter, _stream()),
-               "lv_swiglu_bwd")
+    _call("lv_swiglu_bwd", g2.data_ptr(), d2.data_ptr(), out.data_ptr(), g2.shape[0], inter)
     return out.view(gate_up.shape)
 
 
@@ -905,20 +909,14 @@ class _LinearFn(torch.autograd.Function):
         return dx, dw, db, None
 
 
-def _wgrad_operands(dy2: torch.Tensor, x2: torch.Tensor):
-    """dY [T, N] and X [T, K] as the GEMM reads them transposed in place (MN-major): unit column stride, a row stride
-    that is a multiple of 8 elements, a 16-byte aligned start; any other layout is copied to a contiguous tensor."""
-    return tuple(t if t.stride(1) == 1 and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0 else t.contiguous()
-                 for t in (dy2, x2))
-
-
 def linear_wgrad(dy2: torch.Tensor, x2: torch.Tensor) -> torch.Tensor:
     """dW [N, K] = dY^T [N, T] . X [T, K] on the wgmma GEMM, the token dimension T being the contraction: dY^T and X^T
     are read in place as MN-major operands, so T may be any length.  Without tokens (a context-parallel rank that
     owns no answer token) dW is zero and no GEMM runs."""
     if dy2.shape[0] == 0:
         return torch.zeros((dy2.shape[1], x2.shape[1]), dtype=dy2.dtype, device=dy2.device)
-    dy2, x2 = _wgrad_operands(dy2, x2)
+    # dY and X in place when the GEMM can read their transposes MN-major, else contiguous copies (_gemm_operand)
+    (dy2, _, _), (x2, _, _) = _gemm_operand(dy2, mn_ok=False), _gemm_operand(x2, mn_ok=False)
     return linear(dy2.t(), x2.t())                                           # [N, K] = dY^T [N, T] . (X^T)[K, T]^T
 
 
@@ -937,13 +935,14 @@ def linear_wgrad_accumulate(dy2: torch.Tensor, x2: torch.Tensor, main_grad: torc
         raise RuntimeError(f"linear_wgrad_accumulate: main_grad (strides {main_grad.stride()}) must have unit column "
                            "stride, a row stride that is a multiple of 4 and a 16-byte aligned start")
     T = dy2.shape[0]
+    if x2.shape[0] != T:
+        raise ValueError(f"linear_wgrad_accumulate: dY has {T} tokens, X has {x2.shape[0]}")
     if T == 0:
         return main_grad
-    dy2, x2 = _wgrad_operands(dy2, x2)
+    (dy2, _, lda), (x2, _, ldw) = _gemm_operand(dy2, mn_ok=False), _gemm_operand(x2, mn_ok=False)
     ev0 = _TIMER.start() if _TIMER is not None else None
-    _lib.check(_lib.lib().lv_gemm_wgrad_acc_f32(dy2.data_ptr(), x2.data_ptr(), main_grad.data_ptr(), n_out, k_in, T,
-                                                dy2.stride(0), x2.stride(0), main_grad.stride(0), 1, 1, _stream()),
-               "lv_gemm_wgrad_acc_f32")
+    _call("lv_gemm_wgrad_acc_f32", dy2.data_ptr(), x2.data_ptr(), main_grad.data_ptr(), n_out, k_in, T, lda, ldw,
+          main_grad.stride(0), 1, 1)
     if ev0 is not None:
         _TIMER.stop("gemm_bf16", 2.0 * n_out * k_in * T, ev0)
     return main_grad
@@ -976,7 +975,7 @@ def fused_wgrad_dummy(weight: torch.Tensor, main_grad: torch.Tensor, dtype: torc
 def linear_autograd(x, weight, bias=None, accumulate_wgrad: bool = False):
     """Differentiable linear (see _LinearFn).  accumulate_wgrad: the weight gradient is added to weight.main_grad
     (fp32) and the returned gradient follows fused_wgrad_dummy; the bias gradient is unchanged."""
-    if accumulate_wgrad:
+    if accumulate_wgrad:        # otherwise the node keeps three inputs, as a backward written for x, weight, bias expects
         return _LinearFn.apply(x, weight, bias, True)
     return _LinearFn.apply(x, weight, bias)
 
@@ -990,15 +989,15 @@ def patch_embed(images: torch.Tensor, w_pad: torch.Tensor, bias: Optional[torch.
     n, _, size, _ = images.shape
     Cc = w_pad.shape[0]
     P = (size // patch) ** 2
+    S = P + (0 if cls is None else 1)
+    w_pad = _like("patch_embed", "w_pad", w_pad, (Cc, (3 * patch * patch + 63) // 64 * 64))
+    bias, cls = _param("patch_embed", "bias", bias, Cc), _param("patch_embed", "cls", cls, Cc)
+    pos = _param("patch_embed", "pos", pos, S * Cc)
     ws_bytes = int(_lib.lib().lv_patch_embed_ws_bytes(n, size, patch, Cc))
     ws = torch.empty(ws_bytes // 2, dtype=torch.bfloat16, device=images.device)
-    out = torch.empty((n, P + (0 if cls is None else 1), Cc), dtype=torch.bfloat16, device=images.device)
-    _lib.check(
-        _lib.lib().lv_patch_embed(images.data_ptr(), w_pad.contiguous().data_ptr(), _ptr(bias),
-                                  None if cls is None else cls.contiguous().data_ptr(), pos.contiguous().data_ptr(), out.data_ptr(),
-                                  ws.data_ptr(), n, size, patch, Cc, _stream()),
-        "lv_patch_embed",
-    )
+    out = torch.empty((n, S, Cc), dtype=torch.bfloat16, device=images.device)
+    _call("lv_patch_embed", images.data_ptr(), w_pad.data_ptr(), _ptr(bias), _ptr(cls), pos.data_ptr(), out.data_ptr(),
+          ws.data_ptr(), n, size, patch, Cc)
     return out
 
 
@@ -1028,16 +1027,17 @@ def layernorm_bwd(x: torch.Tensor, weight: torch.Tensor, dy: torch.Tensor, eps: 
         raise ValueError("layernorm_bwd: add_in needs dx")
     _need_cuda_bf16(x, weight, dy, add_in)
     cols = x.shape[-1]
-    x2, dy2 = x.reshape(-1, cols).contiguous(), dy.reshape(-1, cols).contiguous()
-    a2 = None if add_in is None else add_in.reshape(-1, cols).contiguous()
+    x2 = _rows(x, cols)
+    dy2 = _like("layernorm_bwd", "dy", dy, x2.shape)
+    a2 = None if add_in is None else _like("layernorm_bwd", "add_in", add_in, x2.shape)
+    weight = _param("layernorm_bwd", "weight", weight, cols)
     rows = x2.shape[0]
     parts = int(_lib.lib().lv_layernorm_bwd_partials(rows, cols))
     dw_part = torch.empty((parts, cols), dtype=torch.float32, device=x.device)
     db_part = torch.empty((parts, cols), dtype=torch.float32, device=x.device)
     dx = torch.empty_like(x2) if need_dx else None
-    _lib.check(_lib.lib().lv_layernorm_bwd(x2.data_ptr(), weight.data_ptr(), dy2.data_ptr(), _ptr(a2), _ptr(dx),
-                                           dw_part.data_ptr(), db_part.data_ptr(), rows, cols, float(eps), _stream()),
-               "lv_layernorm_bwd")
+    _call("lv_layernorm_bwd", x2.data_ptr(), weight.data_ptr(), dy2.data_ptr(), _ptr(a2), _ptr(dx), dw_part.data_ptr(),
+          db_part.data_ptr(), rows, cols, float(eps))
     return (None if dx is None else dx.view(x.shape)), dw_part.sum(dim=0).to(torch.bfloat16), db_part.sum(dim=0).to(torch.bfloat16)
 
 
@@ -1045,10 +1045,10 @@ def gelu_bwd(pre: torch.Tensor, dy: torch.Tensor, approximate: str = "none"):
     """dx = dy * gelu'(pre); `approximate` as in bias_gelu ("none" = erf, "tanh")."""
     _need_cuda_bf16(pre, dy)
     cols = pre.shape[-1]
-    p2, d2 = pre.reshape(-1, cols).contiguous(), dy.reshape(-1, cols).contiguous()
+    p2 = _rows(pre, cols)
+    d2 = _like("gelu_bwd", "dy", dy, p2.shape)
     dx = torch.empty_like(p2)
-    _lib.check(_lib.lib().lv_gelu_bwd(p2.data_ptr(), d2.data_ptr(), dx.data_ptr(), p2.shape[0], cols,
-                                      1 if approximate == "tanh" else 0, _stream()), "lv_gelu_bwd")
+    _call("lv_gelu_bwd", p2.data_ptr(), d2.data_ptr(), dx.data_ptr(), p2.shape[0], cols, 1 if approximate == "tanh" else 0)
     return dx.view(pre.shape)
 
 
@@ -1057,25 +1057,27 @@ def ls_residual_bwd(dout: torch.Tensor, y: torch.Tensor, ls: torch.Tensor):
     The gradient of x is dout itself."""
     _need_cuda_bf16(dout, y, ls)
     cols = y.shape[-1]
-    d2, y2 = dout.reshape(-1, cols).contiguous(), y.reshape(-1, cols).contiguous()
+    y2 = _rows(y, cols)
+    d2 = _like("ls_residual_bwd", "dout", dout, y2.shape)
+    ls = _param("ls_residual_bwd", "ls", ls, cols)
     rows = y2.shape[0]
     parts = int(_lib.lib().lv_ls_residual_bwd_partials(rows, cols))
     dls_part = torch.empty((parts, cols), dtype=torch.float32, device=y.device)
     dy = torch.empty_like(y2)
-    _lib.check(_lib.lib().lv_ls_residual_bwd(d2.data_ptr(), y2.data_ptr(), ls.contiguous().data_ptr(), dy.data_ptr(),
-                                             dls_part.data_ptr(), rows, cols, _stream()), "lv_ls_residual_bwd")
+    _call("lv_ls_residual_bwd", d2.data_ptr(), y2.data_ptr(), ls.data_ptr(), dy.data_ptr(), dls_part.data_ptr(), rows, cols)
     return dy.view(y.shape), dls_part.sum(dim=0).to(torch.bfloat16)
 
 
 def pixel_shuffle_bwd(dout: torch.Tensor, hw: int, has_cls: bool):
     """[n, (hw/2)^2, 4c] -> [n, (1 +) hw*hw, c]: the inverse permutation of pixel_shuffle (class-token rows zero)."""
     _need_cuda_bf16(dout)
+    if dout.dim() != 3 or dout.shape[1] != (hw // 2) ** 2:
+        raise ValueError(f"pixel_shuffle_bwd: dout {tuple(dout.shape)} is not [n, ({hw}/2)^2, 4c]")
     dout = dout.contiguous()
     n, _, c4 = dout.shape
     c = c4 // 4
     dx = torch.empty((n, hw * hw + (1 if has_cls else 0), c), dtype=torch.bfloat16, device=dout.device)
-    _lib.check(_lib.lib().lv_pixel_shuffle_bwd(dout.data_ptr(), dx.data_ptr(), n, hw, c, 1 if has_cls else 0, _stream()),
-               "lv_pixel_shuffle_bwd")
+    _call("lv_pixel_shuffle_bwd", dout.data_ptr(), dx.data_ptr(), n, hw, c, 1 if has_cls else 0)
     return dx
 
 
@@ -1085,8 +1087,7 @@ def patch_im2col(images: torch.Tensor, patch: int, kpad: int):
     images = images.contiguous()
     n, _, size, _ = images.shape
     col = torch.empty((n * (size // patch) ** 2, kpad), dtype=torch.bfloat16, device=images.device)
-    _lib.check(_lib.lib().lv_patch_im2col(images.data_ptr(), col.data_ptr(), n, size, patch, kpad, _stream()),
-               "lv_patch_im2col")
+    _call("lv_patch_im2col", images.data_ptr(), col.data_ptr(), n, size, patch, kpad)
     return col
 
 
@@ -1216,9 +1217,7 @@ def patch_embed_autograd(images, conv_w, conv_b, cls, pos, patch: int, accumulat
     elements, e.g. [1, 1, C]), pos [1 + (S/patch)^2, C] -> [n, 1 + (S/patch)^2, C].  Gradients: conv weight, conv bias,
     class token (sum over frames of row 0), position embedding (sum over frames); none for the images.
     accumulate_wgrad: the conv weight gradient goes to conv_w.main_grad (see linear_autograd)."""
-    if accumulate_wgrad:
-        return _PatchEmbedFn.apply(images, conv_w, conv_b, cls, pos, patch, True)
-    return _PatchEmbedFn.apply(images, conv_w, conv_b, cls, pos, patch)
+    return _PatchEmbedFn.apply(images, conv_w, conv_b, cls, pos, patch, accumulate_wgrad)
 
 
 class _ViTAttentionFn(torch.autograd.Function):

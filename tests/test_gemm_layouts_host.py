@@ -152,3 +152,41 @@ def test_lv_gemm_ex_rejects_bad_arguments_without_a_gpu(lib_built):
     assert rc == -1 and b"SwiGLU" in msg
     rc, msg = ex(P, P, None, P, 4, 8, 0, 8, 8, 8, 1, 1, 0)
     assert rc == -1 and b"bad shape" in msg
+
+
+P16 = 256          # a 16-byte aligned fake address: every refused tuple fails its checks before touching memory
+#                 A        W    bias  C    M   N   K   lda ldw ldc [a_mn w_mn] act
+REFUSED = [
+    ("lv_gemm_bias_act", (None, P16, None, P16, 4, 8, 8, 8, 8, 8, 0), [b"null pointer"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, -1, 8, 8, 8, 8, 8, 0), [b"bad shape"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, 4, 8, 0, 8, 8, 8, 0), [b"bad shape"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, 4, 8, 7, 8, 8, 8, 0), [b"K=7", b"multiples of 8"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, 4, 12, 8, 8, 8, 16, 0), [b"N=12", b"multiples of 8"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, 4, 8, 8, 8, 8, 8, 4), [b"unknown activation"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, 4, 8, 16, 8, 16, 8, 0), [b"lda=8", b"K=16"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, 4, 8, 16, 16, 12, 8, 0), [b"ldw=12"]),
+    ("lv_gemm_bias_act", (P16, P16, None, P16, 4, 32, 16, 16, 16, 8, 0), [b"ldc=8"]),
+    ("lv_gemm_bias_act", (P16, P16, P16, P16, 4, 32, 16, 16, 16, 16, 3), [b"SwiGLU"]),
+    ("lv_gemm_ex", (P16, P16, None, P16, 4, 8, 8, 8, 8, 8, 0, 0, 0), []),         # K-major both: checked, then bias_act
+    ("lv_gemm_ex", (P16 + 8, P16, None, P16, 4, 8, 8, 8, 8, 8, 0, 0, 0), [b"16-byte aligned"]),
+    ("lv_gemm_ex", (P16, P16, None, P16, 4, 12, 8, 8, 8, 16, 0, 1, 0), [b"N=12"]),
+    ("lv_gemm_ex", (P16, P16, None, P16, 4, 8, 8, 8, 4, 8, 0, 1, 0), [b"ldw=4", b"N=8"]),
+    ("lv_gemm_ex", (P16, P16, None, P16, 4, 8, 1 << 31, 8, 8, 8, 1, 1, 0), [b"too large"]),
+    ("lv_gemm_wgrad_acc_f32", (P16, P16, P16, 64, 64, 16, 64, 64, 64, 1, 1), []),   # accepted (stops at device binding)
+    ("lv_gemm_wgrad_acc_f32", (P16, P16, P16, 64, 64, 16, 64, 64, 64, 1, 2), [b"must be 0 or 1"]),
+    ("lv_gemm_wgrad_acc_f32", (P16, P16, P16, 64, 60, 16, 64, 64, 64, 1, 1), []),   # N a multiple of 4 is enough
+    ("lv_gemm_wgrad_acc_f32", (P16, P16, P16, 64, 64, 7, 64, 64, 64, 1, 1), []),    # any K
+]
+
+
+@pytest.mark.parametrize("entry,args,msgs", REFUSED)
+def test_gemm_entry_points_share_one_argument_check(lib_built, entry, args, msgs):
+    """Refused tuples return -1 with the message; accepted ones pass the checks and stop at device binding here."""
+    from long_vita_b200 import _lib
+
+    h = _lib.lib()
+    rc = getattr(h, entry)(*args, None)
+    if msgs:
+        assert rc == -1 and all(m in h.lv_last_error() for m in msgs), h.lv_last_error()
+    else:
+        assert rc != -1 or b"16-byte" in h.lv_last_error() or b"not device memory" in h.lv_last_error(), h.lv_last_error()
