@@ -408,6 +408,7 @@ class ContextParallelRunner:
             feat = m.encode_images(images[sh.image_sel])
         x = ops.embed_scatter(sh.input_ids, m.embed_tokens, feat, sh.dst_idx if feat is not None else None,
                               sh.src_idx if feat is not None else None)
+        feat = None                         # scattered into x: not held through the decoder
         cos, sin = ops.rope_table(sh.position_ids.to(torch.int64), m.inv_freq)
         T = x.shape[0]
         self.cache = None
@@ -417,7 +418,7 @@ class ContextParallelRunner:
             self.cache = KVCache(len(m.layers), T + -(-max_new_tokens // self.cp) + 1, cfg.num_key_value_heads, cfg.head_dim, dev)
             self.total_len = S
         h = run_layers(m.layers, x, cos, sin, exchange_attention(ctx, self.cache), m.norm_w, cfg.rms_norm_eps,
-                       cache=self.cache, qkv_out=ctx.qkv_buffer)
+                       cache=self.cache, qkv_out=ctx.qkv_buffer, donate=True)
         # logit mask: each rank projects its own last row; the globally-last token lives on rank 0
         # (chunk 2cp-1), generation.py:141-165
         row = sh.last_token_local if sh.last_token_local >= 0 else T - 1

@@ -115,6 +115,37 @@ class ResamplerProjector:
     __call__ = forward
 
 
+# Row chunking of the decoder layer's token-wise work.  Up to ROW_CHUNK_THRESHOLD rows a layer runs each op once over
+# all rows.  Above it, the ops before and after attention run on near-equal chunks of about ROW_CHUNK rows, so that
+# only x, the QKV buffer, the attention output and the RoPE tables span the whole sequence: ~35 KB per token at the
+# 14B geometry instead of ~103 KB (the whole-tensor layer also holds the [T, 13824] SwiGLU output, the MLP output and
+# a second copy of x), which is what lets a ~1M-token prompt prefill on one 80 GB H100.
+#
+# Chunking is bit-identical to the whole-tensor call.  RMSNorm, RoPE and the residual add compute each row on its
+# own, and their launch shape depends only on the column count.  The wgmma GEMM (gemm.cu) has no split-K: an output
+# element is one accumulation over K in a fixed k-order, whatever M is, and since every chunk but the last starts
+# at a multiple of its 128-row tile, each row even sits at the same place in its tile as in the whole call.  What
+# would change the sum order is the GEMV path, which lv_gemm_bias_act takes for M <= 4, so no chunk is that short.
+ROW_CHUNK_THRESHOLD = 262_144
+ROW_CHUNK = 65_536
+_ROW_ALIGN = 128            # the GEMM's M tile
+_GEMV_MAX_ROWS = 4          # lv_gemm_bias_act's GEMV path
+
+
+def row_chunks(T: int) -> List[Tuple[int, int]]:
+    """The row spans [r0, r1) a decoder layer of T rows runs its token-wise ops on: [(0, T)] up to
+    ROW_CHUNK_THRESHOLD rows, else near-equal chunks of about ROW_CHUNK rows, each a multiple of 128 rows but the
+    last, and none of 4 rows or fewer."""
+    if T <= ROW_CHUNK_THRESHOLD:
+        return [(0, T)]
+    n = -(-T // ROW_CHUNK)
+    size = -(-T // (n * _ROW_ALIGN)) * _ROW_ALIGN
+    spans = [(r, min(r + size, T)) for r in range(0, T, size)]
+    if len(spans) > 1 and spans[-1][1] - spans[-1][0] <= _GEMV_MAX_ROWS:
+        spans[-2:] = [(spans[-2][0], T)]
+    return spans
+
+
 class DecoderLayer:
     """Qwen2 decoder layer (transformers Qwen2DecoderLayer, instantiated by the reference at
     modeling_long_vita.py:57-72; mcore twin transformer_layer.py:173-257) with fused QKV and fused
@@ -135,16 +166,25 @@ class DecoderLayer:
         self.ln2 = w[p + "post_attention_layernorm.weight"]
 
     def forward(self, x: torch.Tensor, delta: Optional[torch.Tensor], cos, sin, attend,
-                qkv_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                qkv_out: Optional[torch.Tensor] = None,
+                inplace: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """x [T, H] residual stream, `delta` the previous layer's MLP output not yet added (the add is fused into this
         layer's first RMSNorm), or None.  Returns (x, delta).
 
         `attend(q, k, v)` is the attention step: q [T, hq, d], k / v [T, hkv, d] are views of the QKV GEMM output,
         after RoPE (skipped when `cos` is None); it returns the attention output ([T, hq * d] in any shape).
         `qkv_out` is a caller buffer [T, (hq + 2 hkv) d] for the QKV GEMM, e.g. the peer-mapped buffer that the
-        context-parallel kernel reads the other ranks' K/V from."""
+        context-parallel kernel reads the other ranks' K/V from.
+
+        Above ROW_CHUNK_THRESHOLD rows the ops before and after attention run chunk by chunk (row_chunks); attention
+        is still one call over all rows, enqueued after every QKV row is written.  Each chunk's MLP output is then
+        added to its rows of x at once and the returned delta is None.  With several chunks and `inplace`, x itself
+        is that residual stream (its rows are overwritten); otherwise the layer writes a new one."""
         cfg = self.cfg
         T = x.shape[0]
+        spans = row_chunks(T)
+        if len(spans) > 1:
+            return self._forward_chunked(x, delta, cos, sin, attend, qkv_out, spans, inplace)
         hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
         if delta is None:
             h = ops.rmsnorm(x, self.ln1, cfg.rms_norm_eps)
@@ -162,20 +202,54 @@ class DecoderLayer:
         a = ops.linear(h, self.w_gate_up, act="swiglu")
         return x, ops.linear(a, self.w_down)
 
+    def _forward_chunked(self, x, delta, cos, sin, attend, qkv_out, spans, inplace):
+        """forward() over the row spans `spans`: the same ops, each on its rows of x, the QKV buffer and the RoPE
+        tables; returns (x with this layer's MLP output added, None)."""
+        cfg = self.cfg
+        T = x.shape[0]
+        hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+        eps = cfg.rms_norm_eps
+        qkv = qkv_out if qkv_out is not None else torch.empty((T, (hq + 2 * hkv) * d), dtype=x.dtype, device=x.device)
+        q = qkv[:, : hq * d].view(T, hq, d)
+        k = qkv[:, hq * d : (hq + hkv) * d].view(T, hkv, d)
+        v = qkv[:, (hq + hkv) * d :].view(T, hkv, d)
+        xs = x if delta is None or inplace else torch.empty_like(x)         # x + delta
+        for r0, r1 in spans:
+            if delta is None:
+                h = ops.rmsnorm(x[r0:r1], self.ln1, eps)
+            else:
+                h, _ = ops.rmsnorm(delta[r0:r1], self.ln1, eps, residual=x[r0:r1], out=xs[r0:r1])
+            ops.linear(h, self.wqkv, self.bqkv, out=qkv[r0:r1])
+            if cos is not None:
+                ops.rope(q[r0:r1], cos[r0:r1], sin[r0:r1], out=q[r0:r1])
+                ops.rope(k[r0:r1], cos[r0:r1], sin[r0:r1], out=k[r0:r1])
+        x, h, delta = xs, None, None
+        o = attend(q, k, v).reshape(T, hq * d)
+        del q, k, v, qkv                    # the QKV buffer is released (unless it is the caller's) before the MLP
+        xo = x if inplace else torch.empty_like(x)
+        for r0, r1 in spans:
+            h, _ = ops.rmsnorm(ops.linear(o[r0:r1], self.wo), self.ln2, eps, residual=x[r0:r1], out=xo[r0:r1])
+            m = ops.linear(ops.linear(h, self.w_gate_up, act="swiglu"), self.w_down)
+            ops.ls_residual(xo[r0:r1], m, out=xo[r0:r1])      # the add the next layer's first RMSNorm would fuse
+        return xo, None
+
 
 def run_layers(layers, x: torch.Tensor, cos, sin, attend, norm_w: torch.Tensor, eps: float, *, cache=None,
-               qkv_out=None, hidden: Optional[list] = None) -> torch.Tensor:
+               qkv_out=None, hidden: Optional[list] = None, donate: bool = False) -> torch.Tensor:
     """The decoder stack: x [T, H] embeddings -> the final RMSNorm of the last hidden state [T, H].
 
     Each layer's MLP output is handed on as `delta` and added inside the next RMSNorm (the last one inside the final
-    norm).  `attend(layer_index, q, k, v)` is the attention step (DecoderLayer.forward); `qkv_out()`, if given, the QKV
-    GEMM's output buffer of the next layer.  The K/V rows appended to `cache` during the pass are committed at its
-    end.  `hidden` (a list) receives each layer's input hidden state."""
+    norm); a layer that runs in row chunks (row_chunks) adds it itself.  `attend(layer_index, q, k, v)` is the
+    attention step (DecoderLayer.forward); `qkv_out()`, if given, the QKV GEMM's output buffer of the next layer.  The
+    K/V rows appended to `cache` during the pass are committed at its end.  `hidden` (a list) receives each layer's
+    input hidden state.  `donate`: x was made for this call (an embedding output), so chunked layers may update it in
+    place; the stack's own residual stream is updated in place from the second layer on (unless `hidden` keeps it)."""
     delta = None
     for li, layer in enumerate(layers):
         if hidden is not None:
             hidden.append(x if delta is None else x + delta)
-        x, delta = layer.forward(x, delta, cos, sin, partial(attend, li), None if qkv_out is None else qkv_out())
+        x, delta = layer.forward(x, delta, cos, sin, partial(attend, li), None if qkv_out is None else qkv_out(),
+                                 inplace=(donate or li > 0) and hidden is None)
     if cache is not None:
         cache.commit()
     if delta is None:
@@ -335,6 +409,7 @@ class LongVITAModel(_WeightHolderModule):
                 idx_b, idx_s = image_indices.to(input_ids.device).unbind(dim=0)
                 dst = (idx_b.reshape(-1) * s + idx_s.reshape(-1)).to(torch.int64)
                 x = ops.embed_scatter(input_ids, self.embed_tokens, image_embeds, dst)
+                image_embeds = None                 # scattered into x: not held through the decoder
             else:
                 x = ops.embed_scatter(input_ids, self.embed_tokens)
         else:
@@ -361,7 +436,7 @@ class LongVITAModel(_WeightHolderModule):
 
         hidden = [] if output_hidden_states else None
         h = run_layers(self.layers, x, cos, sin, attention_step(cache, cu), self.norm_w, cfg.rms_norm_eps, cache=cache,
-                       hidden=hidden).view(1, s, -1)
+                       hidden=hidden, donate=inputs_embeds is None).view(1, s, -1)
         all_hidden = tuple(t.view(1, s, -1) for t in hidden) + (h,) if output_hidden_states else None
         out = BaseOutput(last_hidden_state=h, past_key_values=cache, hidden_states=all_hidden)
         return out if (return_dict is None or return_dict) else out.to_tuple()

@@ -143,6 +143,7 @@ class B200GPTVLModel:
                     if "indices" in key or key == "pre_len":
                         efd[key] = external_inputs[key]
                 x = self.embedding(input_ids, position_ids, efd)
+                feat = efd = None                   # scattered into x: not held through the decoder
             else:
                 x = self.embedding(input_ids, position_ids)
             s = x.shape[0]
@@ -181,10 +182,10 @@ class B200GPTVLModel:
 
         if self.cp is None:
             h = run_layers(self.layers, x, cos, sin, attention_step(cache, cu), self.final_layernorm, cfg.rms_norm_eps,
-                           cache=cache)
+                           cache=cache, donate=decoder_input is None)
         else:
             h = run_layers(self.layers, x, cos, sin, exchange_attention(self.cp), self.final_layernorm,
-                           cfg.rms_norm_eps, qkv_out=self.cp.qkv_buffer)
+                           cfg.rms_norm_eps, qkv_out=self.cp.qkv_buffer, donate=decoder_input is None)
         hidden_states = h.view(s, 1, -1)
 
         # training tail, fused: masked row gather -> LM head -> per-token cross-entropy, chunked over the vocabulary so

@@ -153,7 +153,8 @@ class B200TransformerLayer(torch.nn.Module):
         else:
             attend = partial(attention_step(cu_seqlens=megatron_cu_seqlens(s, hidden_states.device)), 0)
         x, d = layer.forward(hidden_states.reshape(s, h), None, cos, sin, attend)
-        out = ops.ls_residual(x, d)           # plain residual add (bias-dropout-add with p = 0, no bias)
+        # plain residual add (bias-dropout-add with p = 0, no bias); a layer run in row chunks has added it already
+        out = x if d is None else ops.ls_residual(x, d)
         return out.view(s, b, h), context
 
 

@@ -437,17 +437,41 @@ def decode_merge(o_part: torch.Tensor, lse_part: torch.Tensor, return_lse: bool 
 # ------------------------------------------------------------------------------------------------
 # token-wise operators
 # ------------------------------------------------------------------------------------------------
-def rmsnorm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, residual: Optional[torch.Tensor] = None):
-    """RMSNorm over the last dim.  With `residual`, returns (norm(x + residual), x + residual)."""
+def _out_rows(op: str, out: torch.Tensor, shape, *inputs: torch.Tensor) -> torch.Tensor:
+    """A caller's output buffer as the contiguous [rows, cols] `shape` the kernel writes.  It may be one of `inputs`
+    itself (in place: each of these kernels writes an element only from the thread that read it, after reading it)
+    but must not partly overlap one, where a thread would overwrite rows another thread has still to read."""
+    _need_cuda_bf16(out)
+    if out.numel() != shape[0] * shape[1] or not out.is_contiguous():
+        raise ValueError(f"{op}: out {tuple(out.shape)} must be a contiguous tensor of the {shape[0]} rows of {shape[1]} "
+                         "it receives")
+    lo, hi = out.data_ptr(), out.data_ptr() + 2 * out.numel()
+    for t in inputs:
+        if t is not None and t.data_ptr() != lo and t.data_ptr() < hi and lo < t.data_ptr() + 2 * t.numel():
+            raise ValueError(f"{op}: out overlaps an input without being it")
+    return out.view(shape)
+
+
+def rmsnorm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6, residual: Optional[torch.Tensor] = None,
+            out: Optional[torch.Tensor] = None):
+    """RMSNorm over the last dim.  With `residual`, returns (norm(x + residual), x + residual); `out`, if given,
+    receives x + residual (it may be `residual` or `x` itself, e.g. a row slice of the residual stream)."""
     _need_cuda_bf16(x, weight, residual)
     cols = x.shape[-1]
     x2 = _rows(x, cols)
     res2 = None if residual is None else _like("rmsnorm", "residual", residual, x2.shape)
+    if out is not None and residual is None:
+        raise ValueError("rmsnorm: out receives x + residual; it needs a residual")
     weight = _param("rmsnorm", "weight", weight, cols)
     y = torch.empty_like(x2)
-    s = None if residual is None else torch.empty_like(x2)
+    if residual is None:
+        s = None
+    else:
+        s = torch.empty_like(x2) if out is None else _out_rows("rmsnorm", out, x2.shape, x2, res2)
     _call("lv_rmsnorm", x2.data_ptr(), _ptr(res2), weight.data_ptr(), y.data_ptr(), _ptr(s), x2.shape[0], cols, float(eps))
-    return y.view(x.shape) if s is None else (y.view(x.shape), s.view(x.shape))
+    if s is None:
+        return y.view(x.shape)
+    return y.view(x.shape), (s.view(x.shape) if out is None else out)
 
 
 def layernorm(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor], eps: float = 1e-6):
@@ -507,16 +531,17 @@ def bias_gelu(x: torch.Tensor, bias: Optional[torch.Tensor] = None, approximate:
 
 
 def ls_residual(x: torch.Tensor, y: torch.Tensor, ls: Optional[torch.Tensor] = None,
-                bias: Optional[torch.Tensor] = None):
-    """x + (y + bias) * ls (layer-scale residual); ls / bias optional."""
+                bias: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None):
+    """x + (y + bias) * ls (layer-scale residual); ls / bias optional.  `out`, if given, receives the result (it may
+    be `x` or `y` itself: `ls_residual(x, d, out=x)` is x += d)."""
     _need_cuda_bf16(x, y, ls, bias)
     cols = x.shape[-1]
     x2 = _rows(x, cols)
     y2 = _like("ls_residual", "y", y, x2.shape)
     ls, bias = _param("ls_residual", "ls", ls, cols), _param("ls_residual", "bias", bias, cols)
-    out = torch.empty_like(x2)
-    _call("lv_ls_residual", x2.data_ptr(), y2.data_ptr(), _ptr(bias), _ptr(ls), out.data_ptr(), x2.shape[0], cols)
-    return out.view(x.shape)
+    o2 = torch.empty_like(x2) if out is None else _out_rows("ls_residual", out, x2.shape, x2, y2)
+    _call("lv_ls_residual", x2.data_ptr(), y2.data_ptr(), _ptr(bias), _ptr(ls), o2.data_ptr(), x2.shape[0], cols)
+    return o2.view(x.shape) if out is None else out
 
 
 def pixel_shuffle(x: torch.Tensor, hw: int, has_cls: bool):
