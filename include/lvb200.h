@@ -253,11 +253,15 @@ int lv_embed_scatter(const int64_t* ids, const void* table, int64_t vocab, const
 
 /* Row gather / scatter used by the logit-masked LM head:
  * gather:  out[i, :] = x[idx[i], :]                     (masked_select, layers.py:402-407)
- * scatter: out[idx[i], :] = x[i, :], other rows zero    (masked_scatter, layers.py:446-451) */
+ * scatter: out[idx[i], :] = x[i, :], other rows zero    (masked_scatter, layers.py:446-451)
+ * lv_row_scatter: out[idx[i], :] = x[i, :] into an existing [n_rows_out, cols] out, other rows untouched (one
+ * chunk of image features into the embedded prompt); a bit-exact copy, targets outside [0, n_rows_out) dropped. */
 int lv_row_gather(const void* x, const int64_t* idx, void* out, int64_t n_idx, int64_t cols,
                   lv_stream_t stream);
 int lv_row_scatter_zero(const void* x, const int64_t* idx, void* out, int64_t n_idx, int64_t n_rows_out,
                         int64_t cols, lv_stream_t stream);
+int lv_row_scatter(const void* x, const int64_t* idx, void* out, int64_t n_idx, int64_t n_rows_out, int64_t cols,
+                   lv_stream_t stream);
 
 /* Backward of the token-wise operators (training through the `--spec` layer, SURVEY.md 8f-1).
  * RMSNorm: g = dy*w, dx = rstd*(g - xhat*mean(g*xhat)) (+ add_in, the gradient arriving on the residual stream),

@@ -88,6 +88,7 @@ SIGNATURES = {
     "lv_embed_scatter": (c_i32, [c_ptr, c_ptr, c_i64, c_ptr, c_ptr, c_ptr, c_i64, c_ptr, c_i64, c_i64, c_ptr]),
     "lv_row_gather": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_ptr]),
     "lv_row_scatter_zero": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr]),
+    "lv_row_scatter": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr]),
     "lv_rmsnorm_bwd_partials": (c_i64, [c_i64, c_i64]),
     "lv_rmsnorm_bwd": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_f32, c_ptr]),
     "lv_swiglu_bwd": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_ptr]),

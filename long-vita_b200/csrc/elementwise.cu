@@ -1039,6 +1039,19 @@ int lv_row_scatter_zero(const void* x, const int64_t* idx, void* out, int64_t n_
   return LV_OK;
 }
 
+int lv_row_scatter(const void* x, const int64_t* idx, void* out, int64_t n_idx, int64_t n_rows_out, int64_t cols,
+                   lv_stream_t stream) {
+  LV_CHECK_ARG(n_idx == 0 || (x && idx && out), "lv_row_scatter: null pointer");
+  LV_CHECK_ARG(cols > 0 && cols % 8 == 0, "lv_row_scatter: cols=%lld must be a multiple of 8", (long long)cols);
+  LV_CHECK_ARG(aligned16(x) && aligned16(out), "lv_row_scatter: pointers must be 16-byte aligned");
+  LV_CHECK_ARG(n_idx < (1ll << 31), "lv_row_scatter: too many rows");
+  if (n_idx == 0) return LV_OK;
+  row_copy_kernel<<<(unsigned)n_idx, 128, 0, (cudaStream_t)stream>>>(BF(x), nullptr, idx, BFM(out), n_idx, cols, n_idx,
+                                                                    n_rows_out);
+  LV_CHECK_LAUNCH("row_copy_kernel(scatter)");
+  return LV_OK;
+}
+
 int lv_attn_decode_merge(const void* o_part, const float* lse_part, void* out, float* lse_out, int64_t n_splits,
                          int64_t group, int64_t hkv, int64_t d, lv_stream_t stream) {
   LV_CHECK_ARG(o_part && lse_part && out, "lv_attn_decode_merge: null pointer");

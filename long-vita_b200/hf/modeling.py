@@ -146,6 +146,33 @@ def row_chunks(T: int) -> List[Tuple[int, int]]:
     return spans
 
 
+# Streamed decoder layer.  Above STREAM_THRESHOLD rows, when the attention step is plain causal attention over this
+# forward's rows, a layer runs everything, attention included, span by span in row order: rows [r0, r1) attend only
+# to keys [0, r1), which are written by then.  Only x and one K|V buffer (shared by the layers of a forward) span the
+# sequence: 14 848 B per token with the RoPE tables at the 14B geometry, against 35 328 for the row-chunked layer.
+# The threshold lies between the 1M bench prompt (1 058 816 rows, row-chunked) and the ~1.33 M rows where the
+# row-chunked layer runs out of memory on one 80 GB H100.
+#
+# Streaming is bit-identical to the whole call.  The QKV GEMM runs as two launches over row slices of the weight (Q
+# columns, then K|V columns); with no split-K each output element keeps its k-order.  A query chunk over its key
+# prefix is lv_attn_fwd with sq < sk, its mask aligned to the last key: its first row sits at global position r0, a
+# multiple of 128, so every 128-row query item and every key tile is the one of the whole call.
+STREAM_THRESHOLD = 1_179_648
+
+
+def query_chunked(attend) -> bool:
+    """Whether the attention step `attend` (bare or under functools.partial) declares `query_chunks`: it may be called
+    with the query rows [r0, r1) over the keys [0, r1) and then returns exactly those rows of the whole call."""
+    while isinstance(attend, partial):
+        attend = attend.func
+    return bool(getattr(attend, "query_chunks", False))
+
+
+def streams(T: int, attend) -> bool:
+    """Whether a decoder layer of T rows with the attention step `attend` runs streamed (STREAM_THRESHOLD)."""
+    return T > STREAM_THRESHOLD and query_chunked(attend)
+
+
 class DecoderLayer:
     """Qwen2 decoder layer (transformers Qwen2DecoderLayer, instantiated by the reference at
     modeling_long_vita.py:57-72; mcore twin transformer_layer.py:173-257) with fused QKV and fused
@@ -167,7 +194,8 @@ class DecoderLayer:
 
     def forward(self, x: torch.Tensor, delta: Optional[torch.Tensor], cos, sin, attend,
                 qkv_out: Optional[torch.Tensor] = None,
-                inplace: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+                inplace: bool = False,
+                kv_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
         """x [T, H] residual stream, `delta` the previous layer's MLP output not yet added (the add is fused into this
         layer's first RMSNorm), or None.  Returns (x, delta).
 
@@ -179,10 +207,19 @@ class DecoderLayer:
         Above ROW_CHUNK_THRESHOLD rows the ops before and after attention run chunk by chunk (row_chunks); attention
         is still one call over all rows, enqueued after every QKV row is written.  Each chunk's MLP output is then
         added to its rows of x at once and the returned delta is None.  With several chunks and `inplace`, x itself
-        is that residual stream (its rows are overwritten); otherwise the layer writes a new one."""
+        is that residual stream (its rows are overwritten); otherwise the layer writes a new one.
+
+        Above STREAM_THRESHOLD rows, with an attention step that declares `query_chunks` (query_chunked), the layer
+        streams: every op, attention included, runs span by span, each span's queries over the keys up to its last
+        row.  K|V rows go to `kv_out` [T, 2 hkv d] (allocated here if None), and x and delta as above."""
         cfg = self.cfg
         T = x.shape[0]
         spans = row_chunks(T)
+        if streams(T, attend):
+            if qkv_out is not None:
+                raise ValueError("DecoderLayer.forward: a streamed layer writes Q per span and K|V to kv_out; it takes "
+                                 "no qkv_out")
+            return self._forward_streamed(x, delta, cos, sin, attend, kv_out, spans, inplace)
         if len(spans) > 1:
             return self._forward_chunked(x, delta, cos, sin, attend, qkv_out, spans, inplace)
         hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
@@ -233,6 +270,37 @@ class DecoderLayer:
             ops.ls_residual(xo[r0:r1], m, out=xo[r0:r1])      # the add the next layer's first RMSNorm would fuse
         return xo, None
 
+    def _forward_streamed(self, x, delta, cos, sin, attend, kv, spans, inplace):
+        """forward() with every op on the row spans `spans` in order (STREAM_THRESHOLD): Q of a span in a span buffer,
+        its K|V rows into `kv`, attention of the span's queries over kv[:r1]; returns (x with this layer's MLP output
+        added, None).  A span reads no row of x but its own, so x may be the residual stream it writes."""
+        cfg = self.cfg
+        T = x.shape[0]
+        hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+        eps = cfg.rms_norm_eps
+        nq = hq * d
+        if kv is None:
+            kv = torch.empty((T, 2 * hkv * d), dtype=x.dtype, device=x.device)
+        k = kv[:, : hkv * d].view(T, hkv, d)
+        v = kv[:, hkv * d :].view(T, hkv, d)
+        xo = x if inplace else torch.empty_like(x)
+        for r0, r1 in spans:
+            n = r1 - r0
+            if delta is None:
+                h, res = ops.rmsnorm(x[r0:r1], self.ln1, eps), x[r0:r1]
+            else:
+                h, res = ops.rmsnorm(delta[r0:r1], self.ln1, eps, residual=x[r0:r1], out=xo[r0:r1])
+            q = ops.linear(h, self.wqkv[:nq], self.bqkv[:nq]).view(n, hq, d)
+            ops.linear(h, self.wqkv[nq:], self.bqkv[nq:], out=kv[r0:r1])
+            if cos is not None:
+                ops.rope(q, cos[r0:r1], sin[r0:r1], out=q)
+                ops.rope(k[r0:r1], cos[r0:r1], sin[r0:r1], out=k[r0:r1])
+            o = attend(q, k[:r1], v[:r1]).reshape(n, nq)
+            h, _ = ops.rmsnorm(ops.linear(o, self.wo), self.ln2, eps, residual=res, out=xo[r0:r1])
+            m = ops.linear(ops.linear(h, self.w_gate_up, act="swiglu"), self.w_down)
+            ops.ls_residual(xo[r0:r1], m, out=xo[r0:r1])
+        return xo, None
+
 
 def run_layers(layers, x: torch.Tensor, cos, sin, attend, norm_w: torch.Tensor, eps: float, *, cache=None,
                qkv_out=None, hidden: Optional[list] = None, donate: bool = False) -> torch.Tensor:
@@ -243,15 +311,27 @@ def run_layers(layers, x: torch.Tensor, cos, sin, attend, norm_w: torch.Tensor, 
     attention step (DecoderLayer.forward); `qkv_out()`, if given, the QKV GEMM's output buffer of the next layer.  The
     K/V rows appended to `cache` during the pass are committed at its end.  `hidden` (a list) receives each layer's
     input hidden state.  `donate`: x was made for this call (an embedding output), so chunked layers may update it in
-    place; the stack's own residual stream is updated in place from the second layer on (unless `hidden` keeps it)."""
+    place; the stack's own residual stream is updated in place from the second layer on (unless `hidden` keeps it).
+    Streamed layers (STREAM_THRESHOLD) share one K|V buffer, allocated here."""
     delta = None
+    kv = None
+    if layers and streams(x.shape[0], attend):
+        c = layers[0].cfg
+        kv = torch.empty((x.shape[0], 2 * c.num_key_value_heads * c.head_dim), dtype=x.dtype, device=x.device)
     for li, layer in enumerate(layers):
         if hidden is not None:
             hidden.append(x if delta is None else x + delta)
         x, delta = layer.forward(x, delta, cos, sin, partial(attend, li), None if qkv_out is None else qkv_out(),
-                                 inplace=(donate or li > 0) and hidden is None)
+                                 inplace=(donate or li > 0) and hidden is None, kv_out=kv)
     if cache is not None:
         cache.commit()
+    if kv is not None:
+        # streamed: x is the stack's own residual stream (the layers replaced or donated it); the final norm writes it
+        # span by span, so that no second [T, H] tensor exists beside it
+        del kv
+        for r0, r1 in row_chunks(x.shape[0]):
+            x[r0:r1].copy_(ops.rmsnorm(x[r0:r1], norm_w, eps))
+        return x
     if delta is None:
         return ops.rmsnorm(x, norm_w, eps)
     return ops.rmsnorm(delta, norm_w, eps, residual=x)[0]
@@ -261,10 +341,17 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None):
     """The single-GPU attention step for run_layers.  Without `cache`: causal attention over this forward's rows
     (inside each packed document with `cu_seqlens`).  With `cache`: the new K/V rows are appended to it and one new
     token attends over the whole cache (flash-decoding), several new tokens over cache + new rows with the causal mask
-    aligned to the last key (the first prefill, or a chunk)."""
+    aligned to the last key (the first prefill, or a chunk).
+
+    The plain step (no cache, one sample) declares `query_chunks` (query_chunked): called with query rows [r0, r1)
+    and the keys [0, r1), its mask aligned to the last key gives exactly those rows of the whole call."""
     kw = ops.docs_kwargs(cu_seqlens)
     if cache is None:
-        return lambda li, q, k, v: ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True, **kw)
+        def attend(li, q, k, v):
+            return ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True, **kw)
+
+        attend.query_chunks = cu_seqlens is None
+        return attend
 
     def attend(li, q, k, v):
         kc, vc, length = cache.append(li, k, v)
@@ -311,6 +398,22 @@ def encode_images(vision_model, projection, images: torch.Tensor, chunk: int = V
     for i in range(0, images.shape[0], chunk):
         feats.append(projection(vision_model(images[i : i + chunk]), has_cls=True))
     return feats[0] if len(feats) == 1 else torch.cat(feats, dim=0)
+
+
+def scatter_images(x: torch.Tensor, vision_model, projection, images: torch.Tensor, dst: torch.Tensor,
+                   chunk: int = VISION_CHUNK) -> torch.Tensor:
+    """Writes the projected features of `images` into the rows `dst` of the embedded prompt x [T, H] (image-major:
+    each image's tokens_per_image rows in turn) and returns x.  Each `chunk` frames' features are scattered as soon
+    as they are made, so the whole-prompt feature tensor of encode_images never exists (21.5 GB at 8192 frames).
+    For unique `dst` the result is bit-identical to ops.embed_scatter with encode_images' features."""
+    n = images.shape[0]
+    if n == 0 or dst.numel() % n:
+        raise ValueError(f"scatter_images: {dst.numel()} target rows for {n} images")
+    tpi = dst.numel() // n
+    for i in range(0, n, chunk):
+        feat = projection(vision_model(images[i : i + chunk]), has_cls=True)
+        ops.row_scatter(feat, dst[i * tpi : (i + feat.shape[0]) * tpi], x)
+    return x
 
 
 def _map_tensors(obj, fn, seen=None):
@@ -396,46 +499,59 @@ class LongVITAModel(_WeightHolderModule):
             raise NotImplementedError("padding masks are not supported; pass unpadded sequences (batch 1)")
 
         past_len = 0 if past_key_values is None else past_key_values.get_seq_length()
-        image_embeds = None
-        if images is not None and past_len == 0:                  # modeling_long_vita.py:90
-            image_embeds = self.encode_images(images)
-            assert image_embeds.shape[0] == len(images)
-
         if inputs_embeds is None:
             b, s = input_ids.shape
             if b != 1:
                 raise NotImplementedError("batch size 1 (the reference's long-context configuration)")
-            if image_embeds is not None:
-                idx_b, idx_s = image_indices.to(input_ids.device).unbind(dim=0)
-                dst = (idx_b.reshape(-1) * s + idx_s.reshape(-1)).to(torch.int64)
-                x = ops.embed_scatter(input_ids, self.embed_tokens, image_embeds, dst)
-                image_embeds = None                 # scattered into x: not held through the decoder
-            else:
-                x = ops.embed_scatter(input_ids, self.embed_tokens)
+            dev = self.embed_tokens.device
         else:
             b, s, _ = inputs_embeds.shape
             if b != 1:
                 raise NotImplementedError("batch size 1")
-            x = inputs_embeds.reshape(s, -1).contiguous()
+            dev = inputs_embeds.device
 
         cache = past_key_values
         if use_cache and cache is None:
             capacity = int(flash_attn_kwargs.pop("max_cache_len", 0)) or s + self.default_new_tokens
-            cache = KVCache(len(self.layers), capacity, cfg.num_key_value_heads, cfg.head_dim, x.device)
+            cache = KVCache(len(self.layers), capacity, cfg.num_key_value_heads, cfg.head_dim, dev)
         flash_attn_kwargs.pop("max_cache_len", None)
         if cache_position is None:
-            cache_position = torch.arange(past_len, past_len + s, device=x.device)     # modeling_long_vita.py:153-158
+            cache_position = torch.arange(past_len, past_len + s, device=dev)     # modeling_long_vita.py:153-158
         cu = None
         if position_ids is None:
             position_ids = cache_position.unsqueeze(0)
         else:
             # packed samples: positions restarting at 0 inside the row are sample boundaries; attention stays inside
             # each sample, as transformers' flash_attention_2 does for the reference (tools/inference_long_vita.py:816)
-            cu = packed_rows(position_ids, s, x.device, cache=cache)
+            cu = packed_rows(position_ids, s, dev, cache=cache)
+        attend = attention_step(cache, cu)
+
+        encode = images is not None and past_len == 0              # modeling_long_vita.py:90
+        # when the decoder streams, so does the vision phase: each ViT chunk's features go into x as they are made
+        stream_images = encode and inputs_embeds is None and streams(s, attend)
+        image_embeds = None
+        if encode and not stream_images:
+            image_embeds = self.encode_images(images)
+            assert image_embeds.shape[0] == len(images)
+
+        if inputs_embeds is None:
+            if encode:
+                idx_b, idx_s = image_indices.to(input_ids.device).unbind(dim=0)
+                dst = (idx_b.reshape(-1) * s + idx_s.reshape(-1)).to(torch.int64)
+                if stream_images:
+                    x = scatter_images(ops.embed_scatter(input_ids, self.embed_tokens), self.vision_model,
+                                       self.vision_projection, images, dst, self.vision_chunk)
+                else:
+                    x = ops.embed_scatter(input_ids, self.embed_tokens, image_embeds, dst)
+                image_embeds = None                 # scattered into x: not held through the decoder
+            else:
+                x = ops.embed_scatter(input_ids, self.embed_tokens)
+        else:
+            x = inputs_embeds.reshape(s, -1).contiguous()
         cos, sin = ops.rope_table(position_ids.reshape(-1).to(torch.int64), self.inv_freq)
 
         hidden = [] if output_hidden_states else None
-        h = run_layers(self.layers, x, cos, sin, attention_step(cache, cu), self.norm_w, cfg.rms_norm_eps, cache=cache,
+        h = run_layers(self.layers, x, cos, sin, attend, self.norm_w, cfg.rms_norm_eps, cache=cache,
                        hidden=hidden, donate=inputs_embeds is None).view(1, s, -1)
         all_hidden = tuple(t.view(1, s, -1) for t in hidden) + (h,) if output_hidden_states else None
         out = BaseOutput(last_hidden_state=h, past_key_values=cache, hidden_states=all_hidden)

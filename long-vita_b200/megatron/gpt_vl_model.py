@@ -40,6 +40,7 @@ import torch
 from .. import ops
 from ..config import LongVITAConfig
 from ..cp import exchange_attention
+from ..hf import modeling
 from ..hf.modeling import (VISION_CHUNK, DecoderLayer, attention_step, encode_images, packed_rows, rope_inv_freq,
                            run_layers, vision_tower)
 from .checkpoint import mcore_to_hf
@@ -75,6 +76,12 @@ class B200GPTVLModel:
     def external_feature_model(self, images: torch.Tensor, **_unused) -> torch.Tensor:
         return encode_images(self.vit, self.vision_projection, images, self.vision_chunk)
 
+    @staticmethod
+    def _indices_dst(indices: torch.Tensor, s: int, dev) -> torch.Tensor:
+        """The flat rows of `indices` mode ([2, n, tokens]: batch, position) in a row of s tokens."""
+        idx_b, idx_s = indices.to(dev).unbind(dim=0)
+        return (idx_b.reshape(-1) * s + idx_s.reshape(-1)).to(torch.int64)
+
     # -- LanguageModelEmbedding.forward (language_model_embedding.py:91-134) -> [s, h] --------------
     def embedding(self, input_ids: torch.Tensor, position_ids, external_feature_dict: Optional[dict] = None):
         b, s = input_ids.shape
@@ -90,9 +97,7 @@ class B200GPTVLModel:
         feat = d["features"]
         dev = input_ids.device
         if "indices" in d:
-            idx_b, idx_s = d["indices"].to(dev).unbind(dim=0)
-            dst = (idx_b.reshape(-1) * s + idx_s.reshape(-1)).to(torch.int64)
-            return ops.embed_scatter(input_ids, self.word_embeddings, feat, dst)
+            return ops.embed_scatter(input_ids, self.word_embeddings, feat, self._indices_dst(d["indices"], s, dev))
         if "pre_len" in d:
             if feat.shape[0] != 1:
                 raise NotImplementedError("pre_len mode broadcasts one feature block per batch row; batch is 1")
@@ -129,28 +134,18 @@ class B200GPTVLModel:
             raise NotImplementedError(f"extra_block_kwargs {sorted(extra_block_kwargs)} are not supported")
         if decoder_input is not None:
             s, b, _ = decoder_input.shape
-            if b != 1:
-                raise NotImplementedError("micro-batch 1")
-            x = decoder_input.reshape(s, -1).contiguous()
         else:
+            b, s = input_ids.shape
             if (getattr(inference_params, "external_inputs", None) is not None
                     and not getattr(inference_params, "key_value_memory_dict", None)):
                 external_inputs = inference_params.external_inputs
-            if external_inputs:
-                feat = self.external_feature_model(**external_inputs)
-                efd = {"features": feat}
-                for key in external_inputs:
-                    if "indices" in key or key == "pre_len":
-                        efd[key] = external_inputs[key]
-                x = self.embedding(input_ids, position_ids, efd)
-                feat = efd = None                   # scattered into x: not held through the decoder
-            else:
-                x = self.embedding(input_ids, position_ids)
-            s = x.shape[0]
+        if b != 1:
+            raise NotImplementedError("micro-batch 1 (the reference's long-context setting)")
         if getattr(inference_params, "logit_mask", None) is not None:
             logit_mask = inference_params.logit_mask
         if hasattr(inference_params, "use_kv_cache") and not inference_params.use_kv_cache:
             inference_params = None
+        dev = self.word_embeddings.device if decoder_input is None else decoder_input.device
         # Megatron's incremental decoding protocol (`--use-kv-cache`, generation.py:127-131): the caller passes only
         # the new tokens and their positions; per-layer K/V live in `inference_params.key_value_memory_dict`.  Here
         # that dict holds one pre-allocated kv_cache.KVCache for the whole model.
@@ -165,7 +160,7 @@ class B200GPTVLModel:
             cache = kv.get("b200_kv_cache")
             if cache is None:
                 capacity = int(getattr(inference_params, "max_sequence_length", 0) or (s + 1024))
-                cache = KVCache(len(self.layers), capacity, cfg.num_key_value_heads, cfg.head_dim, x.device)
+                cache = KVCache(len(self.layers), capacity, cfg.num_key_value_heads, cfg.head_dim, dev)
                 kv["b200_kv_cache"] = cache
 
         # RoPE: Megatron builds the table for positions 0..S-1 and slices it zig-zag under CP
@@ -175,17 +170,37 @@ class B200GPTVLModel:
         if position_ids is None:
             assert self.cp is None, "context parallelism needs this rank's position_ids"
             p0 = 0 if cache is None else len(cache)
-            position_ids = torch.arange(p0, p0 + s, device=x.device).unsqueeze(0)
+            position_ids = torch.arange(p0, p0 + s, device=dev).unsqueeze(0)
         else:
-            cu = packed_rows(position_ids, s, x.device, cache=cache, cp=self.cp)
+            cu = packed_rows(position_ids, s, dev, cache=cache, cp=self.cp)
+        attend = attention_step(cache, cu) if self.cp is None else exchange_attention(self.cp)
+
+        if decoder_input is not None:
+            x = decoder_input.reshape(s, -1).contiguous()
+        else:
+            external_inputs = external_inputs or {}
+            modes = [key for key in external_inputs if "indices" in key or key == "pre_len"]
+            if modes == ["indices"] and modeling.streams(s, attend):
+                # the decoder streams (hf.modeling.STREAM_THRESHOLD): so does the vision phase, each ViT chunk's
+                # features going into x as soon as they are made
+                x = self.embedding(input_ids, position_ids)
+                dst = self._indices_dst(external_inputs["indices"], s, dev)
+                x = modeling.scatter_images(x, self.vit, self.vision_projection, external_inputs["images"], dst,
+                                            self.vision_chunk)
+            elif external_inputs:
+                feat = self.external_feature_model(**external_inputs)
+                efd = {"features": feat}
+                for key in external_inputs:
+                    if "indices" in key or key == "pre_len":
+                        efd[key] = external_inputs[key]
+                x = self.embedding(input_ids, position_ids, efd)
+                feat = efd = None                   # scattered into x: not held through the decoder
+            else:
+                x = self.embedding(input_ids, position_ids)
         cos, sin = ops.rope_table(position_ids.reshape(-1).to(torch.int64), self.inv_freq)
 
-        if self.cp is None:
-            h = run_layers(self.layers, x, cos, sin, attention_step(cache, cu), self.final_layernorm, cfg.rms_norm_eps,
-                           cache=cache, donate=decoder_input is None)
-        else:
-            h = run_layers(self.layers, x, cos, sin, exchange_attention(self.cp), self.final_layernorm,
-                           cfg.rms_norm_eps, qkv_out=self.cp.qkv_buffer, donate=decoder_input is None)
+        h = run_layers(self.layers, x, cos, sin, attend, self.final_layernorm, cfg.rms_norm_eps, cache=cache,
+                       qkv_out=None if self.cp is None else self.cp.qkv_buffer, donate=decoder_input is None)
         hidden_states = h.view(s, 1, -1)
 
         # training tail, fused: masked row gather -> LM head -> per-token cross-entropy, chunked over the vocabulary so

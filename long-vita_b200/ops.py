@@ -303,6 +303,9 @@ def attention_fwd(
             fl = _docs_flops(host, hq, d)
         elif causal and q_seg_len is None and sq == sk:
             fl = 4.0 * b * hq * d * (sq * (sq + 1) / 2)
+        elif causal and q_seg_len is None and q_seg_pos is None and not kv_pos0 and sq < sk:
+            # one query segment aligned to the last key (a query chunk over its key prefix): the visible pairs
+            fl = 4.0 * b * hq * d * (sq * (sk - sq) + sq * (sq + 1) / 2)
         else:
             fl = 4.0 * b * hq * d * sq * sk  # upper bound for masked / segmented calls
         _TIMER.stop("attn_fwd", fl, ev0)
@@ -590,6 +593,18 @@ def row_scatter_zero(x: torch.Tensor, idx: torch.Tensor, n_rows_out: int):
     idx = _vec("row_scatter_zero", "idx", idx, torch.int64)
     out = torch.empty((n_rows_out, x.shape[1]), dtype=torch.bfloat16, device=x.device)
     _call("lv_row_scatter_zero", x.data_ptr(), idx.data_ptr(), out.data_ptr(), idx.numel(), n_rows_out, x.shape[1])
+    return out
+
+
+def row_scatter(x: torch.Tensor, idx: torch.Tensor, out: torch.Tensor):
+    """out[idx[i]] = x[i] in place, every other row of out untouched: x [n, cols], idx n int64 row indices, out a
+    contiguous [rows, cols].  Returns out."""
+    _need_cuda_bf16(x, out)
+    if out.dim() != 2 or not out.is_contiguous():
+        raise ValueError(f"row_scatter: out {tuple(out.shape)} must be a contiguous row matrix")
+    x = _rows(x, out.shape[1])
+    idx = _vec("row_scatter", "idx", idx, torch.int64, x.shape[0])
+    _call("lv_row_scatter", x.data_ptr(), idx.data_ptr(), out.data_ptr(), idx.numel(), out.shape[0], out.shape[1])
     return out
 
 
