@@ -304,6 +304,28 @@ int lv_pixel_shuffle_bwd(const void* dout, void* dx, int64_t n, int64_t hw, int6
 int lv_attn_decode_merge(const void* o_part, const float* lse_part, void* out, float* lse_out, int64_t n_splits,
                          int64_t group, int64_t hkv, int64_t d, lv_stream_t stream);
 
+/* Flash-decoding of one query token over K/V rows in pinned host memory (the host tier of the K/V cache, for
+ * prompts whose cache does not fit in HBM).  q bf16 [hq, d] on the device; kv_host bf16 [capacity, 2 * hkv * d],
+ * token-major, row = K of the hkv heads then V of the hkv heads, allocated pinned and mapped (lv_host_alloc); the
+ * kernel reads rows [0, length) in place over PCIe, never a row at or past `length`.  Split s of n_splits takes
+ * the rows [s * per, min((s + 1) * per, length)), per = ceil(length / n_splits), and writes o_part bf16
+ * [n_splits, G, hkv, d] and lse_part float [n_splits, hkv, G] (G = hq / hkv, natural log, -inf for an empty
+ * split): the inputs of lv_attn_decode_merge.  d = 128 only; hkv must divide 16 and G be at most 8.  kv_host is
+ * checked to be pinned host memory (cudaPointerGetAttributes) before anything launches. */
+int lv_attn_decode_host(const void* q, const void* kv_host, void* o_part, float* lse_part, int64_t length,
+                        int64_t capacity, int64_t hq, int64_t hkv, int64_t d, int64_t n_splits, float scale,
+                        lv_stream_t stream);
+/* Pinned host memory mapped into the device address space (cudaHostAlloc, mapped | portable), and its release.
+ * The host tier's buffers come from here: an exact size, where a caching pinned allocator may round a
+ * multi-gigabyte buffer up to the next power of two. */
+int lv_host_alloc(int64_t bytes, void** ptr);
+int lv_host_free(void* ptr);
+/* Copy `rows` rows of row_bytes from device memory (src_pitch bytes apart) to contiguous pinned host rows, in
+ * stream order (one cudaMemcpy2DAsync): the K|V columns of a QKV buffer go to the host tier without a device
+ * temporary.  host_dst must be pinned host memory. */
+int lv_rows_to_host(void* host_dst, const void* src, int64_t rows, int64_t row_bytes, int64_t src_pitch,
+                    lv_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Dense linears (tensor-core roofline).  C[M,N] = act(A[M,K] . W[N,K]^T + bias[N]), bf16 in,
  * fp32 accumulate, bf16 out.  Replaces torch.matmul / te.Linear at layers.py:270,409, the ViT

@@ -9,7 +9,9 @@ All arithmetic runs in liblvb200.so (long_vita_b200.ops); PyTorch holds the buff
 `use_cache=True` returns a `kv_cache.KVCache` in `past_key_values` (pre-allocated, post-RoPE rows); a
 later call with that cache and the new token(s) runs incremental decoding: one token -> the
 flash-decoding composition `ops.attention_decode`, several tokens -> the fused kernel with the
-bottom-right-aligned causal mask over cache + new rows (chunked prefill).  Images are encoded only when
+bottom-right-aligned causal mask over cache + new rows (chunked prefill).  A cache that does not fit in HBM beside
+the prefill (a ~1M-token prompt) is a `kv_cache.OffloadedKVCache` whose trailing layers live in pinned host memory
+and are decoded in place (`ops.attention_decode_host`); see new_cache.  Images are encoded only when
 the cache is empty (modeling_long_vita.py:90).  The Megatron serving path of the reference re-prefills
 every token (long_vita_megatron/inference/text_generation/generation.py:127-135); SURVEY.md 8f-2.
 """
@@ -21,9 +23,9 @@ from typing import Dict, Iterable, List, Optional, Tuple
 
 import torch
 
-from .. import ops
+from .. import kv_cache, ops
 from ..config import LongVITAConfig
-from ..kv_cache import KVCache
+from ..kv_cache import KVCache, OffloadedKVCache
 
 
 @dataclass
@@ -337,20 +339,69 @@ def run_layers(layers, x: torch.Tensor, cos, sin, attend, norm_w: torch.Tensor, 
     return ops.rmsnorm(delta, norm_w, eps, residual=x)[0]
 
 
-def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None):
+def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool) -> int:
+    """Device bytes per token that a decoder prefill of T rows holds beside the weights (DESIGN §3): whole-tensor
+    layer (x, delta, QKV, attention output, new x, norm output, SwiGLU output, MLP output), row-chunked layer (x, QKV,
+    attention output) or streamed layer (x, K|V), plus the RoPE tables.  At the 14B geometry: 103 936, 35 328 and
+    14 848 B."""
+    H, I = cfg.hidden_size, cfg.intermediate_size
+    hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
+    rope = 2 * 2 * d
+    if streamed:
+        return 2 * (H + 2 * hkv * d) + rope
+    if len(row_chunks(T)) > 1:
+        return 2 * (H + (hq + 2 * hkv) * d + hq * d) + rope
+    return 2 * (5 * H + hq * d + (hq + 2 * hkv) * d + I) + rope
+
+
+def new_cache(cfg: LongVITAConfig, num_layers: int, capacity: int, rows: int, device):
+    """The K/V cache of a generation whose prompt has `rows` tokens (kv_cache.make_cache): on the device when it fits
+    beside that prompt's prefill, else partly in pinned host memory, in which case the prefill streams above
+    STREAM_THRESHOLD (attention_step)."""
+    return kv_cache.make_cache(num_layers, capacity, cfg.num_key_value_heads, cfg.head_dim, device,
+                               prefill_bytes=rows * prefill_bytes_per_token(cfg, rows, False),
+                               offloaded_prefill_bytes=rows * prefill_bytes_per_token(cfg, rows,
+                                                                                      rows > STREAM_THRESHOLD))
+
+
+def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: int = 1):
     """The single-GPU attention step for run_layers.  Without `cache`: causal attention over this forward's rows
     (inside each packed document with `cu_seqlens`).  With `cache`: the new K/V rows are appended to it and one new
     token attends over the whole cache (flash-decoding), several new tokens over cache + new rows with the causal mask
     aligned to the last key (the first prefill, or a chunk).
 
-    The plain step (no cache, one sample) declares `query_chunks` (query_chunked): called with query rows [r0, r1)
-    and the keys [0, r1), its mask aligned to the last key gives exactly those rows of the whole call."""
+    With a kv_cache.OffloadedKVCache, a layer on the host tier copies its new rows to its host buffer; in the prefill
+    it then attends over its own k, v exactly as the step without a cache does, and a new token attends over the
+    host rows in place (ops.attention_decode_host).  `rows` is the number of new tokens of the forward; a cache that
+    cannot take them raises before anything is launched.
+
+    The plain step (no cache, one sample) and the prefill step of an empty offloaded cache declare `query_chunks`
+    (query_chunked): called with query rows [r0, r1) and the keys [0, r1), its mask aligned to the last key gives
+    exactly those rows of the whole call."""
     kw = ops.docs_kwargs(cu_seqlens)
     if cache is None:
         def attend(li, q, k, v):
             return ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True, **kw)
 
         attend.query_chunks = cu_seqlens is None
+        return attend
+
+    if isinstance(cache, OffloadedKVCache):
+        cache.check_rows(rows)
+
+        def attend(li, q, k, v):
+            n = q.shape[0]
+            if cache.on_host(li):
+                kh, length = cache.append_host(li, k, v, n)
+                if n == 1:
+                    return ops.attention_decode_host(q[0], kh, length)
+                return ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True)
+            kc, vc, length = cache.append(li, k, v, n)
+            if n == 1:
+                return ops.attention_decode(q[0], kc, vc, length)
+            return ops.attention_fwd(q.unsqueeze(0), kc[:length].unsqueeze(0), vc[:length].unsqueeze(0), causal=True)
+
+        attend.query_chunks = len(cache) == 0
         return attend
 
     def attend(li, q, k, v):
@@ -489,7 +540,7 @@ class LongVITAModel(_WeightHolderModule):
         cfg = self.config
         if (input_ids is None) ^ (inputs_embeds is not None):
             raise ValueError("You must specify exactly one of input_ids or inputs_embeds")
-        if past_key_values is not None and not isinstance(past_key_values, KVCache):
+        if past_key_values is not None and not isinstance(past_key_values, (KVCache, OffloadedKVCache)):
             if len(past_key_values) != 0:
                 raise NotImplementedError("past_key_values must be the KVCache returned by a use_cache=True call")
             past_key_values = None
@@ -513,7 +564,7 @@ class LongVITAModel(_WeightHolderModule):
         cache = past_key_values
         if use_cache and cache is None:
             capacity = int(flash_attn_kwargs.pop("max_cache_len", 0)) or s + self.default_new_tokens
-            cache = KVCache(len(self.layers), capacity, cfg.num_key_value_heads, cfg.head_dim, dev)
+            cache = new_cache(cfg, len(self.layers), capacity, s, dev)
         flash_attn_kwargs.pop("max_cache_len", None)
         if cache_position is None:
             cache_position = torch.arange(past_len, past_len + s, device=dev)     # modeling_long_vita.py:153-158
@@ -524,7 +575,7 @@ class LongVITAModel(_WeightHolderModule):
             # packed samples: positions restarting at 0 inside the row are sample boundaries; attention stays inside
             # each sample, as transformers' flash_attention_2 does for the reference (tools/inference_long_vita.py:816)
             cu = packed_rows(position_ids, s, dev, cache=cache)
-        attend = attention_step(cache, cu)
+        attend = attention_step(cache, cu, s)
 
         encode = images is not None and past_len == 0              # modeling_long_vita.py:90
         # when the decoder streams, so does the vision phase: each ViT chunk's features go into x as they are made

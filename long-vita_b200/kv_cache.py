@@ -10,12 +10,18 @@ once (`ops.attention_decode`).
 
 Duck-types the part of transformers' `Cache` the reference touches: `len(cache)` (`modeling_long_vita.py:90`)
 and `get_seq_length()` (:154).
+
+A cache that does not fit in HBM beside the prefill is an `OffloadedKVCache`: its leading layers are the device
+buffers above, the others one pinned host buffer each, read in place by the decode kernel (`ops.attention_decode_host`).
+`make_cache` decides which, once, from the free device memory (`device_layers`).
 """
 from __future__ import annotations
 
-from typing import List, Tuple
+from typing import List, Optional, Tuple
 
 import torch
+
+from . import ops
 
 
 class KVCache:
@@ -53,3 +59,121 @@ class KVCache:
 
     def bytes(self) -> int:
         return sum(t.numel() * t.element_size() for t in self.k + self.v)
+
+
+# Device memory a forward with a K/V cache leaves free beside the cache and the prefill's per-token working set: the
+# vision phase's activations, the logits, RoPE and index tensors, the caching allocator's slack.
+KV_RESERVE = 4 << 30
+
+
+def device_free_bytes(device) -> Optional[int]:
+    """Device memory a new cache may take on `device`: free memory plus what PyTorch's allocator holds unused; None
+    for a device without a memory budget (a CPU tensor cache)."""
+    device = torch.device(device)
+    if device.type != "cuda":
+        return None
+    free, _ = torch.cuda.mem_get_info(device)
+    return free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device)
+
+
+def device_layers(free_bytes: Optional[int], capacity: int, num_layers: int, kv_row_bytes: int, prefill_bytes: int,
+                  offloaded_prefill_bytes: int, reserve: int = KV_RESERVE) -> int:
+    """How many leading layers of a cache of `capacity` rows (`kv_row_bytes` of K and V per row and layer) stay on
+    the device.  `num_layers` - the plain KVCache - when the whole cache, the prefill's device working set
+    `prefill_bytes` and `reserve` fit in `free_bytes` (None: no budget); otherwise as many as fit beside the working
+    set of the prefill with the cache offloaded, `offloaded_prefill_bytes`, and at most num_layers - 1."""
+    layer = capacity * kv_row_bytes
+    if free_bytes is None or num_layers * layer + prefill_bytes + reserve <= free_bytes:
+        return num_layers
+    return int(max(0, min(num_layers - 1, (free_bytes - offloaded_prefill_bytes - reserve) // layer)))
+
+
+def make_cache(num_layers: int, capacity: int, num_kv_heads: int, head_dim: int, device, *, prefill_bytes: int,
+               offloaded_prefill_bytes: int, dtype=torch.bfloat16):
+    """The K/V cache of a generation: a KVCache when it fits on the device (device_layers), else an OffloadedKVCache
+    with as many device layers as fit.  Every buffer, host ones included, is allocated here, before the prefill."""
+    row = 2 * num_kv_heads * head_dim * torch.empty((), dtype=dtype).element_size()
+    n_dev = device_layers(device_free_bytes(device), capacity, num_layers, row, prefill_bytes, offloaded_prefill_bytes)
+    if n_dev == num_layers:
+        return KVCache(num_layers, capacity, num_kv_heads, head_dim, device, dtype)
+    return OffloadedKVCache(num_layers, n_dev, capacity, num_kv_heads, head_dim, device)
+
+
+class OffloadedKVCache:
+    """A K/V cache whose layers [0, n_dev) are [capacity, hkv, d] device buffers, as in KVCache, and whose layers
+    [n_dev, num_layers) are one pinned host buffer [capacity, 2 hkv d] bf16 each: token-major rows of K of the hkv
+    heads then V of the hkv heads, the rows of the streamed layer's K|V buffer.
+
+    The first forward fills it (it may stream: the attention step declares query_chunks while the cache is empty);
+    each later forward adds one token.  A multi-token forward on a filled cache (chunked prefill, a second turn) is
+    refused."""
+
+    def __init__(self, num_layers: int, n_dev: int, capacity: int, num_kv_heads: int, head_dim: int, device):
+        if not 0 <= n_dev < num_layers:
+            raise ValueError(f"OffloadedKVCache: {n_dev} device layers of {num_layers}")
+        self.capacity = int(capacity)
+        self.n_dev = int(n_dev)
+        shape = (self.capacity, num_kv_heads, head_dim)
+        self.k = [torch.empty(shape, dtype=torch.bfloat16, device=device) for _ in range(n_dev)]
+        self.v = [torch.empty(shape, dtype=torch.bfloat16, device=device) for _ in range(n_dev)]
+        self.host = [ops.pinned_rows(self.capacity, 2 * num_kv_heads * head_dim) for _ in range(num_layers - n_dev)]
+        self._len = 0
+        self._pending = 0
+
+    def __len__(self) -> int:
+        return self._len
+
+    def get_seq_length(self, layer_idx: int = 0) -> int:
+        return self._len
+
+    def on_host(self, layer_idx: int) -> bool:
+        return layer_idx >= self.n_dev
+
+    def check_rows(self, rows: int) -> None:
+        """Refuses a forward of `rows` new tokens that this cache cannot take (before anything is launched)."""
+        if rows > 1 and self._len:
+            raise NotImplementedError("a K/V cache partly in host memory takes one prompt and then one token per "
+                                      "forward; a multi-token call on a filled cache (chunked prefill, a second "
+                                      "turn) is not supported")
+
+    def _rows(self, k: torch.Tensor, n: Optional[int]) -> Tuple[int, int, int]:
+        """(first, end, n) of the new rows: the last n rows of k (all when None); a streamed span passes the keys up
+        to its last row, of which its own are the last."""
+        kr = k.shape[0]
+        n = kr if n is None else n
+        end = self._len + kr
+        if end > self.capacity:
+            raise RuntimeError(f"KV cache overflow: {end} tokens > capacity {self.capacity}")
+        self._pending = kr
+        return end - n, end, n
+
+    def append(self, layer_idx: int, k: torch.Tensor, v: torch.Tensor,
+               n: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor, int]:
+        """A device layer: write the last `n` rows of k / v [kr, hkv, d] at rows [len + kr - n, len + kr); returns
+        (K, V, len + kr) like KVCache.append."""
+        r0, end, n = self._rows(k, n)
+        self.k[layer_idx][r0:end].copy_(k[k.shape[0] - n :])
+        self.v[layer_idx][r0:end].copy_(v[v.shape[0] - n :])
+        return self.k[layer_idx], self.v[layer_idx], end
+
+    def append_host(self, layer_idx: int, k: torch.Tensor, v: torch.Tensor,
+                    n: Optional[int] = None) -> Tuple[torch.Tensor, int]:
+        """A host layer: the same rows, copied device-to-host in stream order (ops.kv_rows_to_host); returns (the
+        host buffer, len + kr)."""
+        r0, end, n = self._rows(k, n)
+        kr = k.shape[0]
+        host = self.host[layer_idx - self.n_dev]
+        ops.kv_rows_to_host(k[kr - n :], v[kr - n :], host[r0:end])
+        return host, end
+
+    def commit(self) -> None:
+        self._len += self._pending
+        self._pending = 0
+
+    def bytes(self) -> int:
+        """Device bytes of the cache."""
+        return sum(t.numel() * t.element_size() for t in self.k + self.v)
+
+    def host_bytes(self) -> int:
+        """Pinned host bytes of the cache."""
+        return sum(t.numel() * t.element_size() for t in self.host)

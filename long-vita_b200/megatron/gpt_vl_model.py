@@ -11,7 +11,8 @@ What is kept from the reference and what is deliberately not:
   `use_kv_cache == False -> inference_params = None` (:291-292) are honoured.  With a live `inference_params`
   (Megatron's `--use-kv-cache` protocol, generation.py:127-131: only the new tokens are passed) the K/V rows go
   to a pre-allocated `kv_cache.KVCache` kept in `inference_params.key_value_memory_dict` and a single new token
-  runs the flash-decoding path.
+  runs the flash-decoding path.  A cache that does not fit in HBM is partly in pinned host memory
+  (`hf.modeling.new_cache`, `kv_cache.OffloadedKVCache`).
 * `hidden_states += 0.0 * self.unused` (:310-311) is an exact no-op on finite values and only exists
   to keep an otherwise unused parameter in the autograd graph; not executed.
 * labels: `masked_select(labels, logit_mask)` (:389-391), the `is_instruction_dataset` shift
@@ -148,19 +149,17 @@ class B200GPTVLModel:
         dev = self.word_embeddings.device if decoder_input is None else decoder_input.device
         # Megatron's incremental decoding protocol (`--use-kv-cache`, generation.py:127-131): the caller passes only
         # the new tokens and their positions; per-layer K/V live in `inference_params.key_value_memory_dict`.  Here
-        # that dict holds one pre-allocated kv_cache.KVCache for the whole model.
+        # that dict holds one pre-allocated cache for the whole model (hf.modeling.new_cache).
         cache = None
         if inference_params is not None:
             if self.cp is not None:
                 raise NotImplementedError("KV-cache decoding under context parallelism goes through "
                                           "cp.ContextParallelRunner (sharded cache)")
-            from ..kv_cache import KVCache
-
             kv = inference_params.key_value_memory_dict
             cache = kv.get("b200_kv_cache")
             if cache is None:
                 capacity = int(getattr(inference_params, "max_sequence_length", 0) or (s + 1024))
-                cache = KVCache(len(self.layers), capacity, cfg.num_key_value_heads, cfg.head_dim, dev)
+                cache = modeling.new_cache(cfg, len(self.layers), capacity, s, dev)
                 kv["b200_kv_cache"] = cache
 
         # RoPE: Megatron builds the table for positions 0..S-1 and slices it zig-zag under CP
@@ -173,7 +172,7 @@ class B200GPTVLModel:
             position_ids = torch.arange(p0, p0 + s, device=dev).unsqueeze(0)
         else:
             cu = packed_rows(position_ids, s, dev, cache=cache, cp=self.cp)
-        attend = attention_step(cache, cu) if self.cp is None else exchange_attention(self.cp)
+        attend = attention_step(cache, cu, s) if self.cp is None else exchange_attention(self.cp)
 
         if decoder_input is not None:
             x = decoder_input.reshape(s, -1).contiguous()

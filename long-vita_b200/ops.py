@@ -11,6 +11,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import weakref
 from typing import Optional, Tuple
 
 import torch
@@ -435,6 +436,84 @@ def decode_merge(o_part: torch.Tensor, lse_part: torch.Tensor, return_lse: bool 
     lse = torch.empty((hkv * G,), dtype=torch.float32, device=o_part.device) if return_lse else None
     _call("lv_attn_decode_merge", o_part.data_ptr(), lse_part.data_ptr(), out.data_ptr(), _ptr(lse), n, G, hkv, d)
     return (out, lse) if return_lse else out
+
+
+# ------------------------------------------------------------------------------------------------
+# K/V rows in pinned host memory (the host tier of kv_cache.OffloadedKVCache)
+# ------------------------------------------------------------------------------------------------
+def _is_pinned(t: torch.Tensor) -> bool:
+    return not t.is_cuda and t.is_pinned()
+
+
+def _host_rows(op: str, name: str, t: torch.Tensor, cols: Optional[int] = None) -> None:
+    """t must be a pinned host bf16 row matrix [rows, cols] with contiguous rows (the kernel reads it by address)."""
+    if not _is_pinned(t):
+        raise ValueError(f"{op}: {name} must be pinned host memory, got {t.device}"
+                         f"{'' if t.is_cuda else ' (not pinned)'}")
+    if t.dtype != torch.bfloat16 or t.dim() != 2 or (cols is not None and t.shape[1] != cols) \
+            or t.stride() != (t.shape[1], 1):
+        want = "[rows, cols]" if cols is None else f"[rows, {cols}]"
+        raise ValueError(f"{op}: {name} must be a contiguous bfloat16 {want}, got {t.dtype} {tuple(t.shape)} "
+                         f"strides {t.stride()}")
+
+
+def pinned_rows(rows: int, cols: int) -> torch.Tensor:
+    """An uninitialised bf16 [rows, cols] tensor in pinned, device-mapped host memory of exactly that size
+    (lv_host_alloc; a caching pinned allocator rounds a buffer up to a power of two).  The memory is released when
+    the last tensor viewing it is gone."""
+    n = int(rows) * int(cols) * 2
+    p = C.c_void_p()
+    _lib.check(_lib.lib().lv_host_alloc(n, C.byref(p)), "lv_host_alloc")
+    buf = (C.c_uint8 * n).from_address(p.value)
+    weakref.finalize(buf, _lib.lib().lv_host_free, p.value).atexit = False     # the process exit releases it
+    return torch.frombuffer(buf, dtype=torch.bfloat16).view(rows, cols)
+
+
+def kv_rows_to_host(k: torch.Tensor, v: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
+    """Copy the K/V rows k / v [n, hkv, d] (device views whose V follows K in each row, as in the QKV GEMM output or
+    the streamed layer's K|V buffer) into the host rows dst [n, 2 hkv d] (pinned; row = K heads | V heads), in stream
+    order and without a device temporary: one strided copy (lv_rows_to_host).  Returns dst."""
+    _need_cuda_bf16(k, v)
+    n, hkv, d = k.shape
+    _host_rows("kv_rows_to_host", "dst", dst, 2 * hkv * d)
+    rs = k.stride(0) if n > 1 else 2 * hkv * d          # a single row's stride is arbitrary
+    if (v.shape != k.shape or not (k[0].is_contiguous() and v[0].is_contiguous()) or (n > 1 and v.stride(0) != rs)
+            or rs % 8 or rs < 2 * hkv * d or v.data_ptr() != k.data_ptr() + hkv * d * k.element_size()):
+        raise ValueError(f"kv_rows_to_host: k / v {tuple(k.shape)} strides {k.stride()} / {v.stride()} are not the "
+                         f"K and V halves of one row")
+    if dst.shape[0] != n:
+        raise ValueError(f"kv_rows_to_host: dst has {dst.shape[0]} rows for {n}")
+    _call("lv_rows_to_host", dst.data_ptr(), k.data_ptr(), n, 2 * hkv * d * 2, rs * 2)
+    return dst
+
+
+def attention_decode_host(q: torch.Tensor, kv_host: torch.Tensor, length: int, *, scale: Optional[float] = None,
+                          n_splits: Optional[int] = None, return_lse: bool = False):
+    """attention_decode over K/V rows in pinned host memory: q [hq, d] (d = 128) on the device, kv_host
+    [capacity, 2 hkv d] bf16 pinned (row = K of the hkv heads | V of the hkv heads, post-RoPE, the new token's row
+    already written); rows [0, length) are read in place over PCIe by lv_attn_decode_host, split into `n_splits`
+    contiguous key ranges (default: one per SM), and merged by lv_attn_decode_merge.  Returns out [hq, d] (and lse
+    [hq] fp32, natural log)."""
+    _need_cuda_bf16(q)
+    if q.dim() != 2:
+        raise ValueError(f"attention_decode_host: q must be [hq, d], got {tuple(q.shape)}")
+    hq, d = q.shape
+    _host_rows("attention_decode_host", "kv_host", kv_host)
+    cap, cols = kv_host.shape
+    hkv = cols // (2 * d)
+    if hkv == 0 or cols != 2 * hkv * d or hq % hkv:
+        raise ValueError(f"attention_decode_host: kv_host rows of {cols} are not K|V of kv heads of {d} for {hq} "
+                         f"query heads")
+    if not 0 < length <= cap:
+        raise ValueError(f"attention_decode_host: length {length} outside the cache (capacity {cap})")
+    if n_splits is None:
+        n_splits = max(1, min(_sm_count(q.device), -(-length // 128)))
+    G = hq // hkv
+    o = torch.empty((n_splits, G, hkv, d), dtype=torch.bfloat16, device=q.device)
+    lse = torch.empty((n_splits, hkv, G), dtype=torch.float32, device=q.device)
+    _call("lv_attn_decode_host", q.contiguous().data_ptr(), kv_host.data_ptr(), o.data_ptr(), lse.data_ptr(), length,
+          cap, hq, hkv, d, n_splits, float(scale if scale is not None else 1.0 / math.sqrt(d)))
+    return decode_merge(o, lse, return_lse=return_lse)
 
 
 # ------------------------------------------------------------------------------------------------
