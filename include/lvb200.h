@@ -326,6 +326,28 @@ int lv_host_free(void* ptr);
 int lv_rows_to_host(void* host_dst, const void* src, int64_t rows, int64_t row_bytes, int64_t src_pitch,
                     lv_stream_t stream);
 
+/* FP8 host tier (opt-in, lossy: it halves the PCIe bytes and the pinned memory of a host layer).  A row holds K of
+ * the hkv heads, e4m3 [hkv][d]; V of the hkv heads, e4m3 [hkv][d]; then the scales, float [2][hkv] (K scales, then V
+ * scales), zero-padded to a multiple of 16 bytes: 2 * hkv * d + ceil(8 * hkv / 16) * 16 bytes, 2112 at 8:128.  One
+ * head's values x are quantised in fp32: amax = max|x|, inv = 448 / amax, q = e4m3_rn_satfinite(x * inv),
+ * scale = amax / 448, read back as q * scale; a head whose inv is not finite (amax = 0, or a bf16 subnormal amax below
+ * ~1.3e-36) is zero bytes and scale 0 (csrc/kv_fp8_core.h).
+ *
+ * lv_rows_to_host_fp8: quantise `rows` bf16 K|V rows of the device (2 * hkv * d values each, V following K, src_pitch
+ * bytes apart: the K|V columns of a QKV buffer row or the streamed layer's K|V buffer) into contiguous FP8 host rows,
+ * in stream order.  The kernel stores straight into the mapped host memory with 16-byte stores: no device temporary.
+ * d = 128, hkv divides 16, src, src_pitch and host_dst 16-byte aligned; host_dst must be pinned host memory.
+ *
+ * lv_attn_decode_host_fp8: lv_attn_decode_host over FP8 rows, kv_host uint8 [capacity, row bytes] from lv_host_alloc:
+ * the same arguments, split rule (never a row at or past `length`) and outputs for lv_attn_decode_merge.  Each score
+ * is s_k * sum_i q_i k8_i and each value row enters as (p * s_v) v8, in fp32.  d = 128 only; hkv must divide 16 and
+ * G be at most 8.  kv_host is checked to be pinned host memory before anything launches. */
+int lv_rows_to_host_fp8(void* host_dst, const void* src, int64_t rows, int64_t hkv, int64_t d, int64_t src_pitch,
+                        lv_stream_t stream);
+int lv_attn_decode_host_fp8(const void* q, const void* kv_host, void* o_part, float* lse_part, int64_t length,
+                            int64_t capacity, int64_t hq, int64_t hkv, int64_t d, int64_t n_splits, float scale,
+                            lv_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Dense linears (tensor-core roofline).  C[M,N] = act(A[M,K] . W[N,K]^T + bias[N]), bf16 in,
  * fp32 accumulate, bf16 out.  Replaces torch.matmul / te.Linear at layers.py:270,409, the ViT

@@ -354,14 +354,16 @@ def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool) -> int:
     return 2 * (5 * H + hq * d + (hq + 2 * hkv) * d + I) + rope
 
 
-def new_cache(cfg: LongVITAConfig, num_layers: int, capacity: int, rows: int, device):
+def new_cache(cfg: LongVITAConfig, num_layers: int, capacity: int, rows: int, device,
+              host_dtype=torch.bfloat16):
     """The K/V cache of a generation whose prompt has `rows` tokens (kv_cache.make_cache): on the device when it fits
-    beside that prompt's prefill, else partly in pinned host memory, in which case the prefill streams above
-    STREAM_THRESHOLD (attention_step)."""
+    beside that prompt's prefill, else partly in pinned host memory (in `host_dtype`: bf16, or the lossy FP8 e4m3
+    format), in which case the prefill streams above STREAM_THRESHOLD (attention_step)."""
     return kv_cache.make_cache(num_layers, capacity, cfg.num_key_value_heads, cfg.head_dim, device,
                                prefill_bytes=rows * prefill_bytes_per_token(cfg, rows, False),
                                offloaded_prefill_bytes=rows * prefill_bytes_per_token(cfg, rows,
-                                                                                      rows > STREAM_THRESHOLD))
+                                                                                      rows > STREAM_THRESHOLD),
+                               host_dtype=host_dtype)
 
 
 def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: int = 1):
@@ -372,8 +374,9 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: 
 
     With a kv_cache.OffloadedKVCache, a layer on the host tier copies its new rows to its host buffer; in the prefill
     it then attends over its own k, v exactly as the step without a cache does, and a new token attends over the
-    host rows in place (ops.attention_decode_host).  `rows` is the number of new tokens of the forward; a cache that
-    cannot take them raises before anything is launched.
+    host rows in place (ops.attention_decode_host, or ops.attention_decode_host_fp8 for an FP8 host tier; the prefill
+    never reads the host rows, so its logits do not depend on the host format).  `rows` is the number of new tokens
+    of the forward; a cache that cannot take them raises before anything is launched.
 
     The plain step (no cache, one sample) and the prefill step of an empty offloaded cache declare `query_chunks`
     (query_chunked): called with query rows [r0, r1) and the keys [0, r1), its mask aligned to the last key gives
@@ -394,7 +397,7 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: 
             if cache.on_host(li):
                 kh, length = cache.append_host(li, k, v, n)
                 if n == 1:
-                    return ops.attention_decode_host(q[0], kh, length)
+                    return cache.decode_host(q[0], kh, length)
                 return ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True)
             kc, vc, length = cache.append(li, k, v, n)
             if n == 1:
@@ -562,9 +565,11 @@ class LongVITAModel(_WeightHolderModule):
             dev = inputs_embeds.device
 
         cache = past_key_values
+        # kv_host_dtype: the format of the host tier of a cache this call creates (kv_cache.make_cache)
+        host_dtype = kv_cache.check_host_dtype(flash_attn_kwargs.pop("kv_host_dtype", torch.bfloat16))
         if use_cache and cache is None:
             capacity = int(flash_attn_kwargs.pop("max_cache_len", 0)) or s + self.default_new_tokens
-            cache = new_cache(cfg, len(self.layers), capacity, s, dev)
+            cache = new_cache(cfg, len(self.layers), capacity, s, dev, host_dtype)
         flash_attn_kwargs.pop("max_cache_len", None)
         if cache_position is None:
             cache_position = torch.arange(past_len, past_len + s, device=dev)     # modeling_long_vita.py:153-158
@@ -771,11 +776,13 @@ class LongVITAForCausalLM(_WeightHolderModule):
     @torch.no_grad()
     def generate(self, inputs: Optional[torch.Tensor] = None, images: Optional[torch.Tensor] = None,
                  image_indices: Optional[torch.Tensor] = None, generation_config=None, input_ids: Optional[torch.Tensor] = None,
-                 max_new_tokens: Optional[int] = None, eos_token_id=None, do_sample: Optional[bool] = None, **kwargs):
+                 max_new_tokens: Optional[int] = None, eos_token_id=None, do_sample: Optional[bool] = None,
+                 kv_host_dtype=torch.bfloat16, **kwargs):
         """`model.generate(inputs=, images=, image_indices=)` as tools/inference_long_vita.py:868 calls it: greedy
         decoding (the script sets do_sample = False) with the K/V cache; stops at `eos_token_id` (int or list) or after
         `max_new_tokens`; returns prompt + generated ids [1, s + n] like transformers' GenerationMixin.  Inputs on the
-        host are moved to the model's device (the script leaves them on the CPU under device_map="auto")."""
+        host are moved to the model's device (the script leaves them on the CPU under device_map="auto").
+        `kv_host_dtype=torch.float8_e4m3fn` keeps the host tier of a cache that does not fit in HBM in FP8 (lossy)."""
         gc = generation_config if generation_config is not None else self.generation_config
         ids = inputs if inputs is not None else input_ids
         if ids is None:
@@ -792,13 +799,15 @@ class LongVITAForCausalLM(_WeightHolderModule):
             images = images.to(dev, dtype=torch.bfloat16)
         if image_indices is not None:
             image_indices = image_indices.to(dev)
-        new = self.generate_greedy(ids, images, image_indices, max_new_tokens=int(n_new), eos_token_ids=eos)
+        new = self.generate_greedy(ids, images, image_indices, max_new_tokens=int(n_new), eos_token_ids=eos,
+                                   kv_host_dtype=kv_host_dtype)
         return torch.cat([ids, new], dim=1)
 
     @torch.no_grad()
     def generate_greedy(self, input_ids: torch.Tensor, images: Optional[torch.Tensor] = None,
                         image_indices: Optional[torch.Tensor] = None, max_new_tokens: int = 16,
-                        eos_token_id: Optional[int] = None, eos_token_ids=None) -> torch.Tensor:
+                        eos_token_id: Optional[int] = None, eos_token_ids=None,
+                        kv_host_dtype=torch.bfloat16) -> torch.Tensor:
         """Greedy decoding with the K/V cache: one prefill, then one forward per token over a single new
         row (the reference's Megatron loop feeds the whole sequence again for every token,
         generation.py:127-135).  Returns the generated ids [1, n]."""
@@ -807,7 +816,7 @@ class LongVITAForCausalLM(_WeightHolderModule):
         if eos_token_id is not None:
             stop.add(int(eos_token_id))
         out = self.forward(input_ids=input_ids, images=images, image_indices=image_indices, use_cache=True,
-                           num_logits_to_keep=1, max_cache_len=s + max_new_tokens)
+                           num_logits_to_keep=1, max_cache_len=s + max_new_tokens, kv_host_dtype=kv_host_dtype)
         cache = out.past_key_values
         new = []
         tok = out.logits[0, -1].float().argmax().view(1, 1)

@@ -14,6 +14,10 @@ and `get_seq_length()` (:154).
 A cache that does not fit in HBM beside the prefill is an `OffloadedKVCache`: its leading layers are the device
 buffers above, the others one pinned host buffer each, read in place by the decode kernel (`ops.attention_decode_host`).
 `make_cache` decides which, once, from the free device memory (`device_layers`).
+
+The host tier may be kept in FP8 (`host_dtype=torch.float8_e4m3fn`): e4m3 K|V rows with one fp32 scale per head
+(csrc/kv_fp8_core.h), 2112 instead of 4096 bytes per row at 8 kv heads, which halves both the pinned memory and the
+PCIe bytes a decode step reads.  It is lossy and opt-in; the default is bf16, and the device layers are bf16 either way.
 """
 from __future__ import annotations
 
@@ -88,35 +92,55 @@ def device_layers(free_bytes: Optional[int], capacity: int, num_layers: int, kv_
     return int(max(0, min(num_layers - 1, (free_bytes - offloaded_prefill_bytes - reserve) // layer)))
 
 
+HOST_DTYPES = (torch.bfloat16, torch.float8_e4m3fn)
+
+
+def check_host_dtype(host_dtype) -> torch.dtype:
+    """host_dtype if it is a format of the host tier (bf16, the default, or FP8 e4m3), else ValueError."""
+    if host_dtype not in HOST_DTYPES:
+        raise ValueError(f"K/V cache host dtype must be torch.bfloat16 or torch.float8_e4m3fn, got {host_dtype!r}")
+    return host_dtype
+
+
 def make_cache(num_layers: int, capacity: int, num_kv_heads: int, head_dim: int, device, *, prefill_bytes: int,
-               offloaded_prefill_bytes: int, dtype=torch.bfloat16):
+               offloaded_prefill_bytes: int, dtype=torch.bfloat16, host_dtype=torch.bfloat16):
     """The K/V cache of a generation: a KVCache when it fits on the device (device_layers), else an OffloadedKVCache
-    with as many device layers as fit.  Every buffer, host ones included, is allocated here, before the prefill."""
+    with as many device layers as fit, its host layers in `host_dtype`.  The placement does not depend on
+    host_dtype, and a KVCache ignores it.  Every buffer, host ones included, is allocated here, before the prefill."""
+    check_host_dtype(host_dtype)
     row = 2 * num_kv_heads * head_dim * torch.empty((), dtype=dtype).element_size()
     n_dev = device_layers(device_free_bytes(device), capacity, num_layers, row, prefill_bytes, offloaded_prefill_bytes)
     if n_dev == num_layers:
         return KVCache(num_layers, capacity, num_kv_heads, head_dim, device, dtype)
-    return OffloadedKVCache(num_layers, n_dev, capacity, num_kv_heads, head_dim, device)
+    return OffloadedKVCache(num_layers, n_dev, capacity, num_kv_heads, head_dim, device, host_dtype=host_dtype)
 
 
 class OffloadedKVCache:
     """A K/V cache whose layers [0, n_dev) are [capacity, hkv, d] device buffers, as in KVCache, and whose layers
     [n_dev, num_layers) are one pinned host buffer [capacity, 2 hkv d] bf16 each: token-major rows of K of the hkv
-    heads then V of the hkv heads, the rows of the streamed layer's K|V buffer.
+    heads then V of the hkv heads, the rows of the streamed layer's K|V buffer.  With host_dtype=torch.float8_e4m3fn
+    a host layer is uint8 [capacity, ops.kv_fp8_row_bytes(hkv, d)] instead: the same rows quantised per head on the
+    way out (ops.kv_rows_to_host_fp8) and decoded by ops.attention_decode_host_fp8.
 
     The first forward fills it (it may stream: the attention step declares query_chunks while the cache is empty);
     each later forward adds one token.  A multi-token forward on a filled cache (chunked prefill, a second turn) is
     refused."""
 
-    def __init__(self, num_layers: int, n_dev: int, capacity: int, num_kv_heads: int, head_dim: int, device):
+    def __init__(self, num_layers: int, n_dev: int, capacity: int, num_kv_heads: int, head_dim: int, device,
+                 host_dtype=torch.bfloat16):
         if not 0 <= n_dev < num_layers:
             raise ValueError(f"OffloadedKVCache: {n_dev} device layers of {num_layers}")
         self.capacity = int(capacity)
         self.n_dev = int(n_dev)
+        self.host_dtype = check_host_dtype(host_dtype)
         shape = (self.capacity, num_kv_heads, head_dim)
         self.k = [torch.empty(shape, dtype=torch.bfloat16, device=device) for _ in range(n_dev)]
         self.v = [torch.empty(shape, dtype=torch.bfloat16, device=device) for _ in range(n_dev)]
-        self.host = [ops.pinned_rows(self.capacity, 2 * num_kv_heads * head_dim) for _ in range(num_layers - n_dev)]
+        if host_dtype == torch.float8_e4m3fn:
+            self.host = [ops.pinned_fp8_rows(self.capacity, num_kv_heads, head_dim) for _ in range(num_layers - n_dev)]
+        else:
+            self.host = [ops.pinned_rows(self.capacity, 2 * num_kv_heads * head_dim)
+                         for _ in range(num_layers - n_dev)]
         self._len = 0
         self._pending = 0
 
@@ -158,13 +182,20 @@ class OffloadedKVCache:
 
     def append_host(self, layer_idx: int, k: torch.Tensor, v: torch.Tensor,
                     n: Optional[int] = None) -> Tuple[torch.Tensor, int]:
-        """A host layer: the same rows, copied device-to-host in stream order (ops.kv_rows_to_host); returns (the
-        host buffer, len + kr)."""
+        """A host layer: the same rows, copied device-to-host in stream order (ops.kv_rows_to_host; quantised on
+        the way, ops.kv_rows_to_host_fp8, in an FP8 cache); returns (the host buffer, len + kr)."""
         r0, end, n = self._rows(k, n)
         kr = k.shape[0]
         host = self.host[layer_idx - self.n_dev]
-        ops.kv_rows_to_host(k[kr - n :], v[kr - n :], host[r0:end])
+        to_host = ops.kv_rows_to_host_fp8 if self.host_dtype == torch.float8_e4m3fn else ops.kv_rows_to_host
+        to_host(k[kr - n :], v[kr - n :], host[r0:end])
         return host, end
+
+    def decode_host(self, q: torch.Tensor, host: torch.Tensor, length: int) -> torch.Tensor:
+        """One new token's attention over rows [0, length) of a host layer, in its format."""
+        if self.host_dtype == torch.float8_e4m3fn:
+            return ops.attention_decode_host_fp8(q, host, length)
+        return ops.attention_decode_host(q, host, length)
 
     def commit(self) -> None:
         self._len += self._pending

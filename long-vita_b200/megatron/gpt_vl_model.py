@@ -38,7 +38,7 @@ from typing import Dict, Optional
 
 import torch
 
-from .. import ops
+from .. import kv_cache, ops
 from ..config import LongVITAConfig
 from ..cp import exchange_attention
 from ..hf import modeling
@@ -51,7 +51,7 @@ class B200GPTVLModel:
     def __init__(self, cfg: LongVITAConfig, state_dict: Dict[str, torch.Tensor], *, pre_process: bool = True,
                  post_process: bool = True, cp=None, is_instruction_dataset: bool = False,
                  output_multiplier_scale: Optional[float] = None, output_logit_softcapping: Optional[float] = None,
-                 gradient_accumulation_fusion: bool = False):
+                 gradient_accumulation_fusion: bool = False, kv_host_dtype=torch.bfloat16):
         if not (pre_process and post_process):
             raise NotImplementedError("pipeline parallelism is not built (14B bf16 fits one 80 GB H100: pp = 1)")
         self.config = cfg
@@ -63,6 +63,9 @@ class B200GPTVLModel:
         # Megatron's config.gradient_accumulation_fusion for the output layer: when output_weight requires grad, its
         # gradient is added to output_weight.main_grad (fp32) inside the GEMM (ops.masked_lm_head_ce / masked_linear)
         self.gradient_accumulation_fusion = bool(gradient_accumulation_fusion)
+        # the format of the host tier of a K/V cache the inference_params path creates (kv_cache.make_cache): bf16, or
+        # the lossy FP8 e4m3 one that halves its pinned memory and decode traffic
+        self.kv_host_dtype = kv_cache.check_host_dtype(kv_host_dtype)
         w = mcore_to_hf(state_dict, cfg)
         self.word_embeddings = w["model.embed_tokens.weight"]
         self.final_layernorm = w["model.norm.weight"]
@@ -159,7 +162,7 @@ class B200GPTVLModel:
             cache = kv.get("b200_kv_cache")
             if cache is None:
                 capacity = int(getattr(inference_params, "max_sequence_length", 0) or (s + 1024))
-                cache = modeling.new_cache(cfg, len(self.layers), capacity, s, dev)
+                cache = modeling.new_cache(cfg, len(self.layers), capacity, s, dev, self.kv_host_dtype)
                 kv["b200_kv_cache"] = cache
 
         # RoPE: Megatron builds the table for positions 0..S-1 and slices it zig-zag under CP

@@ -445,28 +445,54 @@ def _is_pinned(t: torch.Tensor) -> bool:
     return not t.is_cuda and t.is_pinned()
 
 
-def _host_rows(op: str, name: str, t: torch.Tensor, cols: Optional[int] = None) -> None:
-    """t must be a pinned host bf16 row matrix [rows, cols] with contiguous rows (the kernel reads it by address)."""
+def _host_rows(op: str, name: str, t: torch.Tensor, cols: Optional[int] = None,
+               dtype: torch.dtype = torch.bfloat16) -> None:
+    """t must be a pinned host row matrix [rows, cols] of `dtype` with contiguous rows (the kernel reads it by
+    address)."""
     if not _is_pinned(t):
         raise ValueError(f"{op}: {name} must be pinned host memory, got {t.device}"
                          f"{'' if t.is_cuda else ' (not pinned)'}")
-    if t.dtype != torch.bfloat16 or t.dim() != 2 or (cols is not None and t.shape[1] != cols) \
+    if t.dtype != dtype or t.dim() != 2 or (cols is not None and t.shape[1] != cols) \
             or t.stride() != (t.shape[1], 1):
         want = "[rows, cols]" if cols is None else f"[rows, {cols}]"
-        raise ValueError(f"{op}: {name} must be a contiguous bfloat16 {want}, got {t.dtype} {tuple(t.shape)} "
-                         f"strides {t.stride()}")
+        raise ValueError(f"{op}: {name} must be a contiguous {str(dtype).replace('torch.', '')} {want}, got "
+                         f"{t.dtype} {tuple(t.shape)} strides {t.stride()}")
 
 
-def pinned_rows(rows: int, cols: int) -> torch.Tensor:
-    """An uninitialised bf16 [rows, cols] tensor in pinned, device-mapped host memory of exactly that size
+def pinned_rows(rows: int, cols: int, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """An uninitialised [rows, cols] tensor of `dtype` in pinned, device-mapped host memory of exactly that size
     (lv_host_alloc; a caching pinned allocator rounds a buffer up to a power of two).  The memory is released when
     the last tensor viewing it is gone."""
-    n = int(rows) * int(cols) * 2
+    n = int(rows) * int(cols) * torch.empty((), dtype=dtype).element_size()
     p = C.c_void_p()
     _lib.check(_lib.lib().lv_host_alloc(n, C.byref(p)), "lv_host_alloc")
     buf = (C.c_uint8 * n).from_address(p.value)
     weakref.finalize(buf, _lib.lib().lv_host_free, p.value).atexit = False     # the process exit releases it
-    return torch.frombuffer(buf, dtype=torch.bfloat16).view(rows, cols)
+    return torch.frombuffer(buf, dtype=dtype).view(rows, cols)
+
+
+def kv_fp8_row_bytes(hkv: int, d: int) -> int:
+    """Bytes of one FP8 host row (csrc/kv_fp8_core.h): K and V of the hkv heads in e4m3, then the 2 hkv fp32 scales
+    padded to 16 bytes; 2112 at 8 kv heads of 128."""
+    return 2 * hkv * d + (8 * hkv + 15) // 16 * 16
+
+
+def pinned_fp8_rows(rows: int, hkv: int, d: int) -> torch.Tensor:
+    """The uninitialised uint8 [rows, kv_fp8_row_bytes(hkv, d)] rows of an FP8 host layer (pinned_rows)."""
+    return pinned_rows(rows, kv_fp8_row_bytes(hkv, d), torch.uint8)
+
+
+def _kv_source(op: str, k: torch.Tensor, v: torch.Tensor, dst: torch.Tensor) -> int:
+    """Row stride (elements) of the device K/V rows k / v [n, hkv, d] that V follows K in; dst must have n rows."""
+    n, hkv, d = k.shape
+    rs = k.stride(0) if n > 1 else 2 * hkv * d          # a single row's stride is arbitrary
+    if (v.shape != k.shape or not (k[0].is_contiguous() and v[0].is_contiguous()) or (n > 1 and v.stride(0) != rs)
+            or rs % 8 or rs < 2 * hkv * d or v.data_ptr() != k.data_ptr() + hkv * d * k.element_size()):
+        raise ValueError(f"{op}: k / v {tuple(k.shape)} strides {k.stride()} / {v.stride()} are not the "
+                         f"K and V halves of one row")
+    if dst.shape[0] != n:
+        raise ValueError(f"{op}: dst has {dst.shape[0]} rows for {n}")
+    return rs
 
 
 def kv_rows_to_host(k: torch.Tensor, v: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
@@ -476,14 +502,20 @@ def kv_rows_to_host(k: torch.Tensor, v: torch.Tensor, dst: torch.Tensor) -> torc
     _need_cuda_bf16(k, v)
     n, hkv, d = k.shape
     _host_rows("kv_rows_to_host", "dst", dst, 2 * hkv * d)
-    rs = k.stride(0) if n > 1 else 2 * hkv * d          # a single row's stride is arbitrary
-    if (v.shape != k.shape or not (k[0].is_contiguous() and v[0].is_contiguous()) or (n > 1 and v.stride(0) != rs)
-            or rs % 8 or rs < 2 * hkv * d or v.data_ptr() != k.data_ptr() + hkv * d * k.element_size()):
-        raise ValueError(f"kv_rows_to_host: k / v {tuple(k.shape)} strides {k.stride()} / {v.stride()} are not the "
-                         f"K and V halves of one row")
-    if dst.shape[0] != n:
-        raise ValueError(f"kv_rows_to_host: dst has {dst.shape[0]} rows for {n}")
+    rs = _kv_source("kv_rows_to_host", k, v, dst)
     _call("lv_rows_to_host", dst.data_ptr(), k.data_ptr(), n, 2 * hkv * d * 2, rs * 2)
+    return dst
+
+
+def kv_rows_to_host_fp8(k: torch.Tensor, v: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
+    """kv_rows_to_host into FP8 host rows: dst uint8 [n, kv_fp8_row_bytes(hkv, d)] (pinned) receives the rows of k / v
+    [n, hkv, d] quantised per head (csrc/kv_fp8_core.h), in stream order, by a kernel that stores straight into the
+    mapped host rows (lv_rows_to_host_fp8; no device temporary).  d = 128.  Returns dst."""
+    _need_cuda_bf16(k, v)
+    n, hkv, d = k.shape
+    _host_rows("kv_rows_to_host_fp8", "dst", dst, kv_fp8_row_bytes(hkv, d), torch.uint8)
+    rs = _kv_source("kv_rows_to_host_fp8", k, v, dst)
+    _call("lv_rows_to_host_fp8", dst.data_ptr(), k.data_ptr(), n, hkv, d, rs * 2)
     return dst
 
 
@@ -513,6 +545,34 @@ def attention_decode_host(q: torch.Tensor, kv_host: torch.Tensor, length: int, *
     lse = torch.empty((n_splits, hkv, G), dtype=torch.float32, device=q.device)
     _call("lv_attn_decode_host", q.contiguous().data_ptr(), kv_host.data_ptr(), o.data_ptr(), lse.data_ptr(), length,
           cap, hq, hkv, d, n_splits, float(scale if scale is not None else 1.0 / math.sqrt(d)))
+    return decode_merge(o, lse, return_lse=return_lse)
+
+
+def attention_decode_host_fp8(q: torch.Tensor, kv_host: torch.Tensor, length: int, *, scale: Optional[float] = None,
+                              n_splits: Optional[int] = None, return_lse: bool = False):
+    """attention_decode_host over FP8 host rows: kv_host uint8 [capacity, kv_fp8_row_bytes(hkv, d)] pinned (written by
+    kv_rows_to_host_fp8), read in place by lv_attn_decode_host_fp8 with the same split rule and merged by
+    lv_attn_decode_merge.  The result is attention over the dequantised rows, not over the bf16 ones.  Returns out
+    [hq, d] (and lse [hq] fp32, natural log)."""
+    _need_cuda_bf16(q)
+    if q.dim() != 2:
+        raise ValueError(f"attention_decode_host_fp8: q must be [hq, d], got {tuple(q.shape)}")
+    hq, d = q.shape
+    _host_rows("attention_decode_host_fp8", "kv_host", kv_host, dtype=torch.uint8)
+    cap, cols = kv_host.shape
+    hkv = cols // (2 * d + 8)                            # kv_fp8_row_bytes(h, d) is in [h (2d + 8), h (2d + 8) + 8)
+    if hkv == 0 or cols != kv_fp8_row_bytes(hkv, d) or hq % hkv:
+        raise ValueError(f"attention_decode_host_fp8: kv_host rows of {cols} bytes are not FP8 K|V rows of kv heads "
+                         f"of {d} for {hq} query heads")
+    if not 0 < length <= cap:
+        raise ValueError(f"attention_decode_host_fp8: length {length} outside the cache (capacity {cap})")
+    if n_splits is None:
+        n_splits = max(1, min(_sm_count(q.device), -(-length // 128)))
+    G = hq // hkv
+    o = torch.empty((n_splits, G, hkv, d), dtype=torch.bfloat16, device=q.device)
+    lse = torch.empty((n_splits, hkv, G), dtype=torch.float32, device=q.device)
+    _call("lv_attn_decode_host_fp8", q.contiguous().data_ptr(), kv_host.data_ptr(), o.data_ptr(), lse.data_ptr(),
+          length, cap, hq, hkv, d, n_splits, float(scale if scale is not None else 1.0 / math.sqrt(d)))
     return decode_merge(o, lse, return_lse=return_lse)
 
 
