@@ -383,6 +383,21 @@ int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t 
 int lv_gemm_wgrad_acc_f32(const void* A, const void* W, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                           int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, lv_stream_t stream);
 
+/* FP8 (e4m3) linears of the decoder (csrc/gemm_fp8.cu; the rule of csrc/kv_fp8_core.h applied to whole rows).
+ * lv_quant_rows_fp8: x bf16 [M, K] (row stride ldx elements, a multiple of 8) -> q e4m3 [M, K] contiguous and
+ * scale fp32 [M]: per row amax = max|x|, q = e4m3_rn_satfinite(x * (448 / amax)), scale = amax / 448; a row whose
+ * 448 / amax is not finite is zeros with scale 0.  K a positive multiple of 16; x and q 16-byte aligned.
+ * lv_gemm_fp8: C[M, N] = act(bf16((A . W^T) * a_scale[m] * w_scale[n] + bias[n])) with A e4m3 [M, K] (row stride
+ * lda bytes) and W e4m3 [N, K] (ldw bytes), both K-major, fp32 accumulation promoted out of the tensor cores every
+ * 128 k-values, C bf16 with row stride ldc elements.  act: 0 none (bias optional), 3 fused SwiGLU over interleaved
+ * (gate_i, up_i) W rows as in lv_gemm_bias_act (C is [M, N/2], bias NULL), each of gate and up scaled and rounded to
+ * bf16 before bf16(silu(gate)) * up.  K a multiple of 16, N of 8 (16 for SwiGLU), lda / ldw multiples of 16, ldc of
+ * 8; A, W, C 16-byte aligned.  For M <= 4 the product runs as a weight-stream GEMV (the rule of lv_gemm_bias_act). */
+int lv_quant_rows_fp8(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, lv_stream_t stream);
+int lv_gemm_fp8(const void* A, const float* a_scale, const void* W, const float* w_scale, const void* bias, void* C,
+                int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldw, int64_t ldc, int32_t act,
+                lv_stream_t stream);
+
 /* Patch embedding of 14x14 non-overlapping patches (Conv2d(3, C, k=14, s=14),
  * modeling_intern_vit.py:79-81,98; intern_vit_model.py:139-145,203) + class token + learned
  * position embedding (modeling_intern_vit.py:100-107):

@@ -119,6 +119,9 @@ SIGNATURES = {
     "lv_gemm_ex": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_i32, c_i32,
                            c_ptr]),
     "lv_gemm_wgrad_acc_f32": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_i32, c_ptr]),
+    "lv_quant_rows_fp8": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr]),
+    "lv_gemm_fp8": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32,
+                            c_ptr]),
     "lv_patch_embed_ws_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i64]),
     "lv_patch_embed": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr]),
 }

@@ -1,14 +1,18 @@
-// The FP8 (e4m3) row format of the host tier of the K/V cache and its quantiser, shared by the kernels
-// (csrc/attn_decode_host.cu: rows_to_host_fp8_kernel, attn_decode_host_fp8_kernel) and the host compiler:
-// tests/test_kv_fp8_host.py builds this text with gcc (LV_KV8_HD = static inline) and checks it, bit for bit, against
-// the torch.float8_e4m3fn restatement of the same rule.
+// The FP8 (e4m3) quantiser of the project and the row format of the host tier of the K/V cache, shared by the kernels
+// (csrc/attn_decode_host.cu: rows_to_host_fp8_kernel, attn_decode_host_fp8_kernel; csrc/gemm_fp8.cu:
+// quant_rows_fp8_kernel) and the host compiler: tests/test_kv_fp8_host.py and tests/test_fp8_linear_host.py build this
+// text with gcc (LV_KV8_HD = static inline) and check it, bit for bit, against the torch.float8_e4m3fn restatement of
+// the same rule.
+//
+// The rule quantises a row of n values with one fp32 scale: a K/V head (n = d), or a whole row of a linear layer's
+// operand (n = K: one scale per output channel of W [N, K], one per token of A [M, K]).
 //
 // A row of an FP8 layer holds, in this order: K of the hkv heads, e4m3 [hkv][d]; V of the hkv heads, e4m3 [hkv][d];
 // the scales, fp32 [2][hkv] (K scales, then V scales), zero-padded to a multiple of 16 bytes.  At hkv = 8, d = 128 a
 // row is 1024 + 1024 + 64 = 2112 bytes, against 4096 for bf16.
 //
-// One head's d values x are quantised in fp32: amax = max|x|; inv = 448 / amax (IEEE division, round to nearest);
-// q = e4m3_rn_satfinite(x * inv); scale = amax / 448, and x is read back as float(q) * scale.  A head whose inv is
+// A row's n values x are quantised in fp32: amax = max|x|; inv = 448 / amax (IEEE division, round to nearest);
+// q = e4m3_rn_satfinite(x * inv); scale = amax / 448, and x is read back as float(q) * scale.  A row whose inv is
 // not finite - amax is 0, or below 448 / FLT_MAX ~ 1.3e-36 (bf16 subnormals only) - is all-zero bytes with scale 0.
 #ifndef LV_KV_FP8_CORE_H_
 #define LV_KV_FP8_CORE_H_
@@ -93,25 +97,28 @@ static inline uint8_t lv_kv8_e4m3(float f) {
   return sign | (uint8_t)(((e + 6) << 3) + (q - 8));
 }
 
-// Quantise one head: x [d] bf16 bits -> q [d] e4m3, returns the scale.  The kernel splits a head over 8 lanes and
-// reduces amax with shuffles (max is exact in any order) and multiplies with __fmul_rn.
-static inline float lv_kv8_quant_head(const uint16_t* x, uint8_t* q, int d) {
+// Quantise one row: x [n] bf16 bits -> q [n] e4m3, returns the scale.  The kernels split a row over lanes, reduce
+// amax with shuffles (max is exact in any order) and multiply with __fmul_rn.
+static inline float lv_fp8_quant_row(const uint16_t* x, uint8_t* q, int64_t n) {
   float amax = 0.0f;
-  for (int i = 0; i < d; ++i) {
+  for (int64_t i = 0; i < n; ++i) {
     const float v = fabsf(lv_kv8_bf16_to_f32(x[i]));
     amax = v > amax ? v : amax;
   }
   const float inv = lv_kv8_inv(amax);
   if (lv_kv8_zero_head(inv)) {
-    for (int i = 0; i < d; ++i) q[i] = 0;
+    for (int64_t i = 0; i < n; ++i) q[i] = 0;
     return 0.0f;
   }
-  for (int i = 0; i < d; ++i) {
+  for (int64_t i = 0; i < n; ++i) {
     volatile float t = lv_kv8_bf16_to_f32(x[i]) * inv;
     q[i] = lv_kv8_e4m3(t);
   }
   return lv_kv8_scale(amax);
 }
+
+// One K/V head of d values is one row of the rule.
+static inline float lv_kv8_quant_head(const uint16_t* x, uint8_t* q, int d) { return lv_fp8_quant_row(x, q, d); }
 #endif
 
 #endif  // LV_KV_FP8_CORE_H_

@@ -175,12 +175,27 @@ def streams(T: int, attend) -> bool:
     return T > STREAM_THRESHOLD and query_chunked(attend)
 
 
+LINEAR_DTYPES = (torch.bfloat16, torch.float8_e4m3fn)
+
+
+def check_linear_dtype(linear_dtype) -> torch.dtype:
+    """linear_dtype if it is a format of the decoder's linear weights (bf16, the default, or FP8 e4m3), else
+    ValueError."""
+    if linear_dtype not in LINEAR_DTYPES:
+        raise ValueError(f"linear_dtype must be torch.bfloat16 or torch.float8_e4m3fn, got {linear_dtype!r}")
+    return linear_dtype
+
+
 class DecoderLayer:
     """Qwen2 decoder layer (transformers Qwen2DecoderLayer, instantiated by the reference at
     modeling_long_vita.py:57-72; mcore twin transformer_layer.py:173-257) with fused QKV and fused
-    gate|up weights (layout of tools/hf2mcore_long_vita.py:486-504)."""
+    gate|up weights (layout of tools/hf2mcore_long_vita.py:486-504).
 
-    def __init__(self, cfg: LongVITAConfig, w: Dict[str, torch.Tensor], i: int):
+    With linear_dtype=torch.float8_e4m3fn the four linear weights are ops.Fp8Weight (e4m3, one scale per output
+    channel), quantised here from the fused bf16 weights; ops.linear then runs the FP8 product at every call site.
+    Biases and norm weights stay bf16."""
+
+    def __init__(self, cfg: LongVITAConfig, w: Dict[str, torch.Tensor], i: int, linear_dtype=torch.bfloat16):
         p = f"model.layers.{i}."
         self.cfg = cfg
         self.wqkv = torch.cat([w[p + "self_attn.q_proj.weight"], w[p + "self_attn.k_proj.weight"],
@@ -193,6 +208,14 @@ class DecoderLayer:
         self.w_down = w[p + "mlp.down_proj.weight"]
         self.ln1 = w[p + "input_layernorm.weight"]
         self.ln2 = w[p + "post_attention_layernorm.weight"]
+        if check_linear_dtype(linear_dtype) == torch.float8_e4m3fn:
+            for name in ("wqkv", "wo", "w_gate_up", "w_down"):
+                setattr(self, name, ops.Fp8Weight.quantize(getattr(self, name)))
+
+    def linear_bytes(self) -> int:
+        """Resident bytes of the four linear weights (with their scales in FP8)."""
+        return sum(t.nbytes() if isinstance(t, ops.Fp8Weight) else t.numel() * t.element_size()
+                   for t in (self.wqkv, self.wo, self.w_gate_up, self.w_down))
 
     def forward(self, x: torch.Tensor, delta: Optional[torch.Tensor], cos, sin, attend,
                 qkv_out: Optional[torch.Tensor] = None,
@@ -339,30 +362,36 @@ def run_layers(layers, x: torch.Tensor, cos, sin, attend, norm_w: torch.Tensor, 
     return ops.rmsnorm(delta, norm_w, eps, residual=x)[0]
 
 
-def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool) -> int:
+def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool, linear_dtype=torch.bfloat16) -> int:
     """Device bytes per token that a decoder prefill of T rows holds beside the weights (DESIGN §3): whole-tensor
     layer (x, delta, QKV, attention output, new x, norm output, SwiGLU output, MLP output), row-chunked layer (x, QKV,
     attention output) or streamed layer (x, K|V), plus the RoPE tables.  At the 14B geometry: 103 936, 35 328 and
-    14 848 B."""
+    14 848 B.  With FP8 linears, add the largest quantised A operand (e4m3 rows of the widest linear input and their
+    fp32 scales) over the longest row span, spread over the T rows."""
     H, I = cfg.hidden_size, cfg.intermediate_size
     hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     rope = 2 * 2 * d
+    fp8 = 0
+    if linear_dtype == torch.float8_e4m3fn and T > 0:
+        span = max(r1 - r0 for r0, r1 in row_chunks(T))
+        fp8 = -(-span * (max(H, hq * d, I) + 4) // T)
     if streamed:
-        return 2 * (H + 2 * hkv * d) + rope
+        return 2 * (H + 2 * hkv * d) + rope + fp8
     if len(row_chunks(T)) > 1:
-        return 2 * (H + (hq + 2 * hkv) * d + hq * d) + rope
-    return 2 * (5 * H + hq * d + (hq + 2 * hkv) * d + I) + rope
+        return 2 * (H + (hq + 2 * hkv) * d + hq * d) + rope + fp8
+    return 2 * (5 * H + hq * d + (hq + 2 * hkv) * d + I) + rope + fp8
 
 
 def new_cache(cfg: LongVITAConfig, num_layers: int, capacity: int, rows: int, device,
-              host_dtype=torch.bfloat16):
+              host_dtype=torch.bfloat16, linear_dtype=torch.bfloat16):
     """The K/V cache of a generation whose prompt has `rows` tokens (kv_cache.make_cache): on the device when it fits
-    beside that prompt's prefill, else partly in pinned host memory (in `host_dtype`: bf16, or the lossy FP8 e4m3
-    format), in which case the prefill streams above STREAM_THRESHOLD (attention_step)."""
+    beside that prompt's prefill (with `linear_dtype` linears), else partly in pinned host memory (in `host_dtype`:
+    bf16, or the lossy FP8 e4m3 format), in which case the prefill streams above STREAM_THRESHOLD (attention_step)."""
     return kv_cache.make_cache(num_layers, capacity, cfg.num_key_value_heads, cfg.head_dim, device,
-                               prefill_bytes=rows * prefill_bytes_per_token(cfg, rows, False),
+                               prefill_bytes=rows * prefill_bytes_per_token(cfg, rows, False, linear_dtype),
                                offloaded_prefill_bytes=rows * prefill_bytes_per_token(cfg, rows,
-                                                                                      rows > STREAM_THRESHOLD),
+                                                                                      rows > STREAM_THRESHOLD,
+                                                                                      linear_dtype),
                                host_dtype=host_dtype)
 
 
@@ -492,6 +521,13 @@ def _map_tensors(obj, fn, seen=None):
                     _map_tensors(e, fn, seen)
         elif isinstance(val, (dict, InternVisionModel, ResamplerProjector, DecoderLayer)):
             _map_tensors(val, fn, seen)
+        elif isinstance(val, ops.Fp8Weight):
+            # moved, never cast: fn applied to the fp32 scale says where the weight goes
+            new = val.to(fn(val.scale).device)
+            if isinstance(obj, dict):
+                obj[name] = new
+            else:
+                object.__setattr__(obj, name, new)
 
 
 class _WeightHolderModule(torch.nn.Module):
@@ -507,15 +543,21 @@ class _WeightHolderModule(torch.nn.Module):
 
 class LongVITAModel(_WeightHolderModule):
     def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor],
-                 layers: Optional[Iterable[DecoderLayer]] = None):
+                 layers: Optional[Iterable[DecoderLayer]] = None, linear_dtype=torch.bfloat16):
         """`layers` replaces the decoder layers of `weights` (e.g. layers built one at a time, so that a layer's
-        unfused q/k/v and gate/up weights are freed before the next one is drawn)."""
+        unfused q/k/v and gate/up weights are freed before the next one is drawn); they must have been built with
+        `linear_dtype`, the format of the decoder's linear weights (bf16, or FP8 e4m3: DecoderLayer)."""
         super().__init__()
         self.config = cfg
+        self.linear_dtype = check_linear_dtype(linear_dtype)
         self.embed_tokens = weights["model.embed_tokens.weight"]
         self.norm_w = weights["model.norm.weight"]
-        self.layers = ([DecoderLayer(cfg, weights, i) for i in range(cfg.num_hidden_layers)] if layers is None
-                       else list(layers))
+        self.layers = ([DecoderLayer(cfg, weights, i, linear_dtype) for i in range(cfg.num_hidden_layers)]
+                       if layers is None else list(layers))
+        fp8 = linear_dtype == torch.float8_e4m3fn
+        for i, layer in enumerate(self.layers):
+            if isinstance(layer.wqkv, ops.Fp8Weight) != fp8:
+                raise ValueError(f"decoder layer {i} was not built with linear_dtype={linear_dtype}")
         self.vision_model, self.vision_projection = vision_tower(cfg, weights)
         self.inv_freq = rope_inv_freq(cfg, self.embed_tokens.device)
         self.vision_chunk = VISION_CHUNK
@@ -569,7 +611,7 @@ class LongVITAModel(_WeightHolderModule):
         host_dtype = kv_cache.check_host_dtype(flash_attn_kwargs.pop("kv_host_dtype", torch.bfloat16))
         if use_cache and cache is None:
             capacity = int(flash_attn_kwargs.pop("max_cache_len", 0)) or s + self.default_new_tokens
-            cache = new_cache(cfg, len(self.layers), capacity, s, dev, host_dtype)
+            cache = new_cache(cfg, len(self.layers), capacity, s, dev, host_dtype, self.linear_dtype)
         flash_attn_kwargs.pop("max_cache_len", None)
         if cache_position is None:
             cache_position = torch.arange(past_len, past_len + s, device=dev)     # modeling_long_vita.py:153-158
@@ -615,7 +657,11 @@ class LongVITAModel(_WeightHolderModule):
 
     def hf_state_dict(self, prefix: str = "model.") -> Dict[str, torch.Tensor]:
         """The weights under the reference's HF parameter names (views of the fused buffers; the padded patch-embed
-        operand is cut back to the [C, 3, ps, ps] conv weight)."""
+        operand is cut back to the [C, 3, ps, ps] conv weight).  A model with FP8 linears has no such state dict (no
+        quantised checkpoint format is defined): NotImplementedError."""
+        if self.linear_dtype != torch.bfloat16:
+            raise NotImplementedError("state_dict() of a model with FP8 linears: no quantised checkpoint format is "
+                                      "defined; load the bf16 checkpoint with linear_dtype= instead")
         sd = {prefix + "embed_tokens.weight": self.embed_tokens, prefix + "norm.weight": self.norm_w}
         cfg = self.config
         for i, L in enumerate(self.layers):
@@ -659,10 +705,13 @@ class GenerationDefaults:
 
 class LongVITAForCausalLM(_WeightHolderModule):
     def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor],
-                 layers: Optional[Iterable[DecoderLayer]] = None):
+                 layers: Optional[Iterable[DecoderLayer]] = None, linear_dtype=torch.bfloat16):
+        """`linear_dtype=torch.float8_e4m3fn` runs the decoder's four linears in FP8 (lossy, opt-in; DecoderLayer):
+        their weights are quantised per output channel as the layers are built.  The vision tower, projector,
+        embedding, norms and LM head stay bf16."""
         super().__init__()
         self.config = cfg
-        self.model = LongVITAModel(cfg, weights, layers)
+        self.model = LongVITAModel(cfg, weights, layers, linear_dtype)
         self.lm_head = weights["lm_head.weight"]
         self.generation_config = GenerationDefaults()
 
@@ -681,11 +730,12 @@ class LongVITAForCausalLM(_WeightHolderModule):
 
     @classmethod
     def from_pretrained(cls, model_path: str, torch_dtype=torch.bfloat16, device_map=None, attn_implementation=None,
-                        trust_remote_code: bool = True, **kwargs):
+                        trust_remote_code: bool = True, linear_dtype=torch.bfloat16, **kwargs):
         """Load a Long-VITA HF checkpoint directory (config.json + *.safetensors shards), the call
         tools/inference_long_vita.py:811-817 makes through AutoModelForCausalLM.  Only bfloat16 runs on the fused
         path; `attn_implementation` is accepted and ignored (the fused kernel IS the attention implementation);
-        `device_map` "auto" / None -> the current CUDA device."""
+        `device_map` "auto" / None -> the current CUDA device.  Decoder layers are read and built one at a time;
+        `linear_dtype=torch.float8_e4m3fn` quantises each one's linears as it is built (see __init__)."""
         import glob
         import json
         import os
@@ -694,6 +744,7 @@ class LongVITAForCausalLM(_WeightHolderModule):
 
         if torch_dtype not in (torch.bfloat16, "bfloat16", None, "auto"):
             raise NotImplementedError("the fused path computes in bfloat16 (the reference's torch_dtype)")
+        check_linear_dtype(linear_dtype)
         c = json.load(open(os.path.join(model_path, "config.json")))
         vc = c.get("visual", c.get("vision_config", {})) or {}
         from dataclasses import fields, replace
@@ -706,30 +757,45 @@ class LongVITAForCausalLM(_WeightHolderModule):
 
         cfg = replace(LongVITAConfig(**pick(LongVITAConfig, c)), visual=VisionConfig(**pick(VisionConfig, vc)))
         dev = torch.device("cuda", torch.cuda.current_device()) if device_map in (None, "auto") else torch.device(device_map)
-        w: Dict[str, torch.Tensor] = {}
         shards = sorted(glob.glob(os.path.join(model_path, "*.safetensors")))
         if not shards:
             raise FileNotFoundError(f"no *.safetensors under {model_path}")
+        where: Dict[str, str] = {}
         for sh in shards:
             with safe_open(sh, framework="pt", device=str(dev)) as f:
-                for name in f.keys():
-                    w[name] = f.get_tensor(name).to(torch.bfloat16)
-        return cls(cfg, w)
+                where.update((name, sh) for name in f.keys())
+
+        def read(names):
+            out: Dict[str, torch.Tensor] = {}
+            for sh in sorted({where[n] for n in names}):
+                with safe_open(sh, framework="pt", device=str(dev)) as f:
+                    out.update((n, f.get_tensor(n).to(torch.bfloat16)) for n in names if where[n] == sh)
+            return out
+
+        # the decoder layers one at a time: a layer's bf16 tensors are released once it is built
+        def layer_names(i):
+            return [n for n in where if n.startswith(f"model.layers.{i}.")]
+
+        w = read([n for n in where if not n.startswith("model.layers.")])
+        layers = (DecoderLayer(cfg, read(layer_names(i)), i, linear_dtype) for i in range(cfg.num_hidden_layers))
+        return cls(cfg, w, layers, linear_dtype)
 
     @classmethod
     def from_synthetic(cls, cfg: LongVITAConfig, seed: int = 1234, device="cuda", perturb: bool = False,
-                       num_layers: Optional[int] = None):
+                       num_layers: Optional[int] = None, linear_dtype=torch.bfloat16):
         """Random-init model materialised layer by layer on `device` (14B bf16 = 29.5 GB never
-        exists twice): every decoder layer's q/k/v and gate/up matrices are fused as they are drawn."""
+        exists twice): every decoder layer's q/k/v and gate/up matrices are fused as they are drawn, and with
+        `linear_dtype=torch.float8_e4m3fn` quantised before the next layer is drawn."""
         from ..weights import global_weights, llm_layer_weights, vit_layer_weights
 
+        check_linear_dtype(linear_dtype)
         w = global_weights(cfg, seed, device, torch.bfloat16, perturb)
         for i in range(cfg.visual.num_hidden_layers):
             w.update(vit_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb))
         n_layers = cfg.num_hidden_layers if num_layers is None else num_layers
-        layers = (DecoderLayer(cfg, llm_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb), i)
+        layers = (DecoderLayer(cfg, llm_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb), i, linear_dtype)
                   for i in range(n_layers))
-        return cls(cfg, w, layers)
+        return cls(cfg, w, layers, linear_dtype)
 
     def forward(
         self,

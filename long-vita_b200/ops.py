@@ -768,11 +768,14 @@ def _gemm_operand(t: torch.Tensor, mn_ok: bool = True) -> Tuple[torch.Tensor, bo
     return t, False, t.stride(0)
 
 
-def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] = None, act: Optional[str] = None,
+def linear(x: torch.Tensor, weight, bias: Optional[torch.Tensor] = None, act: Optional[str] = None,
            out: Optional[torch.Tensor] = None):
     """act(x @ weight.T + bias); weight is [N, K] (nn.Linear layout).  Either operand may also be a 2-D transposed
     view (stride(0) == 1, stride(1) a multiple of 8, e.g. t.t() of a contiguous [K, X]): the kernel reads it in place
-    (lv_gemm_ex) instead of a contiguous copy.  Any other layout is copied to a contiguous tensor first."""
+    (lv_gemm_ex) instead of a contiguous copy.  Any other layout is copied to a contiguous tensor first.  An Fp8Weight
+    runs the FP8 product instead (linear_fp8)."""
+    if isinstance(weight, Fp8Weight):
+        return linear_fp8(x, weight, bias, act, out)
     _need_cuda_bf16(x, weight, bias)
     K = x.shape[-1]
     if weight.dim() != 2 or weight.shape[1] != K:
@@ -796,6 +799,134 @@ def linear(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tensor] =
               out.stride(0), _ACT[act])
     if ev0 is not None:
         _TIMER.stop("gemm_bf16", 2.0 * M * N * K, ev0)
+    return out.view(*x.shape[:-1], n_out)
+
+
+# ------------------------------------------------------------------------------------------------
+# FP8 (e4m3) linears: per-row scales on both operands (csrc/kv_fp8_core.h), lv_gemm_fp8
+# ------------------------------------------------------------------------------------------------
+FP8 = torch.float8_e4m3fn
+
+
+def quant_rows_fp8(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """x bf16 [M, K] (K contiguous, K a multiple of 16, row stride a multiple of 8) -> (q e4m3 [M, K], scale fp32
+    [M]): one scale per row, amax / 448, q = e4m3(x * 448 / amax); a row of zeros (or too small to scale) is zeros
+    with scale 0 (lv_quant_rows_fp8).  x ~ q.float() * scale[:, None]."""
+    _need_cuda_bf16(x)
+    if x.dim() != 2:
+        raise ValueError(f"quant_rows_fp8: x must be [M, K], got {tuple(x.shape)}")
+    M, K = x.shape
+    if K == 0 or K % 16:
+        raise ValueError(f"quant_rows_fp8: K={K} must be a positive multiple of 16")
+    if x.stride(1) != 1 or x.stride(0) % 8 or x.data_ptr() % 16:
+        x = x.contiguous()
+    q = torch.empty((M, K), dtype=FP8, device=x.device)
+    scale = torch.empty((M,), dtype=torch.float32, device=x.device)
+    if M:
+        _call("lv_quant_rows_fp8", x.data_ptr(), q.data_ptr(), scale.data_ptr(), M, K, max(x.stride(0), K))
+    return q, scale
+
+
+class Fp8Weight:
+    """A linear layer's weight in FP8: data e4m3 [N, K] with one fp32 scale per output channel (row), scale [N]; the
+    weight reads back as data.float() * scale[:, None].  Row slicing w[a:b] slices both (the Q and K|V rows of a fused
+    QKV weight).  ops.linear takes it in place of a bf16 weight."""
+
+    __slots__ = ("data", "scale")
+
+    def __init__(self, data: torch.Tensor, scale: torch.Tensor):
+        if data.dtype != FP8 or data.dim() != 2 or scale.dtype != torch.float32 or scale.shape != (data.shape[0],):
+            raise ValueError(f"Fp8Weight: data must be float8_e4m3fn [N, K] and scale float32 [N], got {data.dtype} "
+                             f"{tuple(data.shape)} and {scale.dtype} {tuple(scale.shape)}")
+        self.data, self.scale = data, scale
+
+    @classmethod
+    def quantize(cls, w: torch.Tensor) -> "Fp8Weight":
+        """The bf16 weight w [N, K] quantised per row (quant_rows_fp8)."""
+        return cls(*quant_rows_fp8(w))
+
+    @property
+    def shape(self) -> torch.Size:
+        return self.data.shape
+
+    @property
+    def device(self) -> torch.device:
+        return self.data.device
+
+    def dim(self) -> int:
+        return 2
+
+    def nbytes(self) -> int:
+        return self.data.numel() + 4 * self.scale.numel()
+
+    def __getitem__(self, rows) -> "Fp8Weight":
+        if not isinstance(rows, slice) or rows.step not in (None, 1):
+            raise TypeError("Fp8Weight: only contiguous row slices w[a:b] are supported")
+        return Fp8Weight(self.data[rows], self.scale[rows])
+
+    def to(self, device) -> "Fp8Weight":
+        return Fp8Weight(self.data.to(device), self.scale.to(device))
+
+    def dequantize(self) -> torch.Tensor:
+        """The fp32 weight it stands for."""
+        return self.data.float() * self.scale[:, None]
+
+
+def linear_fp8(x: torch.Tensor, weight: Fp8Weight, bias: Optional[torch.Tensor] = None, act: Optional[str] = None,
+               out: Optional[torch.Tensor] = None):
+    """act(bf16((x_q @ w_q.T) * s_x * s_w + bias)): x bf16 [..., K] is quantised per row (quant_rows_fp8), then
+    lv_gemm_fp8 multiplies it with the FP8 weight [N, K] (a GEMV for up to 4 rows).  act is None or "swiglu" (weight
+    rows interleaved (gate_i, up_i), no bias).  `out`, if given, is a bf16 [M, N or N / 2] row matrix with
+    contiguous rows, 16-byte aligned, whose row stride is a multiple of 8 (e.g. rows of a wider buffer)."""
+    for name, t, dtype in (("x", x, torch.bfloat16), ("bias", bias, torch.bfloat16), ("out", out, torch.bfloat16),
+                           ("weight.data", weight.data, FP8), ("weight.scale", weight.scale, torch.float32)):
+        if t is not None and t.dtype != dtype:
+            raise ValueError(f"linear_fp8: {name} must be {dtype}, got {t.dtype}")
+    _need_cuda_bf16(x, bias)
+    _need_cuda(weight.data, FP8)
+    _need_cuda(weight.scale, torch.float32)
+    K = x.shape[-1]
+    N = weight.shape[0]
+    if weight.shape[1] != K:
+        raise ValueError(f"linear_fp8: weight {tuple(weight.shape)} is not [N, K={K}]")
+    if K % 16:
+        raise ValueError(f"linear_fp8: K={K} must be a multiple of 16")
+    if act not in (None, "none", "swiglu"):
+        raise ValueError(f"linear_fp8: activation {act!r} is not built (None or 'swiglu')")
+    if N % (16 if act == "swiglu" else 8):
+        raise ValueError(f"linear_fp8: N={N} must be a multiple of {16 if act == 'swiglu' else 8}")
+    if act == "swiglu" and bias is not None:
+        raise ValueError("linear_fp8: the fused SwiGLU takes no bias")
+    if weight.data.stride(1) != 1 or weight.data.stride(0) % 16 or weight.data.data_ptr() % 16:
+        raise ValueError(f"linear_fp8: weight rows must be contiguous and 16-byte aligned with a row stride that is a "
+                         f"multiple of 16, got strides {weight.data.stride()}")
+    bias = _param("linear_fp8", "bias", bias, N)
+    x2 = x.reshape(-1, K)
+    M = x2.shape[0]
+    n_out = N // 2 if act == "swiglu" else N
+    if out is None:
+        out = torch.empty((M, n_out), dtype=torch.bfloat16, device=x.device)
+    else:
+        _need_cuda_bf16(out)
+        if (out.dim() != 2 or out.shape != (M, n_out) or out.stride(1) != 1
+                or (M > 1 and (out.stride(0) % 8 or out.stride(0) < n_out)) or out.data_ptr() % 16):
+            raise ValueError(f"linear_fp8: out {tuple(out.shape)} strides {out.stride()} is not a 16-byte aligned "
+                             f"[{M}, {n_out}] row matrix with a row stride that is a multiple of 8")
+    if M == 0:
+        return out.view(*x.shape[:-1], n_out)
+    if x2.stride(1) != 1 or x2.stride(0) % 8 or x2.data_ptr() % 16:
+        x2 = x2.contiguous()
+    # the quantised A operand in one temporary, e4m3 rows then their fp32 scales: a decode step is bound by host work
+    # per launch, so the FP8 call allocates once more than the bf16 one, not twice
+    ws = torch.empty((M * K + 4 * M,), dtype=torch.uint8, device=x.device)
+    xq, xs = ws.data_ptr(), ws.data_ptr() + M * K
+    _call("lv_quant_rows_fp8", x2.data_ptr(), xq, xs, M, K, max(x2.stride(0), K))
+    ev0 = _TIMER.start() if _TIMER is not None else None
+    ldc = out.stride(0) if M > 1 else -(-n_out // 8) * 8
+    _call("lv_gemm_fp8", xq, xs, weight.data.data_ptr(), weight.scale.data_ptr(), _ptr(bias),
+          out.data_ptr(), M, N, K, K, weight.data.stride(0), ldc, _ACT[act])
+    if ev0 is not None:
+        _TIMER.stop("gemm_fp8", 2.0 * M * N * K, ev0)
     return out.view(*x.shape[:-1], n_out)
 
 
