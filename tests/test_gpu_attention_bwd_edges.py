@@ -1,20 +1,20 @@
 """GPU parity of the attention backward at the edges of its ABI: ragged lengths on both sides of the 64-row half tiles
 of both passes, sk > sq and sq > sk, `kv_pos0`, an explicit softmax scale, large logits, and strided layouts.
 
-Every case runs lv_attn_fwd then lv_attn_bwd on the device and compares dQ, dK and dV with the float64 reference of
+Every case runs lv_attn_fwd then lv_attn_bwd on the device and holds dQ, dK and dV to `check_attn_bwd` of
 tests/attn_grad_ref.py at the same global positions, given the forward output the backward reads (`out=`, see there
-why), with the bound of tests/test_gpu_attention_bwd.py: error in excess of the bf16 output-rounding floor < 3e-3, and
-every value finite.  Rows and keys the mask hides from everything must come out exactly zero."""
+why): every value finite, exact zeros on rows and keys the mask hides from everything, the elementwise bound, the
+per-row Z, and the error in excess of the bf16 output-rounding floor < 3e-3.  Every row of a causal case is a paired
+plant (`plant_pairs`) aimed at its first hidden key or its diagonal, so a mask off by one key in either pass is an O(1)
+error."""
 import pytest
 import torch
 
-from tests.attn_grad_ref import attention_grads
+from tests.attn_grad_ref import attention_grads, check_rows, edge_targets, plant_edge_pairs
 from tests.test_gpu_attention_bwd import excess
 from tests.util import randn_bf16, seeded
 
 pytestmark = pytest.mark.gpu
-
-TOL_EXCESS = 3e-3
 
 
 @pytest.fixture(scope="module")
@@ -40,24 +40,19 @@ def _run(L, q, k, v, do, *, causal, scale=None, kv_pos0=0):
     return out, lse, grads
 
 
-def _check(got, out, q, k, v, do, *, causal, scale=None, kv_pos0=0):
+def _check(got, out, q, k, v, do, *, causal, scale=None, kv_pos0=0, planted=None):
     sq, sk = q.shape[1], k.shape[1]
-    ref = attention_grads(q, k, v, do, causal=causal, scale=scale, q_pos=torch.arange(sq) + (sk - sq),
-                          kv_pos=torch.arange(sk) + kv_pos0, out=out)
-    errs = {}
-    for name, a, r in zip(("dq", "dk", "dv"), got, ref):
-        assert torch.isfinite(a).all(), name
-        if float(r.abs().max()) < 1e-9:
-            # one visible key per query (sq = sk = 1): P = 1 and dS = dP - delta = 0, so dQ = dK = 0 up to the
-            # rounding of dP and delta (fp32 in the kernel, float64 here); a relative error to zero means nothing
-            assert float(a.abs().max()) < 1e-4, (name, float(a.abs().max()))
-            errs[name] = 0.0
-            continue
-        errs[name] = excess(a, r)
-    print("excess", {n: f"{e:.2e}" for n, e in errs.items()})
-    for name, e in errs.items():
-        assert e < TOL_EXCESS, (name, e)
-    return ref, errs
+    return check_rows(got, q, k, v, do, out, causal=causal, scale=scale, q_pos=torch.arange(sq) + (sk - sq),
+                      kv_pos=torch.arange(sk) + kv_pos0, planted=planted, label=f"{sq}x{sk}")
+
+
+def _plant(q, k, *, kv_pos0=0, scale=None):
+    """Every row a paired plant at its mask edge: even rows the first hidden key, odd rows the diagonal."""
+    sq, sk = q.shape[1], k.shape[1]
+    rows = torch.arange(sq)
+    pos = rows + (sk - sq)
+    return plant_edge_pairs(q, k, rows, edge_targets(rows, pos, kv_pos0), q_pos=pos, kv_pos=torch.arange(sk) + kv_pos0,
+                            scale=scale)
 
 
 # sq = sk on both sides of the 64-row half tiles; d in {64, 128}; causal both ways; GQA 1, 5, 8 (hq = G * hkv)
@@ -73,8 +68,9 @@ RAGGED = [
 def test_ragged_lengths(L, s, d, causal, G):
     b, hkv = 2 if s % 2 else 1, 2
     q, k, v, do = _inputs(b, s, s, G * hkv, hkv, d, seed=s * 10 + G)
+    planted = _plant(q, k) if causal else None
     out, _, got = _run(L, q, k, v, do, causal=causal)
-    _check(got, out, q, k, v, do, causal=causal)
+    _check(got, out, q, k, v, do, causal=causal, planted=planted)
 
 
 @pytest.mark.parametrize("sq,sk", [(100, 612), (65, 1000), (1, 300)])
@@ -82,8 +78,9 @@ def test_ragged_lengths(L, s, d, causal, G):
 def test_cross_lengths_sk_above_sq(L, sq, sk, causal):
     d = 128 if sq != 65 else 64
     q, k, v, do = _inputs(1, sq, sk, 10, 2, d, seed=sq + sk)
+    planted = _plant(q, k) if causal else None
     out, _, got = _run(L, q, k, v, do, causal=causal)
-    _check(got, out, q, k, v, do, causal=causal)
+    _check(got, out, q, k, v, do, causal=causal, planted=planted)
 
 
 @pytest.mark.parametrize("sq,sk,d", [(300, 100, 128), (257, 64, 64)])
@@ -91,13 +88,14 @@ def test_causal_sq_above_sk_rows_that_see_no_key(L, sq, sk, d):
     """Bottom-right alignment: query i sits at position i + sk - sq, so the first sq - sk rows see no key.  The forward
     gives them out = 0 and lse = -inf, and the backward dQ = 0 exactly, with nothing NaN or infinite."""
     q, k, v, do = _inputs(2, sq, sk, 10, 2, d, seed=sq)
+    planted = _plant(q, k)
     out, lse, got = _run(L, q, k, v, do, causal=True)
     blind = sq - sk
     assert not out[:, :blind].any()
     assert bool((lse[:, :, :blind] == float("-inf")).all()) and torch.isfinite(lse[:, :, blind:]).all()
     assert torch.isfinite(out).all()
     assert not got[0][:, :blind].any()
-    _check(got, out, q, k, v, do, causal=True)
+    _check(got, out, q, k, v, do, causal=True, planted=planted)
 
 
 @pytest.mark.parametrize("sq,sk,kv_pos0,d", [(384, 384, 100, 128), (200, 500, 37, 64), (256, 256, 64, 128)])
@@ -105,6 +103,7 @@ def test_kv_pos0_one_segment(L, sq, sk, kv_pos0, d):
     """Keys at kv_pos0 + j: query rows before the first key see nothing (dQ = 0) and key rows past the last query
     position are seen by no query (dK = dV = 0 exactly)."""
     q, k, v, do = _inputs(1, sq, sk, 10, 2, d, seed=kv_pos0)
+    planted = _plant(q, k, kv_pos0=kv_pos0)
     out, _, (dq, dk, dv) = _run(L, q, k, v, do, causal=True, kv_pos0=kv_pos0)
     last_q = sk - 1                                   # position of the last query row
     unseen = last_q - kv_pos0 + 1                     # first key row no query sees
@@ -112,15 +111,16 @@ def test_kv_pos0_one_segment(L, sq, sk, kv_pos0, d):
     assert not dk[:, unseen:].any() and not dv[:, unseen:].any()
     blind = max(0, kv_pos0 - (sk - sq))               # query rows before the first key
     assert not dq[:, :blind].any()
-    _check((dq, dk, dv), out, q, k, v, do, causal=True, kv_pos0=kv_pos0)
+    _check((dq, dk, dv), out, q, k, v, do, causal=True, kv_pos0=kv_pos0, planted=planted)
 
 
 @pytest.mark.parametrize("scale", [0.05, 0.3])
 @pytest.mark.parametrize("d", [64, 128])
 def test_explicit_scale(L, scale, d):
     q, k, v, do = _inputs(1, 333, 333, 10, 2, d, seed=int(scale * 100) + d)
+    planted = _plant(q, k, scale=scale)
     out, _, got = _run(L, q, k, v, do, causal=True, scale=scale)
-    _check(got, out, q, k, v, do, causal=True, scale=scale)
+    _check(got, out, q, k, v, do, causal=True, scale=scale, planted=planted)
 
 
 def _large_logit_inputs():

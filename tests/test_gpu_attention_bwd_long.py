@@ -10,8 +10,11 @@ off the exact one while rounding P and dS to bf16 accounts for 0.88e-3; measured
     positions against all S = 131 072 keys, full tensors, dK / dV being the rank's partial sums;
   * 131 072 and 425 984 tokens on one device: sampled query rows, and sampled 128-key tiles against every query that
     sees them.
-Bounds: the error in excess of the bf16 output-rounding floor < 3e-3 (tests/test_gpu_attention_bwd.py), and per
-(row, head) a relative error bound, so that one wrong tile cannot hide inside a Frobenius norm over millions of rows.
+Bounds: `check_attn_bwd` of tests/attn_grad_ref.py (exact zeros, the elementwise bound, the per-row Z, the error in
+excess of the bf16 output-rounding floor < 3e-3), and per (row, head) a relative error bound, so that one wrong tile
+cannot hide inside a Frobenius norm over millions of rows.  Except at 16 384 (also compared with the exact gradient,
+which a planted row's peaked softmax moves away from), the query tiles at the diagonal or at a zig-zag segment's start
+and end are paired plants (`plant_pairs`) on every row.
 What these lengths exercise that S <= 1025 does not: pass A streams up to G x S/64 query tiles per 128-key item,
 pass B's longest-first order runs over 10^4 - 10^5 items, dK rows sum over > 10^5 query rows, and at 425 984 the row
 offsets of Q / dO / dQ pass 2^31 elements.
@@ -20,7 +23,8 @@ import pytest
 import torch
 
 from oracle import ops as O
-from tests.attn_grad_ref import _sample_rows, attention_grads
+from tests.attn_grad_ref import (_sample_rows, attention_grads, check_attn_bwd, check_planted_pairs, edge_targets,
+                                plant_edge_pairs)
 
 pytestmark = pytest.mark.gpu
 
@@ -65,20 +69,31 @@ def _excess(a, r):
     return max(e * e - f * f, 0.0) ** 0.5
 
 
-def _worst_row(a, r):
-    """Largest relative error of one (batch, row, head) over rows whose reference norm is not tiny."""
+def _worst_row(a, r, keep_rows):
+    """Largest relative error of one (batch, row, head) over the rows `keep_rows` whose reference norm is not tiny."""
+    a, r = a[:, keep_rows], r[:, keep_rows]
     rn = r.norm(dim=-1)
     keep = rn >= ROW_FLOOR * rn.pow(2).mean().sqrt()
     err = (a.double() - r).norm(dim=-1)
     return float((err[keep] / rn[keep]).max())
 
 
-def _check(name, got, ref):
-    """Excess < TOL_EXCESS and worst row < TOL_ROW for each of dq, dk, dv; returns the measurements."""
+def _check(name, got, ref, planted=None):
+    """check_attn_bwd against `ref` (attention_grads with terms), excess < TOL_EXCESS and worst row < TOL_ROW for each
+    of dq, dk, dv; returns the measurements.  The relative row bound skips the planted rows and keys: a planted key's
+    dK sums large terms of both signs (dS_it = -dS_ip on a visible pair), so its relative error means nothing, and the
+    elementwise bound and Z hold those rows instead."""
+    print(name, {k: f"{v:.3g}" for k, v in check_attn_bwd(got, ref, label=name).items()})
+    keep_q = torch.ones(ref["q_rows"].numel(), dtype=torch.bool, device=ref["dq"].device)
+    keep_k = torch.ones(ref["kv_rows"].numel(), dtype=torch.bool, device=ref["dq"].device)
+    if planted is not None:
+        for rows, targets, partners in planted.values():
+            keep_q &= ~torch.isin(ref["q_rows"], rows.to(keep_q.device))
+            keep_k &= ~torch.isin(ref["kv_rows"], torch.cat([targets, partners]).to(keep_k.device))
     m = {}
-    for g, a, r in zip(("dq", "dk", "dv"), got, ref):
+    for g, a, r in zip(("dq", "dk", "dv"), got, (ref["dq"], ref["dk"], ref["dv"])):
         assert torch.isfinite(a).all(), (name, g)
-        m[g] = (_excess(a, r), _worst_row(a, r))
+        m[g] = (_excess(a, r), _worst_row(a, r, keep_q if g == "dq" else keep_k))
     print(name, {g: f"excess {e:.2e} row {w:.2e}" for g, (e, w) in m.items()})
     for g, (e, w) in m.items():
         assert e < TOL_EXCESS and w < TOL_ROW, (name, g, e, w)
@@ -92,7 +107,7 @@ def test_backward_16k_full_tensor(L):
     S = 16384
     q, k, v, do = _device_inputs(S, seed=1)
     out, _, got = _fwd_bwd(L, q, k, v, do)
-    _check("16k", got, attention_grads(q, k, v, do, causal=True, out=out))
+    _check("16k", got, attention_grads(q, k, v, do, causal=True, out=out, terms=True))
     exact = attention_grads(q, k, v, do, causal=True)
     assert all(_excess(a, r) < TOL_EXCESS for a, r in zip(got, exact))
     _, _, again = _fwd_bwd(L, q, k, v, do)
@@ -106,21 +121,33 @@ def test_backward_of_one_context_parallel_rank(L, S, cp, rank):
     own queries: full-tensor parity, and exactly zero past the last key its queries see."""
     c = S // (2 * cp)
     q, k, v, do = _device_inputs(S, seed=S + 10 * cp + rank, sq=2 * c)
+    pos = O.zigzag_positions(S, cp, rank)
+    prow = torch.cat([torch.arange(t * 128, t * 128 + 128) for t in (0, c // 128 - 1, c // 128, 2 * c // 128 - 1)])
+    planted = plant_edge_pairs(q, k, prow, edge_targets(prow, pos), q_pos=pos, kv_pos=torch.arange(S))
     seg = dict(q_seg_len=c, q_seg_pos=(rank * c, (2 * cp - 1 - rank) * c))
     out, _, got = _fwd_bwd(L, q, k, v, do, **seg)
-    ref = attention_grads(q, k, v, do, causal=True, q_pos=O.zigzag_positions(S, cp, rank), out=out)
-    _check(f"cp{cp} rank{rank}", got, ref)
+    ref = attention_grads(q, k, v, do, causal=True, q_pos=pos, out=out, terms=True)
+    check_planted_pairs(q, k, ref, planted)
+    _check(f"cp{cp} rank{rank}", got, ref, planted)
     last_visible = (2 * cp - rank) * c
     assert not got[1][:, last_visible:].any() and not got[2][:, last_visible:].any()
 
 
-def _sampled(L, S, rows, tiles, seed):
+def _sampled(L, S, rows, tiles, seed, planted_tiles):
+    """Sampled dQ rows plus every row of `planted_tiles` (paired plants at the diagonal), and the key tiles `tiles`."""
     q, k, v, do = _device_inputs(S, seed=seed)
+    prow = torch.cat([torch.arange(t * 128, t * 128 + 128) for t in planted_tiles])
+    pos = torch.arange(S)
+    planted = plant_edge_pairs(q, k, prow, edge_targets(prow, pos), q_pos=pos, kv_pos=pos)
+    rows = torch.unique(torch.cat([rows, prow]))
     out, _, (dq, dk, dv) = _fwd_bwd(L, q, k, v, do)
     keys = torch.cat([torch.arange(t * 128, min(t * 128 + 128, S)) for t in tiles])
-    ref = attention_grads(q, k, v, do, causal=True, q_rows=rows, kv_rows=keys, out=out)
+    ref = attention_grads(q, k, v, do, causal=True, q_rows=rows, kv_rows=keys, out=out, terms=True)
+    check_planted_pairs(q, k, ref, planted)
     rc, kc = rows.cuda(), keys.cuda()
-    return (dq[:, rc], dk[:, kc], dv[:, kc]), ref
+    _, _, again = _fwd_bwd(L, q, k, v, do)
+    assert all(torch.equal(a, b) for a, b in zip((dq, dk, dv), again))
+    return (dq[:, rc], dk[:, kc], dv[:, kc]), ref, planted
 
 
 def test_backward_131k_sampled(L):
@@ -128,8 +155,9 @@ def test_backward_131k_sampled(L):
     two for dK / dV, each against every query that sees it."""
     S = 131072
     n_kt = S // 128
-    got, ref = _sampled(L, S, _sample_rows(256, S, seed=S), (0, n_kt // 2, n_kt - 2, n_kt - 1), seed=S)
-    _check("131k sampled", got, ref)
+    got, ref, planted = _sampled(L, S, _sample_rows(256, S, seed=S), (0, n_kt // 2, n_kt - 2, n_kt - 1), seed=S,
+                                 planted_tiles=(0, 1, n_kt // 2, n_kt - 1))
+    _check("131k sampled", got, ref, planted)
 
 
 def test_backward_beyond_2_31_elements(L):
@@ -140,8 +168,9 @@ def test_backward_beyond_2_31_elements(L):
     rows = torch.tensor(sorted({0, 127, 128, 255, 256, S // 2, S - 257, S - 256, S - 129, S - 128, S - 2, S - 1}
                                | {int(x) for x in torch.randint(S // 2, S, (36,), generator=torch.Generator().manual_seed(7))}))
     n_kt = S // 128
-    got, ref = _sampled(L, S, rows, (n_kt - 3, n_kt - 2, n_kt - 1), seed=7)
-    _check("425k sampled", got, ref)
+    got, ref, planted = _sampled(L, S, rows, (n_kt - 3, n_kt - 2, n_kt - 1), seed=7,
+                                 planted_tiles=(0, n_kt // 2, n_kt - 1))
+    _check("425k sampled", got, ref, planted)
 
 
 def test_backward_16k_vs_flash_attn(L):

@@ -3,8 +3,10 @@
 1. One document is today's causal kernel, bit for bit.
 2. Documents whose lengths are multiples of 128 give, row for row, exactly what a standalone causal call on each
    document gives: the tile walks coincide, so any difference is a range or a mask bug.
-3. Unaligned and edge documents against the fp32 oracle with the tolerances of the dense kernels (output excess
-   < 2e-3, lse < 1e-4, gradient excess < 3e-3), and within 1.25x of flash_attn_varlen_func where it is installed.
+3. Unaligned and edge documents: the forward against the fp32 oracle with the tolerances of the dense kernels (output
+   excess < 2e-3, lse < 1e-4), the gradients against the float64 reference of tests/attn_grad_ref.py through
+   `check_attn_bwd`, with the first rows of documents planted at their start (`plant_pairs`: the previous document's
+   last key hidden, the document's first key visible); and within 1.25x of flash_attn_varlen_func where installed.
 4. Two backward runs are bit-identical.
 """
 import math
@@ -14,6 +16,8 @@ import torch
 
 from oracle import ops as O
 from tests import packed_oracle as PO
+from tests.attn_fwd_ref import doc_lo
+from tests.attn_grad_ref import check_rows, plant_edge_pairs
 from tests.util import randn_bf16, rel_fro, seeded
 
 pytestmark = pytest.mark.gpu
@@ -120,15 +124,20 @@ EDGE = [1, 63, 64, 65, 127, 128, 129, 30, 90, 200, 45, 17]   # boundaries inside
 def test_unaligned_documents_against_the_oracle(lib_built, lengths, hq, hkv):
     cu = cu_of(lengths)
     d = 128
-    q, k, v, do = inputs(cu[-1], hq, hkv, d, seed=len(lengths) * 3 + hq)
+    S = cu[-1]
+    q, k, v, do = inputs(S, hq, hkv, d, seed=len(lengths) * 3 + hq)
+    lo = doc_lo(cu, S)
+    rows = torch.cat([torch.arange(a, min(e, a + 130)) for a, e in zip(cu[1:], cu[2:])])
+    planted = plant_edge_pairs(q, k, rows, torch.where(rows % 2 == 0, lo[rows] - 1, lo[rows]), q_pos=torch.arange(S),
+                               kv_pos=torch.arange(S), kv_lo=lo)
     got = run_docs(q, k, v, do, cu)
     ref = oracle_per_doc(q, k, v, do, cu)
     for t in got:
         assert torch.isfinite(t).all()
     assert excess(got[0], ref[0]) < 2e-3, excess(got[0], ref[0])
     assert float((got[1].cpu() - ref[1]).abs().max()) < 1e-4
-    for name, a, r in zip(("dq", "dk", "dv"), got[2:], ref[2:]):
-        assert excess(a, r) < 3e-3, (name, excess(a, r))
+    check_rows(got[2:], *(t.cuda() for t in (q, k, v, do)), got[0], causal=True, kv_lo=lo.cuda(), planted=planted,
+               label=f"documents {len(lengths)} x {hq}:{hkv}")
     if sum(lengths) <= 2048:     # the per-document oracle is the definition; cross-check with the explicit mask once
         o_m, l_m = PO.attention(q, k, v, cu)
         assert torch.allclose(o_m, ref[0], atol=1e-5) and torch.allclose(l_m, ref[1], atol=1e-5)
