@@ -135,6 +135,39 @@ typedef struct lv_attn_docs {
 } lv_attn_docs;
 
 int lv_attn_docs_fwd(const lv_attn_params* a, const lv_attn_docs* docs, lv_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * FP8 (e4m3) attention forward (opt-in, lossy; csrc/attn_fwd_fp8.cu, rule in csrc/attn_fp8_core.h): causal
+ * attention on the FP8 tensor cores with K and V quantised once per call.
+ *
+ * With nt = ceil(sk / 128) key blocks of 128 rows, aligned to key row 0 (the last one zero-padded):
+ *   k8       e4m3 [b][hkv][nt * 128][d]   the quantised keys
+ *   vt8      e4m3 [b][hkv][nt][d][128]    each block of values transposed; inside each 32-key chunk, byte
+ *                                         32 c + 16 h + 4 t + i of a row holds key 32 c + 16 h + 8 (i / 2) + 2 t + i % 2
+ *   k_scale, v_scale  float [b][hkv][nt]
+ * A block's values x are quantised as one row of the host tier's rule: amax = max|x|, q = e4m3_rn_satfinite(x * (448 /
+ * amax)), scale = amax / 448, zero bytes and scale 0 when 448 / amax is not finite.
+ *
+ * lv_attn_fp8_quant_kv: bf16 K and V of `a` (a->k, a->v, batch, sk, hkv, d, k_strides, v_strides; the other fields
+ *   are not read) -> the four buffers of `kv`, one pass.  d = 128; k, v, k8, vt8 16-byte aligned.
+ * lv_attn_fwd_fp8: lv_attn_fwd over the quantised K / V of `kv` (a->k and a->v are not read).  Q is quantised inside
+ *   the kernel, one scale per (batch, query head, 64-row group aligned to query row 0); the scores are
+ *   s_q s_k (q8 . k8) in fp32, p = exp2 of the log2-domain score minus the running max in fp32, the row sum takes
+ *   p, and P V takes e4m3(p * 2^8) * v8 with the 2^-8 in the block's V scale, accumulated in fp32 per key block
+ *   (out of the tensor cores every 128 keys).  Only d = 128 and causal = 1 with sq <= sk, q_seg_len = sq,
+ *   q_seg_pos = {sk - sq, 0}, kv_pos0 = 0 are built; anything else (documents, query segments, context
+ *   parallelism) is LV_EINVAL.  A call over query rows [r0, r1) and keys [0, r1), r0 a multiple of 128, returns
+ *   exactly those rows of the call over all rows. lse as for lv_attn_fwd (may be NULL).
+ * ------------------------------------------------------------------------------------------ */
+typedef struct lv_attn_fp8_kv {
+  void* k8;
+  void* vt8;
+  float* k_scale;
+  float* v_scale;
+} lv_attn_fp8_kv;
+
+int lv_attn_fp8_quant_kv(const lv_attn_params* a, const lv_attn_fp8_kv* kv, lv_stream_t stream);
+int lv_attn_fwd_fp8(const lv_attn_params* a, const lv_attn_fp8_kv* kv, lv_stream_t stream);
 int lv_attn_docs_bwd(const lv_attn_bwd_params* p, const lv_attn_docs* docs, lv_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------

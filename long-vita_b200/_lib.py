@@ -50,6 +50,12 @@ class AttnDocs(C.Structure):
     _fields_ = [("cu_seqlens", c_ptr), ("n_docs", c_i64)]
 
 
+class AttnFp8Kv(C.Structure):
+    """Mirror of `lv_attn_fp8_kv` (include/lvb200.h)."""
+
+    _fields_ = [("k8", c_ptr), ("vt8", c_ptr), ("k_scale", c_ptr), ("v_scale", c_ptr)]
+
+
 class CpParams(C.Structure):
     """Mirror of `lv_cp_params` (include/lvb200.h)."""
 
@@ -70,6 +76,8 @@ SIGNATURES = {
     "lv_attn_bwd": (c_i32, [C.POINTER(AttnBwdParams), c_ptr]),
     "lv_attn_docs_fwd": (c_i32, [C.POINTER(AttnParams), C.POINTER(AttnDocs), c_ptr]),
     "lv_attn_docs_bwd": (c_i32, [C.POINTER(AttnBwdParams), C.POINTER(AttnDocs), c_ptr]),
+    "lv_attn_fp8_quant_kv": (c_i32, [C.POINTER(AttnParams), C.POINTER(AttnFp8Kv), c_ptr]),
+    "lv_attn_fwd_fp8": (c_i32, [C.POINTER(AttnParams), C.POINTER(AttnFp8Kv), c_ptr]),
     "lv_attn_cp_fwd": (c_i32, [C.POINTER(AttnParams), C.POINTER(CpParams), c_ptr]),
     "lv_cp_check_fault": (c_i32, [c_ptr, c_ptr]),
     "lv_ipc_alloc": (c_i32, [c_i64, C.POINTER(c_ptr)]),

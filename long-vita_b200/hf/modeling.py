@@ -176,6 +176,7 @@ def streams(T: int, attend) -> bool:
 
 
 LINEAR_DTYPES = (torch.bfloat16, torch.float8_e4m3fn)
+ATTN_DTYPES = (torch.bfloat16, torch.float8_e4m3fn)
 
 
 def check_linear_dtype(linear_dtype) -> torch.dtype:
@@ -184,6 +185,14 @@ def check_linear_dtype(linear_dtype) -> torch.dtype:
     if linear_dtype not in LINEAR_DTYPES:
         raise ValueError(f"linear_dtype must be torch.bfloat16 or torch.float8_e4m3fn, got {linear_dtype!r}")
     return linear_dtype
+
+
+def check_attn_dtype(attn_dtype) -> torch.dtype:
+    """attn_dtype if it is an operand format of the decoder's prefill attention (bf16, the default, or FP8 e4m3:
+    ops.attention_fwd_fp8), else ValueError."""
+    if attn_dtype not in ATTN_DTYPES:
+        raise ValueError(f"attn_dtype must be torch.bfloat16 or torch.float8_e4m3fn, got {attn_dtype!r}")
+    return attn_dtype
 
 
 class DecoderLayer:
@@ -362,12 +371,14 @@ def run_layers(layers, x: torch.Tensor, cos, sin, attend, norm_w: torch.Tensor, 
     return ops.rmsnorm(delta, norm_w, eps, residual=x)[0]
 
 
-def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool, linear_dtype=torch.bfloat16) -> int:
+def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool, linear_dtype=torch.bfloat16,
+                            attn_dtype=torch.bfloat16) -> int:
     """Device bytes per token that a decoder prefill of T rows holds beside the weights (DESIGN §3): whole-tensor
     layer (x, delta, QKV, attention output, new x, norm output, SwiGLU output, MLP output), row-chunked layer (x, QKV,
     attention output) or streamed layer (x, K|V), plus the RoPE tables.  At the 14B geometry: 103 936, 35 328 and
     14 848 B.  With FP8 linears, add the largest quantised A operand (e4m3 rows of the widest linear input and their
-    fp32 scales) over the longest row span, spread over the T rows."""
+    fp32 scales) over the longest row span, spread over the T rows.  With FP8 attention, add the quantised K / V of a
+    call over all T keys (ops.attn_fp8_kv_bytes: 2 hkv d bytes per key row and the block scales)."""
     H, I = cfg.hidden_size, cfg.intermediate_size
     hq, hkv, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     rope = 2 * 2 * d
@@ -375,6 +386,8 @@ def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool, linear_
     if linear_dtype == torch.float8_e4m3fn and T > 0:
         span = max(r1 - r0 for r0, r1 in row_chunks(T))
         fp8 = -(-span * (max(H, hq * d, I) + 4) // T)
+    if attn_dtype == torch.float8_e4m3fn and T > 0:
+        fp8 += -(-ops.attn_fp8_kv_bytes(T, hkv, d) // T)
     if streamed:
         return 2 * (H + 2 * hkv * d) + rope + fp8
     if len(row_chunks(T)) > 1:
@@ -383,19 +396,20 @@ def prefill_bytes_per_token(cfg: LongVITAConfig, T: int, streamed: bool, linear_
 
 
 def new_cache(cfg: LongVITAConfig, num_layers: int, capacity: int, rows: int, device,
-              host_dtype=torch.bfloat16, linear_dtype=torch.bfloat16):
+              host_dtype=torch.bfloat16, linear_dtype=torch.bfloat16, attn_dtype=torch.bfloat16):
     """The K/V cache of a generation whose prompt has `rows` tokens (kv_cache.make_cache): on the device when it fits
-    beside that prompt's prefill (with `linear_dtype` linears), else partly in pinned host memory (in `host_dtype`:
-    bf16, or the lossy FP8 e4m3 format), in which case the prefill streams above STREAM_THRESHOLD (attention_step)."""
+    beside that prompt's prefill (with `linear_dtype` linears and `attn_dtype` attention), else partly in pinned host
+    memory (in `host_dtype`: bf16, or the lossy FP8 e4m3 format), in which case the prefill streams above
+    STREAM_THRESHOLD (attention_step)."""
     return kv_cache.make_cache(num_layers, capacity, cfg.num_key_value_heads, cfg.head_dim, device,
-                               prefill_bytes=rows * prefill_bytes_per_token(cfg, rows, False, linear_dtype),
+                               prefill_bytes=rows * prefill_bytes_per_token(cfg, rows, False, linear_dtype, attn_dtype),
                                offloaded_prefill_bytes=rows * prefill_bytes_per_token(cfg, rows,
                                                                                       rows > STREAM_THRESHOLD,
-                                                                                      linear_dtype),
+                                                                                      linear_dtype, attn_dtype),
                                host_dtype=host_dtype)
 
 
-def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: int = 1):
+def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: int = 1, attn_dtype=torch.bfloat16):
     """The single-GPU attention step for run_layers.  Without `cache`: causal attention over this forward's rows
     (inside each packed document with `cu_seqlens`).  With `cache`: the new K/V rows are appended to it and one new
     token attends over the whole cache (flash-decoding), several new tokens over cache + new rows with the causal mask
@@ -409,7 +423,17 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: 
 
     The plain step (no cache, one sample) and the prefill step of an empty offloaded cache declare `query_chunks`
     (query_chunked): called with query rows [r0, r1) and the keys [0, r1), its mask aligned to the last key gives
-    exactly those rows of the whole call."""
+    exactly those rows of the whole call.
+
+    `attn_dtype=torch.float8_e4m3fn` runs every call of several new tokens on the FP8 kernel (ops.attention_fwd_fp8:
+    lossy, opt-in), whole-tensor, row-chunked and streamed alike; its blocks are aligned to key row 0, so the span
+    calls of the streamed layer still give exactly the rows of the whole call.  One new token (decode) and the cache
+    contents stay bf16.  Packed rows (`cu_seqlens`) have no FP8 path: NotImplementedError, before anything runs."""
+    if check_attn_dtype(attn_dtype) == torch.float8_e4m3fn:
+        if cu_seqlens is not None:
+            raise NotImplementedError("packed samples (position ids restarting at 0) have no FP8 attention; use "
+                                      "attn_dtype=torch.bfloat16")
+        return _fp8_attention_step(cache, rows)
     kw = ops.docs_kwargs(cu_seqlens)
     if cache is None:
         def attend(li, q, k, v):
@@ -441,6 +465,45 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: 
         if q.shape[0] == 1:
             return ops.attention_decode(q[0], kc, vc, length)
         return ops.attention_fwd(q.unsqueeze(0), kc[:length].unsqueeze(0), vc[:length].unsqueeze(0), causal=True)
+
+    return attend
+
+
+def _fp8_attention_step(cache, rows: int):
+    """attention_step with FP8 prefill attention: the same steps, each multi-token call on ops.attention_fwd_fp8."""
+    def prefill(q, k, v):
+        return ops.attention_fwd_fp8(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True)
+
+    if cache is None:
+        def attend(li, q, k, v):
+            return prefill(q, k, v)
+
+        attend.query_chunks = True
+        return attend
+
+    if isinstance(cache, OffloadedKVCache):
+        cache.check_rows(rows)
+
+        def attend(li, q, k, v):
+            n = q.shape[0]
+            if cache.on_host(li):
+                kh, length = cache.append_host(li, k, v, n)
+                if n == 1:
+                    return cache.decode_host(q[0], kh, length)
+                return prefill(q, k, v)
+            kc, vc, length = cache.append(li, k, v, n)
+            if n == 1:
+                return ops.attention_decode(q[0], kc, vc, length)
+            return prefill(q, kc[:length], vc[:length])
+
+        attend.query_chunks = len(cache) == 0
+        return attend
+
+    def attend(li, q, k, v):
+        kc, vc, length = cache.append(li, k, v)
+        if q.shape[0] == 1:
+            return ops.attention_decode(q[0], kc, vc, length)
+        return prefill(q, kc[:length], vc[:length])
 
     return attend
 
@@ -543,13 +606,16 @@ class _WeightHolderModule(torch.nn.Module):
 
 class LongVITAModel(_WeightHolderModule):
     def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor],
-                 layers: Optional[Iterable[DecoderLayer]] = None, linear_dtype=torch.bfloat16):
+                 layers: Optional[Iterable[DecoderLayer]] = None, linear_dtype=torch.bfloat16,
+                 attn_dtype=torch.bfloat16):
         """`layers` replaces the decoder layers of `weights` (e.g. layers built one at a time, so that a layer's
         unfused q/k/v and gate/up weights are freed before the next one is drawn); they must have been built with
-        `linear_dtype`, the format of the decoder's linear weights (bf16, or FP8 e4m3: DecoderLayer)."""
+        `linear_dtype`, the format of the decoder's linear weights (bf16, or FP8 e4m3: DecoderLayer).  `attn_dtype`
+        is the operand format of the decoder's prefill attention (bf16, or FP8 e4m3: attention_step)."""
         super().__init__()
         self.config = cfg
         self.linear_dtype = check_linear_dtype(linear_dtype)
+        self.attn_dtype = check_attn_dtype(attn_dtype)
         self.embed_tokens = weights["model.embed_tokens.weight"]
         self.norm_w = weights["model.norm.weight"]
         self.layers = ([DecoderLayer(cfg, weights, i, linear_dtype) for i in range(cfg.num_hidden_layers)]
@@ -611,7 +677,7 @@ class LongVITAModel(_WeightHolderModule):
         host_dtype = kv_cache.check_host_dtype(flash_attn_kwargs.pop("kv_host_dtype", torch.bfloat16))
         if use_cache and cache is None:
             capacity = int(flash_attn_kwargs.pop("max_cache_len", 0)) or s + self.default_new_tokens
-            cache = new_cache(cfg, len(self.layers), capacity, s, dev, host_dtype, self.linear_dtype)
+            cache = new_cache(cfg, len(self.layers), capacity, s, dev, host_dtype, self.linear_dtype, self.attn_dtype)
         flash_attn_kwargs.pop("max_cache_len", None)
         if cache_position is None:
             cache_position = torch.arange(past_len, past_len + s, device=dev)     # modeling_long_vita.py:153-158
@@ -622,7 +688,7 @@ class LongVITAModel(_WeightHolderModule):
             # packed samples: positions restarting at 0 inside the row are sample boundaries; attention stays inside
             # each sample, as transformers' flash_attention_2 does for the reference (tools/inference_long_vita.py:816)
             cu = packed_rows(position_ids, s, dev, cache=cache)
-        attend = attention_step(cache, cu, s)
+        attend = attention_step(cache, cu, s, self.attn_dtype)
 
         encode = images is not None and past_len == 0              # modeling_long_vita.py:90
         # when the decoder streams, so does the vision phase: each ViT chunk's features go into x as they are made
@@ -705,13 +771,15 @@ class GenerationDefaults:
 
 class LongVITAForCausalLM(_WeightHolderModule):
     def __init__(self, cfg: LongVITAConfig, weights: Dict[str, torch.Tensor],
-                 layers: Optional[Iterable[DecoderLayer]] = None, linear_dtype=torch.bfloat16):
+                 layers: Optional[Iterable[DecoderLayer]] = None, linear_dtype=torch.bfloat16,
+                 attn_dtype=torch.bfloat16):
         """`linear_dtype=torch.float8_e4m3fn` runs the decoder's four linears in FP8 (lossy, opt-in; DecoderLayer):
-        their weights are quantised per output channel as the layers are built.  The vision tower, projector,
-        embedding, norms and LM head stay bf16."""
+        their weights are quantised per output channel as the layers are built.  `attn_dtype=torch.float8_e4m3fn` runs
+        the decoder's prefill attention on the FP8 kernel (lossy, opt-in; attention_step).  The vision tower,
+        projector, embedding, norms and LM head stay bf16."""
         super().__init__()
         self.config = cfg
-        self.model = LongVITAModel(cfg, weights, layers, linear_dtype)
+        self.model = LongVITAModel(cfg, weights, layers, linear_dtype, attn_dtype)
         self.lm_head = weights["lm_head.weight"]
         self.generation_config = GenerationDefaults()
 
@@ -730,12 +798,14 @@ class LongVITAForCausalLM(_WeightHolderModule):
 
     @classmethod
     def from_pretrained(cls, model_path: str, torch_dtype=torch.bfloat16, device_map=None, attn_implementation=None,
-                        trust_remote_code: bool = True, linear_dtype=torch.bfloat16, **kwargs):
+                        trust_remote_code: bool = True, linear_dtype=torch.bfloat16, attn_dtype=torch.bfloat16,
+                        **kwargs):
         """Load a Long-VITA HF checkpoint directory (config.json + *.safetensors shards), the call
         tools/inference_long_vita.py:811-817 makes through AutoModelForCausalLM.  Only bfloat16 runs on the fused
         path; `attn_implementation` is accepted and ignored (the fused kernel IS the attention implementation);
         `device_map` "auto" / None -> the current CUDA device.  Decoder layers are read and built one at a time;
-        `linear_dtype=torch.float8_e4m3fn` quantises each one's linears as it is built (see __init__)."""
+        `linear_dtype=torch.float8_e4m3fn` quantises each one's linears as it is built, `attn_dtype` selects the
+        prefill attention (see __init__)."""
         import glob
         import json
         import os
@@ -745,6 +815,7 @@ class LongVITAForCausalLM(_WeightHolderModule):
         if torch_dtype not in (torch.bfloat16, "bfloat16", None, "auto"):
             raise NotImplementedError("the fused path computes in bfloat16 (the reference's torch_dtype)")
         check_linear_dtype(linear_dtype)
+        check_attn_dtype(attn_dtype)
         c = json.load(open(os.path.join(model_path, "config.json")))
         vc = c.get("visual", c.get("vision_config", {})) or {}
         from dataclasses import fields, replace
@@ -778,24 +849,25 @@ class LongVITAForCausalLM(_WeightHolderModule):
 
         w = read([n for n in where if not n.startswith("model.layers.")])
         layers = (DecoderLayer(cfg, read(layer_names(i)), i, linear_dtype) for i in range(cfg.num_hidden_layers))
-        return cls(cfg, w, layers, linear_dtype)
+        return cls(cfg, w, layers, linear_dtype, attn_dtype)
 
     @classmethod
     def from_synthetic(cls, cfg: LongVITAConfig, seed: int = 1234, device="cuda", perturb: bool = False,
-                       num_layers: Optional[int] = None, linear_dtype=torch.bfloat16):
+                       num_layers: Optional[int] = None, linear_dtype=torch.bfloat16, attn_dtype=torch.bfloat16):
         """Random-init model materialised layer by layer on `device` (14B bf16 = 29.5 GB never
         exists twice): every decoder layer's q/k/v and gate/up matrices are fused as they are drawn, and with
-        `linear_dtype=torch.float8_e4m3fn` quantised before the next layer is drawn."""
+        `linear_dtype=torch.float8_e4m3fn` quantised before the next layer is drawn; `attn_dtype` as in __init__."""
         from ..weights import global_weights, llm_layer_weights, vit_layer_weights
 
         check_linear_dtype(linear_dtype)
+        check_attn_dtype(attn_dtype)
         w = global_weights(cfg, seed, device, torch.bfloat16, perturb)
         for i in range(cfg.visual.num_hidden_layers):
             w.update(vit_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb))
         n_layers = cfg.num_hidden_layers if num_layers is None else num_layers
         layers = (DecoderLayer(cfg, llm_layer_weights(cfg, i, seed, device, torch.bfloat16, perturb), i, linear_dtype)
                   for i in range(n_layers))
-        return cls(cfg, w, layers, linear_dtype)
+        return cls(cfg, w, layers, linear_dtype, attn_dtype)
 
     def forward(
         self,

@@ -17,7 +17,7 @@ from typing import Optional, Tuple
 import torch
 
 from . import _lib
-from ._lib import AttnBwdParams, AttnDocs, AttnParams
+from ._lib import AttnBwdParams, AttnDocs, AttnFp8Kv, AttnParams
 
 
 def _stream() -> int:
@@ -310,6 +310,80 @@ def attention_fwd(
         else:
             fl = 4.0 * b * hq * d * sq * sk  # upper bound for masked / segmented calls
         _TIMER.stop("attn_fwd", fl, ev0)
+    return (out, lse) if return_lse else out
+
+
+ATTN_FP8_BLOCK = 128   # key rows per K / V scale of the FP8 attention (csrc/attn_fp8_core.h)
+
+
+def attn_fp8_kv_bytes(sk: int, hkv: int, d: int, batch: int = 1) -> int:
+    """Device bytes of the quantised K / V that attention_fwd_fp8 holds during a call: K8 and Vt8 (e4m3, whole
+    128-row blocks) and the two fp32 scales per block."""
+    nt = -(-sk // ATTN_FP8_BLOCK)
+    return batch * hkv * nt * (2 * ATTN_FP8_BLOCK * d + 8)
+
+
+def attn_fp8_quant_kv(k: torch.Tensor, v: torch.Tensor):
+    """K / V [b, sk, hkv, 128] bf16 views (strided, e.g. columns of a QKV buffer) -> (k8 [b, hkv, nt * 128, d],
+    vt8 [b, hkv, nt, d, 128], k_scale, v_scale [b, hkv, nt]) in the layout of the FP8 attention (lv_attn_fp8_quant_kv;
+    e4m3 as float8_e4m3fn, one scale per 128-key block, each V block transposed with the key permutation of
+    csrc/attn_fp8_core.h)."""
+    _need_cuda_bf16(k, v)
+    if k.dim() != 4 or k.shape != v.shape:
+        raise ValueError(f"attn_fp8_quant_kv: k {tuple(k.shape)} and v {tuple(v.shape)} must both be [b, sk, hkv, d]")
+    kv_, vv = tma_view(k), tma_view(v)
+    p = attn_params(kv_, kv_, vv, kv_, causal=True)
+    return _attn_fp8_kv(p, k.device)[0]
+
+
+def _attn_fp8_kv(p: AttnParams, device):
+    """Quantise the K / V of the filled `p` (lv_attn_fp8_quant_kv) into new buffers; returns them and the AttnFp8Kv."""
+    b, sk, hkv, d = p.batch, p.sk, p.hkv, p.d
+    if d != 128:
+        raise ValueError(f"FP8 attention: head_dim {d} is not supported (128 only)")
+    nt = -(-sk // ATTN_FP8_BLOCK)
+    k8 = torch.empty((b, hkv, nt * ATTN_FP8_BLOCK, d), dtype=torch.uint8, device=device)
+    vt8 = torch.empty((b, hkv, nt, d, ATTN_FP8_BLOCK), dtype=torch.uint8, device=device)
+    ks = torch.empty((b, hkv, nt), dtype=torch.float32, device=device)
+    vs = torch.empty((b, hkv, nt), dtype=torch.float32, device=device)
+    f = AttnFp8Kv()
+    f.k8, f.vt8, f.k_scale, f.v_scale = k8.data_ptr(), vt8.data_ptr(), ks.data_ptr(), vs.data_ptr()
+    _call("lv_attn_fp8_quant_kv", C.byref(p), C.byref(f))
+    return (k8.view(FP8), vt8.view(FP8), ks, vs), f
+
+
+def attention_fwd_fp8(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, causal: bool = True,
+                      return_lse: bool = False, *, scale: Optional[float] = None, out: Optional[torch.Tensor] = None):
+    """Causal attention on the FP8 tensor cores (opt-in, lossy): q [b, sq, hq, 128], k / v [b, sk, hkv, 128] bf16
+    ("bshd" views, consumed in place as attention_fwd consumes them), sq <= sk, the mask aligned to the last key.
+    K and V are quantised into a temporary (attn_fp8_quant_kv, attn_fp8_kv_bytes), Q inside the kernel; the rule is
+    that of csrc/attn_fp8_core.h.  Returns out [b, sq, hq, 128] bf16, or (out, lse [b, hq, sq] float32).  Anything
+    else the FP8 kernel does not build (no causal mask, sq > sk, d != 128) is a ValueError before any launch; documents,
+    query segments and context parallelism have no FP8 path."""
+    _need_cuda_bf16(q, k, v)
+    if not causal:
+        raise ValueError("attention_fwd_fp8: only causal attention is built")
+    if q.dim() != 4 or k.dim() != 4 or k.shape != v.shape:
+        raise ValueError(f"attention_fwd_fp8: q {tuple(q.shape)}, k {tuple(k.shape)}, v {tuple(v.shape)} must be "
+                         "[b, s, h, d] with k and v alike")
+    b, sq, hq, d = q.shape
+    sk = k.shape[1]
+    if d != 128 or k.shape[0] != b or k.shape[3] != d or hq % k.shape[2] != 0:
+        raise ValueError(f"attention_fwd_fp8: head_dim 128 and hq a multiple of hkv needed, got q {tuple(q.shape)}, "
+                         f"k {tuple(k.shape)}")
+    if sq > sk:
+        raise ValueError(f"attention_fwd_fp8: sq={sq} > sk={sk} (the queries are the last sq rows of the keys)")
+    qv, kv_, vv = tma_view(q), tma_view(k), tma_view(v)
+    if out is None:
+        out = torch.empty(q.shape, dtype=torch.bfloat16, device=q.device)
+    lse = torch.empty((b, hq, sq), dtype=torch.float32, device=q.device) if return_lse else None
+    p = attn_params(qv, kv_, vv, out, lse, scale=scale, causal=True)
+    ev0 = _TIMER.start() if _TIMER is not None else None
+    bufs, f = _attn_fp8_kv(p, q.device)
+    _call("lv_attn_fwd_fp8", C.byref(p), C.byref(f))
+    del bufs                     # freed in stream order after the kernel
+    if ev0 is not None:
+        _TIMER.stop("attn_fwd_fp8", 4.0 * b * hq * d * (sq * (sk - sq) + sq * (sq + 1) / 2), ev0)
     return (out, lse) if return_lse else out
 
 
