@@ -508,6 +508,10 @@ def _fp8_attention_step(cache, rows: int):
     return attend
 
 
+PACKED_WITH_CACHE = ("packed samples (position ids restarting at 0) cannot be combined with a KV cache "
+                     "(use_cache / past_key_values / inference_params)")
+
+
 def packed_rows(position_ids: torch.Tensor, seq_len: int, device, *, cache=None, cp=None) -> Optional[torch.Tensor]:
     """cu_seqlens of a packed row (position ids restarting at 0 mark the sample boundaries; one host synchronisation),
     or None when the row holds one sample.  Packing under context parallelism (`cp`) or with a K/V cache raises."""
@@ -517,8 +521,7 @@ def packed_rows(position_ids: torch.Tensor, seq_len: int, device, *, cache=None,
             raise NotImplementedError("packed samples (position ids restarting at 0) under context parallelism are "
                                       "not supported")
         if cache is not None:
-            raise NotImplementedError("packed samples (position ids restarting at 0) cannot be combined with a KV cache "
-                                      "(use_cache / past_key_values / inference_params)")
+            raise NotImplementedError(PACKED_WITH_CACHE)
     return cu
 
 

@@ -11,6 +11,10 @@ once (`ops.attention_decode`).
 Duck-types the part of transformers' `Cache` the reference touches: `len(cache)` (`modeling_long_vita.py:90`)
 and `get_seq_length()` (:154).
 
+Rows appended by a forward pass are pending until it ends: `commit()` when one call runs every layer (run_layers),
+`commit_to(offset)` under Megatron's `--use-kv-cache` protocol, where each layer is a call of its own and
+`inference_params.sequence_len_offset` says how many tokens earlier forwards have written.
+
 A cache that does not fit in HBM beside the prefill is an `OffloadedKVCache`: its leading layers are the device
 buffers above, the others one pinned host buffer each, read in place by the decode kernel (`ops.attention_decode_host`).
 `make_cache` decides which, once, from the free device memory (`device_layers`).
@@ -61,8 +65,25 @@ class KVCache:
         self._len += self._pending
         self._pending = 0
 
+    def commit_to(self, offset: int) -> None:
+        _commit_to(self, offset)
+
     def bytes(self) -> int:
         return sum(t.numel() * t.element_size() for t in self.k + self.v)
+
+
+def _commit_to(cache, offset: int) -> None:
+    """Megatron's protocol: a forward starts with `offset` (inference_params.sequence_len_offset) tokens written by
+    earlier forwards, and Megatron advances the offset by the forward's length after it.  So an offset equal to the
+    committed length is this forward (its first layer, or a later one with rows pending), and an offset that moved by
+    exactly the pending rows starts the next forward: those rows are committed first.  Anything else (the offset moved
+    back, or past the pending rows) cannot come from that protocol and raises, with the cache unchanged."""
+    offset = int(offset)
+    if cache._pending and offset == cache._len + cache._pending:
+        cache.commit()
+    elif offset != cache._len:
+        raise ValueError(f"K/V cache: sequence_len_offset {offset} does not follow the cache ({cache._len} tokens "
+                         f"committed, {cache._pending} pending)")
 
 
 # Device memory a forward with a K/V cache leaves free beside the cache and the prefill's per-token working set: the
@@ -200,6 +221,9 @@ class OffloadedKVCache:
     def commit(self) -> None:
         self._len += self._pending
         self._pending = 0
+
+    def commit_to(self, offset: int) -> None:
+        _commit_to(self, offset)
 
     def bytes(self) -> int:
         """Device bytes of the cache."""

@@ -28,6 +28,15 @@ Packed samples (`--reset-attention-mask`): when the training loop has published 
 Inference takes the fused path (GEMM epilogues, in-place RoPE, fused add + norm).  When gradients are enabled and
 anything requires grad, `_forward_train` builds the same layer from differentiable pieces whose backward passes are
 kernels too (`lv_rmsnorm_bwd`, `lv_swiglu_bwd`, `lv_attn_bwd`, the GEMM on transposed operands).
+
+Megatron's `--use-kv-cache` generation (text_generation/generation.py:127-131: the prompt once, then one token per
+forward) passes `inference_params` (megatron-core 0.7 `InferenceParams`).  The layers then share one K/V cache per
+model, `key_value_memory_dict["b200_kv_cache"]`, made by the first layer of the first forward with
+`hf.modeling.new_cache` (on the device, or partly in pinned host memory when it does not fit), exactly as the
+Megatron-free `B200GPTVLModel` makes it.  Layer `layer_number` reads and writes its index `layer_number - 1`; the
+cache's length follows `sequence_len_offset` (kv_cache's `commit_to`), and RoPE takes the rows [offset, offset + s)
+of the `max_sequence_length`-row table Megatron passes.  The host tier's format is `config.kv_host_dtype` (absent:
+bf16; torch.float8_e4m3fn is the lossy FP8 one).
 """
 from __future__ import annotations
 
@@ -37,9 +46,9 @@ from typing import Optional
 
 import torch
 
-from .. import ops
-from ..hf.modeling import DecoderLayer, attention_step
-from .core_attention import megatron_cp_context, megatron_cu_seqlens, records_grad
+from .. import kv_cache, ops
+from ..hf.modeling import PACKED_WITH_CACHE, DecoderLayer, attention_step, new_cache
+from .core_attention import megatron_cp_context, megatron_cu_seqlens, megatron_packed_ends, records_grad
 
 
 class _Params(torch.nn.Module):
@@ -85,7 +94,7 @@ class B200TransformerLayer(torch.nn.Module):
         self._decoder = None
         self._decoder_stamp = None
         self._dims = types.SimpleNamespace(num_attention_heads=np_, num_key_value_heads=ng, head_dim=hn,
-                                           rms_norm_eps=self.eps)
+                                           rms_norm_eps=self.eps, hidden_size=h, intermediate_size=ffn)
         self._rope_cache = (None, None, None)
         if int(getattr(config, "tensor_model_parallel_size", 1) or 1) > 1:
             raise NotImplementedError("B200TransformerLayer holds whole weights: tensor_model_parallel_size must be 1 "
@@ -93,13 +102,18 @@ class B200TransformerLayer(torch.nn.Module):
         self.cp_size = int(getattr(config, "context_parallel_size", 1) or 1)
         self._cp_ctx = None
         self.cp_group = getattr(config, "cp_group", None)   # tests / Megatron-free callers may hand the group in
+        # the format of the host tier of a K/V cache this layer creates under inference_params (kv_cache.make_cache)
+        self.kv_host_dtype = kv_cache.check_host_dtype(getattr(config, "kv_host_dtype", torch.bfloat16))
+        # (parameter dict, name) of every parameter, for the stamp of _decoder_layer: looked up per call, so a
+        # re-assigned parameter is seen, without walking the submodules on every forward
+        self._param_slots = [(m._parameters, n) for m in self.modules() for n in m._parameters]
 
     def _decoder_layer(self) -> DecoderLayer:
         """The inference layer on this module's parameters: Megatron's grouped QKV rows [ng, (np/ng + 2), hn, h] become
         [all q | all k | all v] and fc1 = cat(gate, up) the interleaved SwiGLU operand.  The copies follow
         load_state_dict() / optimizer steps / .to(): every in-place update of a parameter bumps its `_version`, and a
         re-assigned `.data` or parameter changes `data_ptr()`."""
-        stamp = tuple((p._version, p.data_ptr()) for p in self.parameters())
+        stamp = tuple((d[n]._version, d[n].data_ptr()) for d, n in self._param_slots)
         if self._decoder is None or stamp != self._decoder_stamp:
             self._decoder = None               # free the stale copies before the new ones are made
             ng, hn, g = self.ng, self.hn, self.np // self.ng
@@ -123,26 +137,31 @@ class B200TransformerLayer(torch.nn.Module):
         self._cp_ctx = megatron_cp_context(self._cp_ctx, self.cp_size, s, self.np, self.ng, self.hn, device, self.cp_group)
         return self._cp_ctx
 
-    def _rope(self, rotary_pos_emb):
+    def _rope(self, rotary_pos_emb, holder=None):
         """Megatron hands the layer `freqs` [s, 1, 1, hn] fp32 (rotary_pos_embedding.py:84-122); the
-        cos / sin tables (bf16, cast as at :200-201) are cached per tensor."""
+        cos / sin tables (bf16, cast as at :200-201) are cached per tensor, in this layer or, under inference_params,
+        in `holder` (the key_value_memory_dict the layers share: Megatron builds one table per forward for all of
+        them)."""
         if isinstance(rotary_pos_emb, (tuple, list)):
             rotary_pos_emb = rotary_pos_emb[0]
-        key, cos, sin = self._rope_cache
+        key, cos, sin = self._rope_cache if holder is None else holder.get("b200_rope", (None, None, None))
         if key is not rotary_pos_emb:
             f = rotary_pos_emb.reshape(rotary_pos_emb.shape[0], -1).float()
             cos, sin = torch.cos(f).to(torch.bfloat16), torch.sin(f).to(torch.bfloat16)
-            self._rope_cache = (rotary_pos_emb, cos, sin)
+            if holder is None:
+                self._rope_cache = (rotary_pos_emb, cos, sin)
+            else:
+                holder["b200_rope"] = (rotary_pos_emb, cos, sin)
         return cos, sin
 
     def forward(self, hidden_states, attention_mask=None, context=None, context_mask=None, rotary_pos_emb=None,
                 inference_params=None, packed_seq_params=None):
         assert packed_seq_params is None, "Packed sequence is not supported by B200TransformerLayer."
-        if inference_params is not None:
-            raise NotImplementedError("KV-cache decode is outside this build's scope (prefill forward only)")
         s, b, h = hidden_states.shape
         if b != 1:
             raise NotImplementedError("micro-batch 1 (the reference's long-context setting)")
+        if inference_params is not None:
+            return self._forward_cached(hidden_states, rotary_pos_emb, inference_params), context
         if records_grad(hidden_states, *self.parameters()):
             return self._forward_train(hidden_states, rotary_pos_emb), context
         layer = self._decoder_layer()
@@ -157,6 +176,44 @@ class B200TransformerLayer(torch.nn.Module):
         out = x if d is None else ops.ls_residual(x, d)
         return out.view(s, b, h), context
 
+    def _forward_cached(self, hidden_states, rotary_pos_emb, ip):
+        """forward() under Megatron's `--use-kv-cache` protocol (see the module doc).  Every refusal is raised before
+        anything is launched."""
+        s, b, h = hidden_states.shape
+        if torch.is_grad_enabled() and records_grad(hidden_states, *self.parameters()):
+            raise NotImplementedError("inference_params (the K/V cache of generation) with gradients enabled: "
+                                      "training runs without it")
+        if self.cp_size > 1:
+            raise NotImplementedError("inference_params (--use-kv-cache) under context parallelism is not supported: "
+                                      "the sharded cache lives in cp.ContextParallelRunner")
+        if int(getattr(ip, "max_batch_size", 1) or 1) > 1:
+            raise NotImplementedError(f"inference_params.max_batch_size {ip.max_batch_size}: the K/V cache holds one "
+                                      "sequence (micro-batch 1)")
+        if megatron_packed_ends() is not None:
+            raise NotImplementedError(PACKED_WITH_CACHE)
+        offset = int(ip.sequence_len_offset)
+        if rotary_pos_emb is not None:
+            rows = (rotary_pos_emb[0] if isinstance(rotary_pos_emb, (tuple, list)) else rotary_pos_emb).shape[0]
+            if rows < offset + s:
+                raise ValueError(f"rotary_pos_emb has {rows} rows; the tokens at sequence_len_offset {offset} need "
+                                 f"{offset + s} (Megatron builds it for max_sequence_length positions)")
+        kv = ip.key_value_memory_dict
+        cache = kv.get("b200_kv_cache")
+        if cache is None:
+            capacity = int(getattr(ip, "max_sequence_length", 0) or (s + 1024))
+            cache = new_cache(self._dims, int(self.config.num_layers), capacity, s, hidden_states.device,
+                              self.kv_host_dtype)
+            kv["b200_kv_cache"] = cache
+        cache.commit_to(offset)
+        attend = partial(attention_step(cache, None, s), self.layer_number - 1)
+        layer = self._decoder_layer()
+        cos = sin = None
+        if rotary_pos_emb is not None:
+            cos, sin = self._rope(rotary_pos_emb, kv)
+            cos, sin = cos[offset : offset + s], sin[offset : offset + s]             # views: no table per layer
+        x, d = layer.forward(hidden_states.reshape(s, h), None, cos, sin, attend)
+        out = x if d is None else ops.ls_residual(x, d)
+        return out.view(s, b, h)
 
     # -- training: the same layer out of differentiable pieces (ops.*_autograd) --------------------------------
     def _forward_train(self, hidden_states, rotary_pos_emb):
