@@ -431,6 +431,26 @@ int lv_gemm_fp8(const void* A, const float* a_scale, const void* W, const float*
                 int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldw, int64_t ldc, int32_t act,
                 lv_stream_t stream);
 
+/* FP8 training of the decoder's linears (csrc/gemm_fp8.cu).  fmt: 0 = e4m3 (largest finite value 448), 1 = e5m2
+ * (57 344); both quantise with the rule of lv_quant_rows_fp8 and their own largest value (satfinite conversion).
+ * lv_quant_rows_fp8_fmt: lv_quant_rows_fp8 in either format (fmt 0 is lv_quant_rows_fp8).
+ * lv_quant_cols_fp8_t: cast-transpose.  x bf16 [R, C] (row stride ldx elements, a multiple of 8; C a multiple of 8)
+ * -> q [C, R16] contiguous, R16 = R rounded up to 16, with q[c, r] = x[r, c] quantised by the scale of column c,
+ * scale fp32 [C]; columns R..R16 of q are zero.  amax_ws is a workspace of C unsigned words.  x and q 16-byte aligned.
+ * lv_gemm_fp8_grad: the backward products.  C[M, N] = bf16((A . B^T) * a_scale[m] * b_scale[n]) with A [M, K] in
+ * format a_fmt and B e4m3 [N, K] (row strides lda / ldb bytes, multiples of 16), K-major, accumulation promoted out of
+ * the tensor cores every 128 k-values as in lv_gemm_fp8; C bf16 with row stride ldc (a multiple of 8).  With
+ * accumulate = 1, C is fp32 (ldc a multiple of 4) and each element becomes one IEEE round-to-nearest add
+ * C + (acc * a_scale[m]) * b_scale[n], the value whose bf16 rounding accumulate = 0 stores (Megatron's fp32
+ * main_grad, gradient-accumulation fusion).  K a multiple of 16, N of 8; A, B, C 16-byte aligned. */
+int lv_quant_rows_fp8_fmt(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, int32_t fmt,
+                          lv_stream_t stream);
+int lv_quant_cols_fp8_t(const void* x, void* q, float* scale, unsigned* amax_ws, int64_t R, int64_t C, int64_t ldx,
+                        int32_t fmt, lv_stream_t stream);
+int lv_gemm_fp8_grad(const void* A, int32_t a_fmt, const float* a_scale, const void* B, const float* b_scale, void* C,
+                     int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int32_t accumulate,
+                     lv_stream_t stream);
+
 /* Patch embedding of 14x14 non-overlapping patches (Conv2d(3, C, k=14, s=14),
  * modeling_intern_vit.py:79-81,98; intern_vit_model.py:139-145,203) + class token + learned
  * position embedding (modeling_intern_vit.py:100-107):

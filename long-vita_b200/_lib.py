@@ -130,6 +130,10 @@ SIGNATURES = {
     "lv_quant_rows_fp8": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr]),
     "lv_gemm_fp8": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32,
                             c_ptr]),
+    "lv_quant_rows_fp8_fmt": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i32, c_ptr]),
+    "lv_quant_cols_fp8_t": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i32, c_ptr]),
+    "lv_gemm_fp8_grad": (c_i32, [c_ptr, c_i32, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
+                                 c_i32, c_ptr]),
     "lv_patch_embed_ws_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i64]),
     "lv_patch_embed": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr]),
 }

@@ -47,12 +47,24 @@ __device__ __forceinline__ float fp8_out(float sum, float sa, float sw, float b)
   return __fmaf_rn(__fmul_rn(sum, sa), sw, b);
 }
 
+// One k32 step of a consumer: A e4m3 or (A_E5M2, a gradient of the backward products) e5m2; B e4m3.
+template <bool A_E5M2>
+__device__ __forceinline__ void fp8_mma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  if constexpr (A_E5M2)
+    wgmma_ss_n128_e5m2_e4m3(d, adesc, bdesc, accumulate);
+  else
+    wgmma_ss_n128_e4m3(d, adesc, bdesc, accumulate);
+}
+
 // act: 0 = none (bias optional), 3 = fused SwiGLU over interleaved (gate_i, up_i) W rows, no bias.
+// ACC selects the gradient-accumulation epilogue (lv_gemm_fp8_grad): accC[M, N] (fp32, row stride ldacc) +=
+// (sum * s_a) * s_w, the value whose bf16 rounding the plain epilogue stores; tmC, bias and act are then unused.
+template <bool A_E5M2, bool ACC>
 __global__ void __launch_bounds__(F_THREADS, 1)
     gemm_fp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                     const __grid_constant__ CUtensorMap tmC, const float* __restrict__ sa_g,
                     const float* __restrict__ sw_g, const __nv_bfloat16* __restrict__ bias, int M, int N, int K,
-                    int act, int gm) {
+                    int act, int gm, float* __restrict__ accC, long long ldacc) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
@@ -70,7 +82,7 @@ __global__ void __launch_bounds__(F_THREADS, 1)
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmC);
+    if constexpr (!ACC) tma_prefetch_desc(&tmC);
     for (int i = 0; i < F_STAGES; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 2);
@@ -130,14 +142,14 @@ __global__ void __launch_bounds__(F_THREADS, 1)
         // the unpromoted accumulation whose error tests/test_gpu_fp8_linear.py must tell apart
 #pragma unroll
         for (int kk = 0; kk < F_BK / 32; ++kk)
-          wgmma_ss_n128_e4m3(sum, adesc + 2 * kk, bdesc + 2 * kk, (kb | kk) != 0 ? 1u : 0u);
+          fp8_mma<A_E5M2>(sum, adesc + 2 * kk, bdesc + 2 * kk, (kb | kk) != 0 ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_keep(sum);
         if (wg_tid == 0) mbar_arrive(&empty[stage]);
 #else
 #pragma unroll
-        for (int kk = 0; kk < F_BK / 32; ++kk) wgmma_ss_n128_e4m3(acc, adesc + 2 * kk, bdesc + 2 * kk, kk != 0 ? 1u : 0u);
+        for (int kk = 0; kk < F_BK / 32; ++kk) fp8_mma<A_E5M2>(acc, adesc + 2 * kk, bdesc + 2 * kk, kk != 0 ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();
         wgmma_keep(acc);
@@ -155,6 +167,44 @@ __global__ void __launch_bounds__(F_THREADS, 1)
       // ------------------------------- epilogue -----------------------------------
       const int grow = mb * F_BM + cw * 64 + r_lo;
       const float sa0 = grow < M ? sa_g[grow] : 0.f, sa1 = grow + 8 < M ? sa_g[grow + 8] : 0.f;
+      if constexpr (ACC) {
+        // accC += value as a read-add-write from registers with one IEEE round-to-nearest add (add.rn.f32, subnormals
+        // kept), as the bf16 accumulate epilogue of gemm.cu does it; one writer per element, deterministic.  A quad's
+        // column pairs span one 32-byte sector per row.  Per 64-column chunk the 16 loads go before the adds.
+#pragma unroll
+        for (int c = 0; c < F_BN / 64; ++c) {
+          float2 prior[16];
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int col = nb * F_BN + 64 * c + 8 * jj + cq;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = grow + 8 * h;
+              prior[2 * jj + h] = make_float2(0.f, 0.f);
+              if (row < M && col < N) prior[2 * jj + h] = *reinterpret_cast<const float2*>(accC + row * ldacc + col);
+            }
+          }
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = c * 8 + jj;
+            const int col = nb * F_BN + 64 * c + 8 * jj + cq;
+            const float sw0 = col < N ? sw_g[col] : 0.f, sw1 = col + 1 < N ? sw_g[col + 1] : 0.f;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = grow + 8 * h;
+              if (row < M && col < N) {
+                const float sa = h ? sa1 : sa0;
+                float2 v = prior[2 * jj + h];
+                const float p0 = fp8_out(sum[4 * j + 2 * h], sa, sw0, 0.f), p1 = fp8_out(sum[4 * j + 2 * h + 1], sa, sw1, 0.f);
+                asm("add.rn.f32 %0, %0, %1;" : "+f"(v.x) : "f"(p0));
+                asm("add.rn.f32 %0, %0, %1;" : "+f"(v.y) : "f"(p1));
+                *reinterpret_cast<float2*>(accC + row * ldacc + col) = v;
+              }
+            }
+          }
+        }
+        continue;
+      }
       auto stage_begin = [&]() -> uint8_t* {
         uint8_t* stg = stg_base + (chunk_counter & 1) * F_C_BYTES;
         // the TMA store that last read this staging buffer (two chunks ago) must have drained
@@ -218,7 +268,9 @@ __global__ void __launch_bounds__(F_THREADS, 1)
         }
       }
     }
-    if (wg_tid == 0) tma_store_wait_all0();
+    if constexpr (!ACC) {
+      if (wg_tid == 0) tma_store_wait_all0();
+    }
   }
 }
 
@@ -230,6 +282,31 @@ __global__ void __launch_bounds__(F_THREADS, 1)
 // ---------------------------------------------------------------------------------------------
 constexpr int Q_THREADS = 256;
 
+// The two FP8 formats of the quantisers.  E5M2 (hybrid training's gradients) follows the rule of kv_fp8_core.h with
+// its own largest finite value: inv = 57344 / amax, q = e5m2_rn_satfinite(x * inv), scale = amax / 57344, a column or
+// row whose inv is not finite is zeros with scale 0.  The E4M3 members are exactly lv_kv8_inv / lv_kv8_scale /
+// lv_kv8_pack2, so the e4m3 instantiations compute what the e4m3-only kernels computed.
+constexpr float LV_E5M2_MAX = 57344.0f;
+
+template <bool E5M2>
+__device__ __forceinline__ float fp8_inv(float amax) {
+  return E5M2 ? __fdiv_rn(LV_E5M2_MAX, amax) : lv_kv8_inv(amax);
+}
+template <bool E5M2>
+__device__ __forceinline__ float fp8_scale(float amax) {
+  return E5M2 ? __fdiv_rn(amax, LV_E5M2_MAX) : lv_kv8_scale(amax);
+}
+template <bool E5M2>
+__device__ __forceinline__ uint16_t fp8_pack2(float lo, float hi) {
+  if constexpr (E5M2) {
+    uint16_t r;
+    asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+    return r;
+  } else {
+    return lv_kv8_pack2(lo, hi);
+  }
+}
+
 __device__ __forceinline__ void bf16x8(const uint4& v, float (&f)[8]) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -240,6 +317,7 @@ __device__ __forceinline__ void bf16x8(const uint4& v, float (&f)[8]) {
   }
 }
 
+template <bool E5M2>
 __global__ void __launch_bounds__(Q_THREADS)
     quant_rows_fp8_kernel(const __nv_bfloat16* __restrict__ X, uint8_t* __restrict__ Q, float* __restrict__ S, int K,
                           long long ldx) {
@@ -263,7 +341,7 @@ __global__ void __launch_bounds__(Q_THREADS)
   __syncthreads();
 #pragma unroll
   for (int w = 0; w < Q_THREADS / 32; ++w) amax = fmaxf(amax, warp_max[w]);
-  const float inv = lv_kv8_inv(amax);
+  const float inv = fp8_inv<E5M2>(amax);
   const bool zero = lv_kv8_zero_head(inv);
   for (int k = threadIdx.x * 16; k < K; k += Q_THREADS * 16) {
     uint32_t o[4] = {0u, 0u, 0u, 0u};
@@ -274,13 +352,104 @@ __global__ void __launch_bounds__(Q_THREADS)
         bf16x8(*reinterpret_cast<const uint4*>(x + k + 8 * h), f);
 #pragma unroll
         for (int i = 0; i < 2; ++i)
-          o[2 * h + i] = (uint32_t)lv_kv8_pack2(__fmul_rn(f[4 * i], inv), __fmul_rn(f[4 * i + 1], inv)) |
-                         ((uint32_t)lv_kv8_pack2(__fmul_rn(f[4 * i + 2], inv), __fmul_rn(f[4 * i + 3], inv)) << 16);
+          o[2 * h + i] = (uint32_t)fp8_pack2<E5M2>(__fmul_rn(f[4 * i], inv), __fmul_rn(f[4 * i + 1], inv)) |
+                         ((uint32_t)fp8_pack2<E5M2>(__fmul_rn(f[4 * i + 2], inv), __fmul_rn(f[4 * i + 3], inv)) << 16);
       }
     }
     *reinterpret_cast<uint4*>(q + k) = make_uint4(o[0], o[1], o[2], o[3]);
   }
-  if (threadIdx.x == 0) S[row] = zero ? 0.f : lv_kv8_scale(amax);
+  if (threadIdx.x == 0) S[row] = zero ? 0.f : fp8_scale<E5M2>(amax);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Cast-transpose (the backward operands): x bf16 [R, C] -> q [C, R16] with one scale per column of x (a row of q),
+// R16 = R rounded up to 16, columns R..R16 of q zero.  Two passes, both reading x with 16-byte loads along its rows:
+//   col_amax_kernel        per column max|x| over a band of CT_AMAX_ROWS rows, merged with atomicMax on the fp32 bits
+//                          (non-negative floats order as their bits; max is exact in any order)
+//   cast_transpose_kernel  a 128-row x 64-column tile per CTA: quantised as read, transposed through shared memory,
+//                          stored as 64 rows of 128 bytes with 16-byte stores.  A tile row c holds its eight 16-byte
+//                          chunks in the order chunk ^ (c / 8 % 8): a warp's byte stores (columns 8g + i of the
+//                          tile, g = 0..7) then fall on eight different banks instead of one
+// ---------------------------------------------------------------------------------------------
+constexpr int CT_R = 128, CT_C = 64, CT_THREADS = 256, CT_AMAX_ROWS = 256;
+
+__global__ void __launch_bounds__(CT_THREADS)
+    col_amax_kernel(const __nv_bfloat16* __restrict__ X, unsigned* __restrict__ amax_bits, int R, int C, long long ldx) {
+  // 32 threads x 8 columns across, 8 row lanes down
+  __shared__ float part[8][CT_THREADS];
+  const int cv = threadIdx.x & 31, rl = threadIdx.x >> 5;
+  const int c = (blockIdx.x * 32 + cv) * 8;
+  const int r_end = min(R, (int)(blockIdx.y + 1) * CT_AMAX_ROWS);
+  float m[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  if (c < C) {
+    for (int r = blockIdx.y * CT_AMAX_ROWS + rl; r < r_end; r += 8) {
+      float f[8];
+      bf16x8(*reinterpret_cast<const uint4*>(X + (long long)r * ldx + c), f);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) m[i] = fmaxf(m[i], fabsf(f[i]));
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) part[i][threadIdx.x] = m[i];
+  __syncthreads();
+  if (rl == 0 && c < C) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      float v = m[i];
+#pragma unroll
+      for (int l = 1; l < 8; ++l) v = fmaxf(v, part[i][l * 32 + cv]);
+      atomicMax(amax_bits + c + i, __float_as_uint(v));
+    }
+  }
+}
+
+template <bool E5M2>
+__global__ void __launch_bounds__(CT_THREADS)
+    cast_transpose_kernel(const __nv_bfloat16* __restrict__ X, const unsigned* __restrict__ amax_bits,
+                          uint8_t* __restrict__ Q, float* __restrict__ S, int R, int R16, int C, long long ldx) {
+  __shared__ __align__(16) uint8_t tile[CT_C][CT_R];   // [column of x][row of x, chunk-swizzled] = a row of q
+  const int r0 = blockIdx.x * CT_R, c0 = blockIdx.y * CT_C;
+  // read: 8 threads x 8 columns across a row, 32 rows per step
+  const int g = threadIdx.x & 7, rr = threadIdx.x >> 3;
+  const int c = c0 + 8 * g;
+  float inv[8];
+  bool zero[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float amax = c + i < C ? __uint_as_float(amax_bits[c + i]) : 0.f;
+    inv[i] = fp8_inv<E5M2>(amax);
+    zero[i] = lv_kv8_zero_head(inv[i]);
+  }
+  if (blockIdx.x == 0 && threadIdx.x < CT_C && c0 + threadIdx.x < C) {
+    const float amax = __uint_as_float(amax_bits[c0 + threadIdx.x]);
+    S[c0 + threadIdx.x] = lv_kv8_zero_head(fp8_inv<E5M2>(amax)) ? 0.f : fp8_scale<E5M2>(amax);
+  }
+#pragma unroll
+  for (int step = 0; step < CT_R / 32; ++step) {
+    const int lr = step * 32 + rr, r = r0 + lr;
+    uint8_t b[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (r < R && c < C) {
+      float f[8];
+      bf16x8(*reinterpret_cast<const uint4*>(X + (long long)r * ldx + c), f);
+#pragma unroll
+      for (int i = 0; i < 8; i += 2) {
+        const uint16_t p = fp8_pack2<E5M2>(__fmul_rn(f[i], inv[i]), __fmul_rn(f[i + 1], inv[i + 1]));
+        b[i] = zero[i] ? 0 : (uint8_t)(p & 0xFF);
+        b[i + 1] = zero[i + 1] ? 0 : (uint8_t)(p >> 8);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) tile[8 * g + i][(((lr >> 4) ^ g) << 4) | (lr & 15)] = b[i];
+  }
+  __syncthreads();
+  // write: 8 threads x 16 bytes along a row of q, 32 rows of q per step
+#pragma unroll
+  for (int step = 0; step < CT_C / 32; ++step) {
+    const int lc = step * 32 + rr, qc = c0 + lc, qr = r0 + 16 * g;
+    if (qc < C && qr < R16)
+      *reinterpret_cast<uint4*>(Q + (long long)qc * R16 + qr) =
+          *reinterpret_cast<const uint4*>(&tile[lc][(g ^ ((lc >> 3) & 7)) << 4]);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -415,7 +584,8 @@ static int launch_gemm_fp8(const void* A, const float* sa, const void* W, const 
   static PerDeviceOnce attr_once;
   int attr_dev;
   if (attr_once.needed(&attr_dev)) {
-    LV_CHECK_CUDA(cudaFuncSetAttribute(gemm_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F_SMEM));
+    LV_CHECK_CUDA(cudaFuncSetAttribute(gemm_fp8_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       F_SMEM));
     attr_once.done(attr_dev);
   }
   const int64_t tiles = ((M + F_BM - 1) / F_BM) * ((N + F_BN - 1) / F_BN);
@@ -423,8 +593,44 @@ static int launch_gemm_fp8(const void* A, const float* sa, const void* W, const 
   // M-blocks per rasterisation group, as in gemm.cu: the group's A panel (gm x 128 rows x K bytes) takes ~16 MB of L2
   int gm = (int)((16ll << 20) / (128 * K));
   gm = gm < 8 ? 8 : (gm > 64 ? 64 : gm);
-  gemm_fp8_kernel<<<grid, F_THREADS, F_SMEM, s>>>(tmA, tmB, tmC, sa, sw, reinterpret_cast<const __nv_bfloat16*>(bias),
-                                                  (int)M, (int)N, (int)K, act, gm);
+  gemm_fp8_kernel<false, false><<<grid, F_THREADS, F_SMEM, s>>>(
+      tmA, tmB, tmC, sa, sw, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M, (int)N, (int)K, act, gm, nullptr, 0ll);
+  LV_CHECK_LAUNCH("gemm_fp8_kernel");
+  return LV_OK;
+}
+
+// The backward products (lv_gemm_fp8_grad): gemm_fp8_kernel without bias or activation, A e4m3 or e5m2, C bf16 or
+// (ACC) fp32 accumulated into.
+template <bool A_E5M2, bool ACC>
+static int launch_gemm_fp8_grad(const void* A, const float* sa, const void* B, const float* sb, void* C, int64_t M,
+                                int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, cudaStream_t s) {
+  CUtensorMap tmA, tmB, tmC;
+  int r = encode_fp8_operand(&tmA, A, M, K, lda, F_BM);
+  if (r) return r;
+  r = encode_fp8_operand(&tmB, B, N, K, ldb, F_BN);
+  if (r) return r;
+  if constexpr (!ACC) {
+    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
+    const uint64_t str[2] = {2, (uint64_t)ldc * 2};
+    const uint32_t box[2] = {64, 64};
+    r = encode_tmap_bf16(&tmC, C, 2, dims, str, box, true);
+    if (r) return r;
+  } else {
+    memset(&tmC, 0, sizeof(tmC));
+  }
+  auto* const kernel = gemm_fp8_kernel<A_E5M2, ACC>;
+  static PerDeviceOnce attr_once;
+  int attr_dev;
+  if (attr_once.needed(&attr_dev)) {
+    LV_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F_SMEM));
+    attr_once.done(attr_dev);
+  }
+  const int64_t tiles = ((M + F_BM - 1) / F_BM) * ((N + F_BN - 1) / F_BN);
+  const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
+  int gm = (int)((16ll << 20) / (128 * K));
+  gm = gm < 8 ? 8 : (gm > 64 ? 64 : gm);
+  kernel<<<grid, F_THREADS, F_SMEM, s>>>(tmA, tmB, tmC, sa, sb, nullptr, (int)M, (int)N, (int)K, 0, gm,
+                                         ACC ? reinterpret_cast<float*>(C) : nullptr, ACC ? (long long)ldc : 0ll);
   LV_CHECK_LAUNCH("gemm_fp8_kernel");
   return LV_OK;
 }
@@ -456,7 +662,13 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 extern "C" {
 
 int lv_quant_rows_fp8(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, lv_stream_t stream) {
+  return lv_quant_rows_fp8_fmt(x, q, scale, M, K, ldx, 0, stream);
+}
+
+int lv_quant_rows_fp8_fmt(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, int32_t fmt,
+                          lv_stream_t stream) {
   LV_CHECK_ARG(x && q && scale, "lv_quant_rows_fp8: null pointer");
+  LV_CHECK_ARG(fmt == 0 || fmt == 1, "lv_quant_rows_fp8: format %d is not built (0 = e4m3, 1 = e5m2)", fmt);
   LV_CHECK_ARG(M >= 0 && K > 0 && K % 16 == 0 && M < (1ll << 31) && K < (1ll << 31),
                "lv_quant_rows_fp8: bad shape M=%lld K=%lld (K must be a positive multiple of 16)", (long long)M,
                (long long)K);
@@ -465,9 +677,38 @@ int lv_quant_rows_fp8(const void* x, void* q, float* scale, int64_t M, int64_t K
   LV_CHECK_ARG(aligned16(x) && aligned16(q), "lv_quant_rows_fp8: x and q must be 16-byte aligned");
   if (M == 0) return LV_OK;
   LV_BIND_DEVICE(x);
-  quant_rows_fp8_kernel<<<(unsigned)M, Q_THREADS, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x), reinterpret_cast<uint8_t*>(q), scale, (int)K, (long long)ldx);
+  auto* const kernel = fmt ? quant_rows_fp8_kernel<true> : quant_rows_fp8_kernel<false>;
+  kernel<<<(unsigned)M, Q_THREADS, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __nv_bfloat16*>(x),
+                                                              reinterpret_cast<uint8_t*>(q), scale, (int)K,
+                                                              (long long)ldx);
   LV_CHECK_LAUNCH("quant_rows_fp8_kernel");
+  return LV_OK;
+}
+
+int lv_quant_cols_fp8_t(const void* x, void* q, float* scale, unsigned* amax_ws, int64_t R, int64_t C, int64_t ldx,
+                        int32_t fmt, lv_stream_t stream) {
+  LV_CHECK_ARG(x && q && scale && amax_ws, "lv_quant_cols_fp8_t: null pointer");
+  LV_CHECK_ARG(fmt == 0 || fmt == 1, "lv_quant_cols_fp8_t: format %d is not built (0 = e4m3, 1 = e5m2)", fmt);
+  LV_CHECK_ARG(R >= 0 && C > 0 && C % 8 == 0 && R < (1ll << 31) - 16 && C < (1ll << 31),
+               "lv_quant_cols_fp8_t: bad shape R=%lld C=%lld (C must be a positive multiple of 8)", (long long)R,
+               (long long)C);
+  LV_CHECK_ARG(ldx % 8 == 0 && ldx >= C, "lv_quant_cols_fp8_t: ldx=%lld must be a multiple of 8 and >= C=%lld",
+               (long long)ldx, (long long)C);
+  LV_CHECK_ARG(aligned16(x) && aligned16(q), "lv_quant_cols_fp8_t: x and q must be 16-byte aligned");
+  LV_BIND_DEVICE(x);
+  const cudaStream_t s = (cudaStream_t)stream;
+  const int64_t R16 = (R + 15) / 16 * 16;
+  LV_CHECK_CUDA(cudaMemsetAsync(amax_ws, 0, C * sizeof(unsigned), s));
+  if (R > 0) {
+    col_amax_kernel<<<dim3((unsigned)((C + 255) / 256), (unsigned)((R + CT_AMAX_ROWS - 1) / CT_AMAX_ROWS)), CT_THREADS,
+                      0, s>>>(reinterpret_cast<const __nv_bfloat16*>(x), amax_ws, (int)R, (int)C, (long long)ldx);
+    LV_CHECK_LAUNCH("col_amax_kernel");
+  }
+  const dim3 grid((unsigned)((R16 + CT_R - 1) / CT_R > 0 ? (R16 + CT_R - 1) / CT_R : 1), (unsigned)((C + CT_C - 1) / CT_C));
+  auto* const kernel = fmt ? cast_transpose_kernel<true> : cast_transpose_kernel<false>;
+  kernel<<<grid, CT_THREADS, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(x), amax_ws, reinterpret_cast<uint8_t*>(q),
+                                     scale, (int)R, (int)R16, (int)C, (long long)ldx);
+  LV_CHECK_LAUNCH("cast_transpose_kernel");
   return LV_OK;
 }
 
@@ -496,6 +737,32 @@ int lv_gemm_fp8(const void* A, const float* a_scale, const void* W, const float*
   if (M <= 4 && (N + 255) / 256 < sm_count())
     return launch_gemv_fp8(A, a_scale, W, w_scale, bias, C, M, N, K, lda, ldw, ldc, act, s);
   return launch_gemm_fp8(A, a_scale, W, w_scale, bias, C, M, N, K, lda, ldw, ldc, act, s);
+}
+
+int lv_gemm_fp8_grad(const void* A, int32_t a_fmt, const float* a_scale, const void* B, const float* b_scale, void* C,
+                     int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int32_t accumulate,
+                     lv_stream_t stream) {
+  LV_CHECK_ARG(A && a_scale && B && b_scale && C, "lv_gemm_fp8_grad: null pointer");
+  LV_CHECK_ARG(a_fmt == 0 || a_fmt == 1, "lv_gemm_fp8_grad: A format %d is not built (0 = e4m3, 1 = e5m2)", a_fmt);
+  LV_CHECK_ARG(M >= 0 && N > 0 && K > 0 && M < (1ll << 31) && N < (1ll << 31) && K < (1ll << 31),
+               "lv_gemm_fp8_grad: bad shape M=%lld N=%lld K=%lld", (long long)M, (long long)N, (long long)K);
+  LV_CHECK_ARG(K % 16 == 0 && N % 8 == 0, "lv_gemm_fp8_grad: K=%lld must be a multiple of 16 and N=%lld of 8",
+               (long long)K, (long long)N);
+  LV_CHECK_ARG(lda % 16 == 0 && lda >= K && ldb % 16 == 0 && ldb >= K,
+               "lv_gemm_fp8_grad: lda=%lld and ldb=%lld must be multiples of 16 and >= K=%lld", (long long)lda,
+               (long long)ldb, (long long)K);
+  LV_CHECK_ARG(ldc % (accumulate ? 4 : 8) == 0 && ldc >= N,
+               "lv_gemm_fp8_grad: ldc=%lld must be a multiple of %d and >= N=%lld", (long long)ldc, accumulate ? 4 : 8,
+               (long long)N);
+  LV_CHECK_ARG(aligned16(A) && aligned16(B) && aligned16(C), "lv_gemm_fp8_grad: A, B and C must be 16-byte aligned");
+  if (M == 0) return LV_OK;
+  LV_BIND_DEVICE(A);
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (accumulate)
+    return a_fmt ? launch_gemm_fp8_grad<true, true>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s)
+                 : launch_gemm_fp8_grad<false, true>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s);
+  return a_fmt ? launch_gemm_fp8_grad<true, false>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s)
+               : launch_gemm_fp8_grad<false, false>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s);
 }
 
 }  // extern "C"

@@ -37,6 +37,16 @@ Megatron-free `B200GPTVLModel` makes it.  Layer `layer_number` reads and writes 
 cache's length follows `sequence_len_offset` (kv_cache's `commit_to`), and RoPE takes the rows [offset, offset + s)
 of the `max_sequence_length`-row table Megatron passes.  The host tier's format is `config.kv_host_dtype` (absent:
 bf16; torch.float8_e4m3fn is the lossy FP8 one).
+
+FP8 (`--fp8-format e4m3|hybrid`, `config.fp8` = "e4m3" / "hybrid"; opt-in, lossy): every forward runs the four linears
+(linear_qkv, linear_proj, linear_fc1, linear_fc2) in FP8, as TransformerEngine's fp8_autocast does around the
+reference's layers.  Inference and `--use-kv-cache` decode use `DecoderLayer(linear_dtype=torch.float8_e4m3fn)`;
+`_forward_train` uses `ops.linear_fp8_autograd`, with e4m3 gradients for "e4m3" and e5m2 gradients for "hybrid", and
+dW in bf16 when `config.fp8_wgrad` is False.  Attention, the norms, RoPE, SwiGLU and the fp32 `main_grad` stay bf16 /
+fp32.  Scales are current scales, computed from the tensor being quantised, so TransformerEngine's delayed-scaling
+fields (fp8_margin, fp8_interval, fp8_amax_history_len, fp8_amax_compute_algo) have nothing to act on and are ignored.
+fp8_dot_product_attention / fp8_multi_head_attention are refused (NotImplementedError), any other `fp8` value is a
+ValueError, both when the layer is built.  `config.fp8` absent or None: the bf16 layer, unchanged.
 """
 from __future__ import annotations
 
@@ -49,6 +59,14 @@ import torch
 from .. import kv_cache, ops
 from ..hf.modeling import PACKED_WITH_CACHE, DecoderLayer, attention_step, new_cache
 from .core_attention import megatron_cp_context, megatron_cu_seqlens, megatron_packed_ends, records_grad
+
+
+# config.fp8 (Megatron's --fp8-format) -> the format of the gradients in the FP8 backward products
+FP8_GRAD_DTYPE = {"e4m3": torch.float8_e4m3fn, "hybrid": torch.float8_e5m2}
+
+
+def _linear_fp8(x, weight, bias, accumulate_wgrad, *, grad_dtype, fp8_wgrad):
+    return ops.linear_fp8_autograd(x, weight, bias, grad_dtype, fp8_wgrad, accumulate_wgrad)
 
 
 class _Params(torch.nn.Module):
@@ -104,6 +122,15 @@ class B200TransformerLayer(torch.nn.Module):
         self.cp_group = getattr(config, "cp_group", None)   # tests / Megatron-free callers may hand the group in
         # the format of the host tier of a K/V cache this layer creates under inference_params (kv_cache.make_cache)
         self.kv_host_dtype = kv_cache.check_host_dtype(getattr(config, "kv_host_dtype", torch.bfloat16))
+        self.fp8 = getattr(config, "fp8", None)
+        if self.fp8 is not None:
+            if self.fp8 not in FP8_GRAD_DTYPE:
+                raise ValueError(f"config.fp8 must be None, 'e4m3' or 'hybrid', got {self.fp8!r}")
+            for name in ("fp8_dot_product_attention", "fp8_multi_head_attention"):
+                if getattr(config, name, False):
+                    raise NotImplementedError(f"config.{name}: attention runs in bf16 under config.fp8 (only the "
+                                              "linears are FP8)")
+        self.fp8_wgrad = bool(getattr(config, "fp8_wgrad", True))
         # (parameter dict, name) of every parameter, for the stamp of _decoder_layer: looked up per call, so a
         # re-assigned parameter is seen, without walking the submodules on every forward
         self._param_slots = [(m._parameters, n) for m in self.modules() for n in m._parameters]
@@ -130,7 +157,8 @@ class B200TransformerLayer(torch.nn.Module):
             for name, rows in (("q_proj", slice(0, g)), ("k_proj", g), ("v_proj", g + 1)):
                 hf[p + f"self_attn.{name}.weight"] = w[:, rows].reshape(-1, w.shape[-1])
                 hf[p + f"self_attn.{name}.bias"] = b[:, rows].reshape(-1)
-            self._decoder, self._decoder_stamp = DecoderLayer(self._dims, hf, 0), stamp
+            dtype = torch.bfloat16 if self.fp8 is None else torch.float8_e4m3fn
+            self._decoder, self._decoder_stamp = DecoderLayer(self._dims, hf, 0, dtype), stamp
         return self._decoder
 
     def _cp(self, s: int, device):
@@ -224,16 +252,23 @@ class B200TransformerLayer(torch.nn.Module):
         used here (the un-fused gate|up activation is what the SwiGLU backward needs).
 
         `config.gradient_accumulation_fusion` (absent: off) adds the four weight gradients to each weight's fp32
-        `main_grad` inside the GEMM, as Megatron's linears do (ops.linear_autograd, accumulate_wgrad)."""
+        `main_grad` inside the GEMM, as Megatron's linears do (ops.linear_autograd, accumulate_wgrad).
+
+        With `config.fp8` the four linears are ops.linear_fp8_autograd (see the module doc); nothing else changes."""
         s, b, h = hidden_states.shape
         np_, ng, hn = self.np, self.ng, self.hn
         g = np_ // ng
         self._decoder = None               # the re-ordered inference copies go stale once the parameters train
         fuse = bool(getattr(self.config, "gradient_accumulation_fusion", False))
+        linear = ops.linear_autograd
+        if self.fp8 is not None:
+            # the weights are quantised by every forward (W) and backward (W^T), from their current values: Megatron's
+            # optimizers write updated weights into .data, which moves neither _version nor data_ptr
+            linear = partial(_linear_fp8, grad_dtype=FP8_GRAD_DTYPE[self.fp8], fp8_wgrad=self.fp8_wgrad)
         x = hidden_states.reshape(s, h)
         a = self.self_attention
         hcur = ops.rmsnorm_autograd(x, a.linear_qkv.layer_norm_weight, self.eps)
-        qkv = ops.linear_autograd(hcur, a.linear_qkv.weight, a.linear_qkv.bias, fuse).view(s, ng, g + 2, hn)
+        qkv = linear(hcur, a.linear_qkv.weight, a.linear_qkv.bias, fuse).view(s, ng, g + 2, hn)
         q = qkv[:, :, :g].reshape(s, np_, hn)
         k = qkv[:, :, g].contiguous()
         v = qkv[:, :, g + 1].contiguous()
@@ -249,10 +284,10 @@ class B200TransformerLayer(torch.nn.Module):
         else:
             att = ops.attention(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True,
                                 **ops.docs_kwargs(megatron_cu_seqlens(s, hidden_states.device)))    # [1, s, np, hn]
-        o = ops.linear_autograd(att.reshape(s, np_ * hn), a.linear_proj.weight, None, fuse)
+        o = linear(att.reshape(s, np_ * hn), a.linear_proj.weight, None, fuse)
         hcur, x = ops.rmsnorm_autograd(o, self.mlp.linear_fc1.layer_norm_weight, self.eps, residual=x)
-        gate_up = ops.linear_autograd(hcur, self.mlp.linear_fc1.weight, None, fuse)             # cat(gate, up)
-        d = ops.linear_autograd(ops.swiglu_autograd(gate_up), self.mlp.linear_fc2.weight, None, fuse)
+        gate_up = linear(hcur, self.mlp.linear_fc1.weight, None, fuse)             # cat(gate, up)
+        d = linear(ops.swiglu_autograd(gate_up), self.mlp.linear_fc2.weight, None, fuse)
         return (x + d).view(s, b, h)
 
 

@@ -880,13 +880,24 @@ def linear(x: torch.Tensor, weight, bias: Optional[torch.Tensor] = None, act: Op
 # FP8 (e4m3) linears: per-row scales on both operands (csrc/kv_fp8_core.h), lv_gemm_fp8
 # ------------------------------------------------------------------------------------------------
 FP8 = torch.float8_e4m3fn
+FP8_E5M2 = torch.float8_e5m2
+_FP8_FMT = {FP8: 0, FP8_E5M2: 1}            # the `fmt` argument of the C entry points
+FP8_MAX = {FP8: 448.0, FP8_E5M2: 57344.0}   # largest finite value of each format
 
 
-def quant_rows_fp8(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    """x bf16 [M, K] (K contiguous, K a multiple of 16, row stride a multiple of 8) -> (q e4m3 [M, K], scale fp32
-    [M]): one scale per row, amax / 448, q = e4m3(x * 448 / amax); a row of zeros (or too small to scale) is zeros
-    with scale 0 (lv_quant_rows_fp8).  x ~ q.float() * scale[:, None]."""
+def _fp8_fmt(op: str, dtype) -> int:
+    if dtype not in _FP8_FMT:
+        raise ValueError(f"{op}: dtype must be torch.float8_e4m3fn or torch.float8_e5m2, got {dtype!r}")
+    return _FP8_FMT[dtype]
+
+
+def quant_rows_fp8(x: torch.Tensor, dtype: torch.dtype = FP8) -> Tuple[torch.Tensor, torch.Tensor]:
+    """x bf16 [M, K] (K contiguous, K a multiple of 16, row stride a multiple of 8) -> (q [M, K] of `dtype`, scale
+    fp32 [M]): one scale per row, amax / max, q = fp8(x * max / amax) saturating at max, where max is 448 for e4m3 (the
+    default) and 57 344 for e5m2; a row of zeros (or too small to scale) is zeros with scale 0
+    (lv_quant_rows_fp8_fmt).  x ~ q.float() * scale[:, None]."""
     _need_cuda_bf16(x)
+    fmt = _fp8_fmt("quant_rows_fp8", dtype)
     if x.dim() != 2:
         raise ValueError(f"quant_rows_fp8: x must be [M, K], got {tuple(x.shape)}")
     M, K = x.shape
@@ -894,10 +905,35 @@ def quant_rows_fp8(x: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         raise ValueError(f"quant_rows_fp8: K={K} must be a positive multiple of 16")
     if x.stride(1) != 1 or x.stride(0) % 8 or x.data_ptr() % 16:
         x = x.contiguous()
-    q = torch.empty((M, K), dtype=FP8, device=x.device)
+    q = torch.empty((M, K), dtype=dtype, device=x.device)
     scale = torch.empty((M,), dtype=torch.float32, device=x.device)
-    if M:
+    if M and fmt == 0:
         _call("lv_quant_rows_fp8", x.data_ptr(), q.data_ptr(), scale.data_ptr(), M, K, max(x.stride(0), K))
+    elif M:
+        _call("lv_quant_rows_fp8_fmt", x.data_ptr(), q.data_ptr(), scale.data_ptr(), M, K, max(x.stride(0), K), fmt)
+    return q, scale
+
+
+def quant_cols_fp8_t(x: torch.Tensor, dtype: torch.dtype = FP8) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Cast-transpose: x bf16 [R, C] (C contiguous, C a multiple of 8, row stride a multiple of 8) -> (q [C, R16] of
+    `dtype`, scale fp32 [C]) with q[c, r] = x[r, c] quantised by the scale of column c (the rule of quant_rows_fp8
+    applied to each column) and R16 = R rounded up to 16, columns R..R16 of q being zero, so that q is a K-major
+    operand of the FP8 GEMM with the R rows of x as its contraction (lv_quant_cols_fp8_t).
+    x ~ (q.float() * scale[:, None]).t()[:R]."""
+    _need_cuda_bf16(x)
+    fmt = _fp8_fmt("quant_cols_fp8_t", dtype)
+    if x.dim() != 2:
+        raise ValueError(f"quant_cols_fp8_t: x must be [R, C], got {tuple(x.shape)}")
+    R, Cn = x.shape
+    if Cn == 0 or Cn % 8:
+        raise ValueError(f"quant_cols_fp8_t: C={Cn} must be a positive multiple of 8")
+    if x.stride(1) != 1 or (R > 1 and x.stride(0) % 8) or x.data_ptr() % 16:
+        x = x.contiguous()
+    q = torch.empty((Cn, -(-R // 16) * 16), dtype=dtype, device=x.device)
+    scale = torch.empty((Cn,), dtype=torch.float32, device=x.device)
+    amax_ws = torch.empty((Cn,), dtype=torch.int32, device=x.device)
+    _call("lv_quant_cols_fp8_t", x.data_ptr(), q.data_ptr(), scale.data_ptr(), amax_ws.data_ptr(), R, Cn,
+          x.stride(0) if R > 1 else Cn, fmt)
     return q, scale
 
 
@@ -1002,6 +1038,157 @@ def linear_fp8(x: torch.Tensor, weight: Fp8Weight, bias: Optional[torch.Tensor] 
     if ev0 is not None:
         _TIMER.stop("gemm_fp8", 2.0 * M * N * K, ev0)
     return out.view(*x.shape[:-1], n_out)
+
+
+# ------------------------------------------------------------------------------------------------
+# FP8 training of a linear: backward products on lv_gemm_fp8_grad.  Both operands of every product are K-major with
+# one scale per row (FP8 wgmma reads nothing else), so each backward operand is an FP8 copy quantised along the axis
+# the product reduces over:
+#   forward  Y  [T, N] = X [T, K] . W [N, K]^T      X per token (row),      W per output channel (row)
+#   dgrad    dX [T, K] = dY [T, N] . (W^T) [K, N]^T  dY per token (row),     W^T per input channel (quant_cols_fp8_t)
+#   wgrad    dW [N, K] = (dY^T) [N, T] . (X^T) [K, T]^T   dY^T per output channel, X^T per input channel
+#                                                        (both quant_cols_fp8_t, T padded to 16 with zeros)
+# ------------------------------------------------------------------------------------------------
+def _gemm_fp8_grad(op: str, a: torch.Tensor, sa: torch.Tensor, b: torch.Tensor, sb: torch.Tensor, out: torch.Tensor,
+                   accumulate: bool) -> torch.Tensor:
+    """out [M, N] (bf16; fp32 added into with `accumulate`) from A [M, K] (e4m3 / e5m2) and B [N, K] (e4m3), both
+    K-major with 16-byte aligned rows (lv_gemm_fp8_grad)."""
+    (M, K), N = a.shape, b.shape[0]
+    if b.dtype != FP8 or a.dtype not in _FP8_FMT or b.shape[1] != K or sa.shape != (M,) or sb.shape != (N,):
+        raise ValueError(f"{op}: operands {a.dtype} {tuple(a.shape)} and {b.dtype} {tuple(b.shape)} (scales "
+                         f"{tuple(sa.shape)}, {tuple(sb.shape)}) are not FP8 [M, K], e4m3 [N, K] with one scale per row")
+    for t in (a, b):
+        if t.stride(1) != 1 or (t.shape[0] > 1 and t.stride(0) % 16) or t.data_ptr() % 16:
+            raise ValueError(f"{op}: FP8 operand strides {t.stride()} are not 16-byte aligned rows")
+    if M == 0:
+        return out
+    ev0 = _TIMER.start() if _TIMER is not None else None
+    _call("lv_gemm_fp8_grad", a.data_ptr(), _FP8_FMT[a.dtype], sa.data_ptr(), b.data_ptr(), sb.data_ptr(),
+          out.data_ptr(), M, N, K, a.stride(0) if M > 1 else K, b.stride(0) if N > 1 else K, out.stride(0),
+          int(accumulate))
+    if ev0 is not None:
+        _TIMER.stop("gemm_fp8", 2.0 * M * N * K, ev0)
+    return out
+
+
+def linear_fp8_dgrad(dy: torch.Tensor, weight_t: "Fp8Weight", dtype: torch.dtype = FP8) -> torch.Tensor:
+    """dX [..., K] = dY [..., N] . W [N, K] in FP8: dY bf16 quantised per token in `dtype` (quant_rows_fp8), weight_t
+    = Fp8Weight(*quant_cols_fp8_t(W)), the e4m3 [K, N] copy of W scaled per input channel.  N a multiple of 16.
+    Returns bf16."""
+    _need_cuda_bf16(dy)
+    N = dy.shape[-1]
+    if N % 16 or weight_t.shape[1] != N:
+        raise ValueError(f"linear_fp8_dgrad: dY [..., {N}] and W^T {tuple(weight_t.shape)} are not [.., N], [K, N] "
+                         "with N a multiple of 16")
+    dq, ds = quant_rows_fp8(dy.reshape(-1, N), dtype)
+    dx = torch.empty((dq.shape[0], weight_t.shape[0]), dtype=torch.bfloat16, device=dy.device)
+    _gemm_fp8_grad("linear_fp8_dgrad", dq, ds, weight_t.data, weight_t.scale, dx, False)
+    return dx.view(*dy.shape[:-1], weight_t.shape[0])
+
+
+def _wgrad_operands(op: str, dy2: torch.Tensor, x_t, dtype):
+    _need_cuda_bf16(dy2)
+    T, N = dy2.shape
+    xq, xs = x_t
+    if xq.dim() != 2 or xq.shape[1] != -(-T // 16) * 16:
+        raise ValueError(f"{op}: X^T {tuple(xq.shape)} is not the [K, {-(-T // 16) * 16}] cast-transpose of {T} tokens")
+    dq, ds = quant_cols_fp8_t(dy2, dtype)
+    return dq, ds, xq, xs
+
+
+def linear_fp8_wgrad(dy2: torch.Tensor, x_t: Tuple[torch.Tensor, torch.Tensor],
+                     dtype: torch.dtype = FP8) -> torch.Tensor:
+    """dW [N, K] = dY^T [N, T] . X [T, K] in FP8, the token dimension T being the contraction: dY bf16 [T, N] is
+    cast-transposed in `dtype` (quant_cols_fp8_t), x_t = quant_cols_fp8_t(X) (e4m3 [K, T16], scale [K]) is X^T.
+    Without tokens dW is zero and nothing is launched.  Returns bf16."""
+    T, N = dy2.shape
+    if T == 0:
+        return torch.zeros((N, x_t[0].shape[0]), dtype=torch.bfloat16, device=dy2.device)
+    dq, ds, xq, xs = _wgrad_operands("linear_fp8_wgrad", dy2, x_t, dtype)
+    dw = torch.empty((N, xq.shape[0]), dtype=torch.bfloat16, device=dy2.device)
+    return _gemm_fp8_grad("linear_fp8_wgrad", dq, ds, xq, xs, dw, False)
+
+
+def linear_fp8_wgrad_accumulate(dy2: torch.Tensor, x_t: Tuple[torch.Tensor, torch.Tensor], main_grad: torch.Tensor,
+                                dtype: torch.dtype = FP8) -> torch.Tensor:
+    """main_grad [N, K] fp32 += the product of linear_fp8_wgrad, in place: each element gets one fp32 add of the value
+    whose bf16 rounding linear_fp8_wgrad returns.  main_grad: unit column stride, a row stride that is a multiple of 4,
+    16-byte aligned (as linear_wgrad_accumulate).  Without tokens nothing is launched.  Returns main_grad."""
+    _need_cuda(main_grad, torch.float32)
+    T, N = dy2.shape
+    if tuple(main_grad.shape) != (N, x_t[0].shape[0]):
+        raise RuntimeError(f"linear_fp8_wgrad_accumulate: main_grad is {tuple(main_grad.shape)}, the weight gradient "
+                           f"is [{N}, {x_t[0].shape[0]}]")
+    if main_grad.stride(1) != 1 or main_grad.stride(0) % 4 != 0 or main_grad.data_ptr() % 16 != 0:
+        raise RuntimeError(f"linear_fp8_wgrad_accumulate: main_grad (strides {main_grad.stride()}) must have unit "
+                           "column stride, a row stride that is a multiple of 4 and a 16-byte aligned start")
+    if T == 0:
+        return main_grad
+    dq, ds, xq, xs = _wgrad_operands("linear_fp8_wgrad_accumulate", dy2, x_t, dtype)
+    return _gemm_fp8_grad("linear_fp8_wgrad_accumulate", dq, ds, xq, xs, main_grad, True)
+
+
+class _LinearFp8Fn(torch.autograd.Function):
+    """y = x W^T + b in FP8 (linear_fp8 on W quantised per output channel), with the backward of _LinearFn in FP8: dX
+    by linear_fp8_dgrad on W^T quantised per input channel, dW by linear_fp8_wgrad[_accumulate], gradients quantised
+    in `grad_dtype`.  Both copies of W are made from the weight as it is when they are needed - W in the forward, W^T
+    in the backward - so whatever writes the weight between steps (an optimizer copying into .data included) is seen,
+    and no FP8 weight copy outlives its product.  The forward keeps only X^T in e4m3 with its scales for dW (one byte
+    per element), or, without fp8_wgrad, X in bf16 for the bf16 wgrad."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, grad_dtype, fp8_wgrad, accumulate_wgrad):
+        K = x.shape[-1]
+        ctx.grad_dtype, ctx.fp8_wgrad = grad_dtype, fp8_wgrad
+        ctx.has_bias, ctx.accumulate_wgrad, ctx.x_shape = bias is not None, accumulate_wgrad, x.shape
+        ctx.weight = weight
+        if not ctx.needs_input_grad[1]:
+            ctx.save_for_backward()
+        elif fp8_wgrad:
+            ctx.save_for_backward(*quant_cols_fp8_t(x.reshape(-1, K)))
+        else:
+            ctx.save_for_backward(x)
+        return linear_fp8(x, Fp8Weight.quantize(weight.detach()), bias)
+
+    @staticmethod
+    def backward(ctx, dy):
+        weight = ctx.weight
+        n_out, k_in = weight.shape
+        dy2 = dy.reshape(-1, n_out).contiguous()
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            w_t = Fp8Weight(*quant_cols_fp8_t(weight.detach()))
+            dx = linear_fp8_dgrad(dy2, w_t, ctx.grad_dtype).view(ctx.x_shape)
+        if ctx.needs_input_grad[1]:
+            saved = ctx.saved_tensors
+            main_grad = fused_wgrad_main_grad(weight) if ctx.accumulate_wgrad else None
+            if ctx.fp8_wgrad:
+                if main_grad is None:
+                    dw = linear_fp8_wgrad(dy2, saved, ctx.grad_dtype)
+                else:
+                    linear_fp8_wgrad_accumulate(dy2, saved, main_grad, ctx.grad_dtype)
+            else:
+                x2 = saved[0].reshape(-1, k_in)
+                if main_grad is None:
+                    dw = linear_wgrad(dy2, x2)
+                else:
+                    linear_wgrad_accumulate(dy2, x2, main_grad)
+            if main_grad is not None:
+                dw = fused_wgrad_dummy(weight, main_grad, dy2.dtype)
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            db = dy2.float().sum(dim=0).to(dy2.dtype)
+        return dx, dw, db, None, None, None
+
+
+def linear_fp8_autograd(x, weight, bias=None, grad_dtype: torch.dtype = FP8, fp8_wgrad: bool = True,
+                        accumulate_wgrad: bool = False):
+    """Differentiable FP8 linear (see _LinearFp8Fn): weight is the bf16 parameter [N, K] (N a multiple of 16: dgrad's
+    contraction) that receives the gradient.  Scales are current scales, computed from the tensor being quantised.
+    accumulate_wgrad: as linear_autograd."""
+    _fp8_fmt("linear_fp8_autograd", grad_dtype)
+    if weight.dim() != 2 or weight.shape[0] % 16:
+        raise ValueError(f"linear_fp8_autograd: weight {tuple(weight.shape)} must be [N, K] with N a multiple of 16")
+    return _LinearFp8Fn.apply(x, weight, bias, grad_dtype, bool(fp8_wgrad), bool(accumulate_wgrad))
 
 
 def interleave_gate_up(gate_w: torch.Tensor, up_w: torch.Tensor) -> torch.Tensor:
