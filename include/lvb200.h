@@ -137,6 +137,13 @@ typedef struct lv_attn_docs {
 int lv_attn_docs_fwd(const lv_attn_params* a, const lv_attn_docs* docs, lv_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * The FP8 row rule (csrc/fp8_core.h), which every FP8 entry point below quantises with.  fmt: 0 = e4m3 (largest
+ * finite value M = 448), 1 = e5m2 (M = 57344).  A row of values x is quantised in fp32: amax = max|x|,
+ * inv = M / amax, q = fp8_rn_satfinite(x * inv), scale = amax / M, read back as q * scale; a row whose inv is not
+ * finite (amax = 0, or a bf16 subnormal amax) is zero bytes and scale 0.
+ * ------------------------------------------------------------------------------------------ */
+
+/* ------------------------------------------------------------------------------------------
  * FP8 (e4m3) attention forward (opt-in, lossy; csrc/attn_fwd_fp8.cu, rule in csrc/attn_fp8_core.h): causal
  * attention on the FP8 tensor cores with K and V quantised once per call.
  *
@@ -145,8 +152,7 @@ int lv_attn_docs_fwd(const lv_attn_params* a, const lv_attn_docs* docs, lv_strea
  *   vt8      e4m3 [b][hkv][nt][d][128]    each block of values transposed; inside each 32-key chunk, byte
  *                                         32 c + 16 h + 4 t + i of a row holds key 32 c + 16 h + 8 (i / 2) + 2 t + i % 2
  *   k_scale, v_scale  float [b][hkv][nt]
- * A block's values x are quantised as one row of the host tier's rule: amax = max|x|, q = e4m3_rn_satfinite(x * (448 /
- * amax)), scale = amax / 448, zero bytes and scale 0 when 448 / amax is not finite.
+ * A block's values are quantised as one e4m3 row of the FP8 row rule.
  *
  * lv_attn_fp8_quant_kv: bf16 K and V of `a` (a->k, a->v, batch, sk, hkv, d, k_strides, v_strides; the other fields
  *   are not read) -> the four buffers of `kv`, one pass.  d = 128; k, v, k8, vt8 16-byte aligned.
@@ -361,10 +367,8 @@ int lv_rows_to_host(void* host_dst, const void* src, int64_t rows, int64_t row_b
 
 /* FP8 host tier (opt-in, lossy: it halves the PCIe bytes and the pinned memory of a host layer).  A row holds K of
  * the hkv heads, e4m3 [hkv][d]; V of the hkv heads, e4m3 [hkv][d]; then the scales, float [2][hkv] (K scales, then V
- * scales), zero-padded to a multiple of 16 bytes: 2 * hkv * d + ceil(8 * hkv / 16) * 16 bytes, 2112 at 8:128.  One
- * head's values x are quantised in fp32: amax = max|x|, inv = 448 / amax, q = e4m3_rn_satfinite(x * inv),
- * scale = amax / 448, read back as q * scale; a head whose inv is not finite (amax = 0, or a bf16 subnormal amax below
- * ~1.3e-36) is zero bytes and scale 0 (csrc/kv_fp8_core.h).
+ * scales), zero-padded to a multiple of 16 bytes: 2 * hkv * d + ceil(8 * hkv / 16) * 16 bytes, 2112 at 8:128.  Each
+ * head is one e4m3 row of the FP8 row rule.
  *
  * lv_rows_to_host_fp8: quantise `rows` bf16 K|V rows of the device (2 * hkv * d values each, V following K, src_pitch
  * bytes apart: the K|V columns of a QKV buffer row or the streamed layer's K|V buffer) into contiguous FP8 host rows,
@@ -416,24 +420,22 @@ int lv_gemm_ex(const void* A, const void* W, const void* bias, void* C, int64_t 
 int lv_gemm_wgrad_acc_f32(const void* A, const void* W, float* C, int64_t M, int64_t N, int64_t K, int64_t lda,
                           int64_t ldw, int64_t ldc, int32_t a_mn_major, int32_t w_mn_major, lv_stream_t stream);
 
-/* FP8 (e4m3) linears of the decoder (csrc/gemm_fp8.cu; the rule of csrc/kv_fp8_core.h applied to whole rows).
- * lv_quant_rows_fp8: x bf16 [M, K] (row stride ldx elements, a multiple of 8) -> q e4m3 [M, K] contiguous and
- * scale fp32 [M]: per row amax = max|x|, q = e4m3_rn_satfinite(x * (448 / amax)), scale = amax / 448; a row whose
- * 448 / amax is not finite is zeros with scale 0.  K a positive multiple of 16; x and q 16-byte aligned.
+/* FP8 linears of the decoder (csrc/gemm_fp8.cu).
+ * lv_quant_rows_fp8_fmt: x bf16 [M, K] (row stride ldx elements, a multiple of 8) -> q [M, K] contiguous in format fmt
+ * and scale fp32 [M], each row quantised by the FP8 row rule.  K a positive multiple of 16; x and q 16-byte aligned.
  * lv_gemm_fp8: C[M, N] = act(bf16((A . W^T) * a_scale[m] * w_scale[n] + bias[n])) with A e4m3 [M, K] (row stride
  * lda bytes) and W e4m3 [N, K] (ldw bytes), both K-major, fp32 accumulation promoted out of the tensor cores every
  * 128 k-values, C bf16 with row stride ldc elements.  act: 0 none (bias optional), 3 fused SwiGLU over interleaved
  * (gate_i, up_i) W rows as in lv_gemm_bias_act (C is [M, N/2], bias NULL), each of gate and up scaled and rounded to
  * bf16 before bf16(silu(gate)) * up.  K a multiple of 16, N of 8 (16 for SwiGLU), lda / ldw multiples of 16, ldc of
  * 8; A, W, C 16-byte aligned.  For M <= 4 the product runs as a weight-stream GEMV (the rule of lv_gemm_bias_act). */
-int lv_quant_rows_fp8(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, lv_stream_t stream);
+int lv_quant_rows_fp8_fmt(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, int32_t fmt,
+                          lv_stream_t stream);
 int lv_gemm_fp8(const void* A, const float* a_scale, const void* W, const float* w_scale, const void* bias, void* C,
                 int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldw, int64_t ldc, int32_t act,
                 lv_stream_t stream);
 
-/* FP8 training of the decoder's linears (csrc/gemm_fp8.cu).  fmt: 0 = e4m3 (largest finite value 448), 1 = e5m2
- * (57 344); both quantise with the rule of lv_quant_rows_fp8 and their own largest value (satfinite conversion).
- * lv_quant_rows_fp8_fmt: lv_quant_rows_fp8 in either format (fmt 0 is lv_quant_rows_fp8).
+/* FP8 training of the decoder's linears (csrc/gemm_fp8.cu), fmt as in the FP8 row rule.
  * lv_quant_cols_fp8_t: cast-transpose.  x bf16 [R, C] (row stride ldx elements, a multiple of 8; C a multiple of 8)
  * -> q [C, R16] contiguous, R16 = R rounded up to 16, with q[c, r] = x[r, c] quantised by the scale of column c,
  * scale fp32 [C]; columns R..R16 of q are zero.  amax_ws is a workspace of C unsigned words.  x and q 16-byte aligned.
@@ -443,8 +445,6 @@ int lv_gemm_fp8(const void* A, const float* a_scale, const void* W, const float*
  * accumulate = 1, C is fp32 (ldc a multiple of 4) and each element becomes one IEEE round-to-nearest add
  * C + (acc * a_scale[m]) * b_scale[n], the value whose bf16 rounding accumulate = 0 stores (Megatron's fp32
  * main_grad, gradient-accumulation fusion).  K a multiple of 16, N of 8; A, B, C 16-byte aligned. */
-int lv_quant_rows_fp8_fmt(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, int32_t fmt,
-                          lv_stream_t stream);
 int lv_quant_cols_fp8_t(const void* x, void* q, float* scale, unsigned* amax_ws, int64_t R, int64_t C, int64_t ldx,
                         int32_t fmt, lv_stream_t stream);
 int lv_gemm_fp8_grad(const void* A, int32_t a_fmt, const float* a_scale, const void* B, const float* b_scale, void* C,

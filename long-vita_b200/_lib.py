@@ -127,10 +127,9 @@ SIGNATURES = {
     "lv_gemm_ex": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_i32, c_i32,
                            c_ptr]),
     "lv_gemm_wgrad_acc_f32": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_i32, c_ptr]),
-    "lv_quant_rows_fp8": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr]),
+    "lv_quant_rows_fp8_fmt": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i32, c_ptr]),
     "lv_gemm_fp8": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32,
                             c_ptr]),
-    "lv_quant_rows_fp8_fmt": (c_i32, [c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i32, c_ptr]),
     "lv_quant_cols_fp8_t": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i32, c_ptr]),
     "lv_gemm_fp8_grad": (c_i32, [c_ptr, c_i32, c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64,
                                  c_i32, c_ptr]),

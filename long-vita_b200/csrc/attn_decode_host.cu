@@ -13,14 +13,14 @@
 // lse_part [n, hkv, G] fp32 (natural log), exactly what lv_attn_decode_merge consumes.
 //
 // The FP8 host tier (opt-in, lossy) halves the bytes per row: e4m3 K | V with one fp32 scale per head and row, the
-// format and quantisation rule of kv_fp8_core.h (2112 B per row at 8 kv heads).  rows_to_host_fp8_kernel quantises
+// format and quantisation rule of fp8_core.h (2112 B per row at 8 kv heads).  rows_to_host_fp8_kernel quantises
 // device rows straight into the mapped host rows; attn_decode_host_fp8_kernel is the flash-decoding above over them.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math.h>
 
 #include "common.cuh"
-#include "kv_fp8_core.h"
+#include "fp8_core.h"
 
 namespace {
 
@@ -206,19 +206,19 @@ __global__ void __launch_bounds__(kQuantThreads) rows_to_host_fp8_kernel(const _
     for (int e = 0; e < 16; ++e) amax = fmaxf(amax, fabsf(x[e]));
 #pragma unroll
     for (int o = 4; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));  // the 8 lanes
-    const float inv = lv_kv8_inv(amax);
-    const bool zero = lv_kv8_zero_head(inv);                                 // amax 0: all-zero bytes, scale 0
+    const float inv = lv_fp8_inv(LV_FP8_E4M3, amax);
+    const bool zero = lv_fp8_zero_row(inv);                                 // amax 0: all-zero bytes, scale 0
     uint4 out = make_uint4(0u, 0u, 0u, 0u);
     if (!zero) {
       uint32_t w[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i)
-        w[i] = (uint32_t)lv_kv8_pack2(__fmul_rn(x[4 * i], inv), __fmul_rn(x[4 * i + 1], inv)) |
-               (uint32_t)lv_kv8_pack2(__fmul_rn(x[4 * i + 2], inv), __fmul_rn(x[4 * i + 3], inv)) << 16;
+        w[i] = (uint32_t)lv_fp8_pack2(LV_FP8_E4M3, __fmul_rn(x[4 * i], inv), __fmul_rn(x[4 * i + 1], inv)) |
+               (uint32_t)lv_fp8_pack2(LV_FP8_E4M3, __fmul_rn(x[4 * i + 2], inv), __fmul_rn(x[4 * i + 3], inv)) << 16;
       out = make_uint4(w[0], w[1], w[2], w[3]);
     }
     if (valid) *reinterpret_cast<uint4*>(dst + row * row_bytes + j * kD + lane * 16) = out;
-    if (lane == 0) sm_scale[grp] = zero ? 0.f : lv_kv8_scale(amax);
+    if (lane == 0) sm_scale[grp] = zero ? 0.f : lv_fp8_scale(LV_FP8_E4M3, amax);
     __syncthreads();
     if (threadIdx.x < rows_per_it * scale_vecs) {
       const int rr = threadIdx.x / scale_vecs, c = threadIdx.x % scale_vecs;

@@ -1,7 +1,7 @@
 // The FP8 (e4m3) operand rule of the FP8 attention forward (csrc/attn_fwd_fp8.cu), shared by the kernels and the host
-// compiler: tests/test_fp8_attn_host.py builds this text with gcc (LV_KV8_HD = static inline) and checks it, byte for
-// byte, against the torch.float8_e4m3fn restatement of the same rule.  Each block below is one row of the rule of
-// csrc/kv_fp8_core.h (lv_fp8_quant_row: amax / 448, zero bytes and scale 0 when 448 / amax is not finite).
+// compiler: tests/test_fp8_attn_host.py builds this text with gcc (LV_FP8_HD = static inline) and checks it, byte for
+// byte, against the torch restatement of tests/attn_fp8_ref.py.  Each block below is one e4m3 row of the rule of
+// csrc/fp8_core.h (lv_fp8_quant_row).
 //
 // K and V: one fp32 scale per (batch, kv head, 128-row key block), blocks aligned to key row 0; the ragged last block
 // holds the rows [128 (nt - 1), sk) and is zero-padded to 128 rows (nt = ceil(sk / 128)).
@@ -23,19 +23,19 @@
 #ifndef LV_ATTN_FP8_CORE_H_
 #define LV_ATTN_FP8_CORE_H_
 
-#include "kv_fp8_core.h"
+#include "fp8_core.h"
 
 #define LV_ATTN8_BLOCK 128  /* key rows per K / V block (the kernel's key tile) */
 #define LV_ATTN8_QROWS 64   /* query rows per Q scale (one consumer warpgroup) */
 
 // Key (0..127, within its block) whose value sits at byte kappa of a transposed V row: kappa = 32 c + 16 h + 4 t + i
 // holds key 32 c + 16 h + 8 (i / 2) + 2 t + i % 2.
-LV_KV8_HD int lv_attn8_key_of(int kappa) {
+LV_FP8_HD int lv_attn8_key_of(int kappa) {
   return (kappa & ~15) | (((kappa >> 1) & 1) << 3) | (((kappa >> 2) & 3) << 1) | (kappa & 1);
 }
 
 // Number of key blocks of sk keys.
-LV_KV8_HD int64_t lv_attn8_blocks(int64_t sk) { return (sk + LV_ATTN8_BLOCK - 1) / LV_ATTN8_BLOCK; }
+LV_FP8_HD int64_t lv_attn8_blocks(int64_t sk) { return (sk + LV_ATTN8_BLOCK - 1) / LV_ATTN8_BLOCK; }
 
 #ifndef __CUDA_ARCH__
 // One (kv head, key block) of K and of V: rows x [n][d] bf16 bits with row stride ld elements (n <= 128 valid rows)
@@ -45,7 +45,7 @@ static inline float lv_attn8_quant_k_block(const uint16_t* x, int64_t ld, int n,
                                            uint8_t* wq) {
   for (int r = 0; r < n; ++r)
     for (int c = 0; c < d; ++c) work[(int64_t)r * d + c] = x[r * ld + c];
-  const float s = lv_fp8_quant_row(work, wq, (int64_t)n * d);
+  const float s = lv_fp8_quant_row(LV_FP8_E4M3, work, wq, (int64_t)n * d);
   for (int64_t i = 0; i < (int64_t)LV_ATTN8_BLOCK * d; ++i) k8[i] = i < (int64_t)n * d ? wq[i] : 0;
   return s;
 }
@@ -54,7 +54,7 @@ static inline float lv_attn8_quant_v_block(const uint16_t* x, int64_t ld, int n,
                                            uint8_t* wq) {
   for (int r = 0; r < n; ++r)
     for (int c = 0; c < d; ++c) work[(int64_t)r * d + c] = x[r * ld + c];
-  const float s = lv_fp8_quant_row(work, wq, (int64_t)n * d);
+  const float s = lv_fp8_quant_row(LV_FP8_E4M3, work, wq, (int64_t)n * d);
   for (int c = 0; c < d; ++c)
     for (int kappa = 0; kappa < LV_ATTN8_BLOCK; ++kappa) {
       const int key = lv_attn8_key_of(kappa);

@@ -23,7 +23,6 @@
 #include "attn_fp8_core.h"
 #include "attn_sched.cuh"
 #include "common.cuh"
-#include "kv_fp8_core.h"
 #include "ptx.cuh"
 
 namespace lv {
@@ -53,7 +52,7 @@ __device__ __forceinline__ void unpack_bf16x8(const uint4& v, float (&f)[8]) {
 
 // four fp32 values (already scaled) -> four e4m3 bytes, a in the low byte
 __device__ __forceinline__ uint32_t pack_e4m3x4(float a, float b, float c, float d) {
-  return (uint32_t)lv_kv8_pack2(a, b) | ((uint32_t)lv_kv8_pack2(c, d) << 16);
+  return (uint32_t)lv_fp8_pack2(LV_FP8_E4M3, a, b) | ((uint32_t)lv_fp8_pack2(LV_FP8_E4M3, c, d) << 16);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -96,8 +95,8 @@ __global__ void __launch_bounds__(256)
   __syncthreads();
 #pragma unroll
   for (int w = 0; w < 8; ++w) amax = fmaxf(amax, warp_max[w]);
-  const float inv = lv_kv8_inv(amax);
-  const bool zero = lv_kv8_zero_head(inv);
+  const float inv = lv_fp8_inv(LV_FP8_E4M3, amax);
+  const bool zero = lv_fp8_zero_row(inv);
   uint32_t q[16];
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -107,7 +106,7 @@ __global__ void __launch_bounds__(256)
     q[2 * i + 1] = zero ? 0u : pack_e4m3x4(__fmul_rn(f[4], inv), __fmul_rn(f[5], inv), __fmul_rn(f[6], inv), __fmul_rn(f[7], inv));
   }
   const long long blk = (long long)(b * hkv + kvh) * nt + tile;
-  const float scale = zero ? 0.f : lv_kv8_scale(amax);
+  const float scale = zero ? 0.f : lv_fp8_scale(LV_FP8_E4M3, amax);
   if (!is_v) {
     uint4* dst = reinterpret_cast<uint4*>(k8 + (blk * 128 + r) * 128 + h * 64);
 #pragma unroll
@@ -160,8 +159,8 @@ __device__ __forceinline__ float quant_q_rows(const uint8_t* sQ, uint8_t* sQ8, i
   if ((wg_tid & 31) == 0) red[wg_tid >> 5] = amax;
   named_bar_sync(1 + c, 128);
   amax = fmaxf(fmaxf(red[0], red[1]), fmaxf(red[2], red[3]));
-  const float inv = lv_kv8_inv(amax);
-  const bool zero = lv_kv8_zero_head(inv);
+  const float inv = lv_fp8_inv(LV_FP8_E4M3, amax);
+  const bool zero = lv_fp8_zero_row(inv);
   uint8_t* dst = sQ8 + c * 8192 + rl * 128;
 #pragma unroll
   for (int j = 0; j < 4; ++j) {        // 16-byte chunk 4 h + j of the e4m3 row = bf16 chunks 2 j, 2 j + 1
@@ -177,7 +176,7 @@ __device__ __forceinline__ float quant_q_rows(const uint8_t* sQ, uint8_t* sQ8, i
   }
   fence_proxy_async_smem();           // the generic stores above are read by wgmma (async proxy)
   named_bar_sync(1 + c, 128);
-  return zero ? 0.f : lv_kv8_scale(amax);
+  return zero ? 0.f : lv_fp8_scale(LV_FP8_E4M3, amax);
 }
 
 __global__ void __launch_bounds__(F8A_THREADS, 1)

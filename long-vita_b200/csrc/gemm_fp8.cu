@@ -1,7 +1,7 @@
 // FP8 (e4m3) linear layers of the decoder on the Hopper tensor cores:
 //   C[M, N] = act(bf16((A_q . W_q^T) * s_a[m] * s_w[n] + bias[n]))
-// with A_q / W_q e4m3, both K-major, and one fp32 scale per row of each (csrc/kv_fp8_core.h, the rule of the K/V host
-// tier applied to a whole row).  Three kernels:
+// with A_q / W_q e4m3, both K-major, and one fp32 scale per row of each (the rule of csrc/fp8_core.h applied to a whole
+// row).  Three kernels:
 //   quant_rows_fp8_kernel  bf16 rows -> e4m3 rows + fp32 scales (weights at load, the A operand before each product)
 //   gemm_fp8_kernel        the persistent warp-specialised structure of gemm_bf16_kernel (gemm.cu): one TMA producer
 //                          thread, two consumer warpgroups, a shared-memory ring of 128-byte-swizzled rows, grouped
@@ -19,7 +19,7 @@
 #include <string.h>
 
 #include "common.cuh"
-#include "kv_fp8_core.h"
+#include "fp8_core.h"
 #include "ptx.cuh"
 
 namespace lv {
@@ -278,34 +278,10 @@ __global__ void __launch_bounds__(F_THREADS, 1)
 // Row quantiser: one CTA of 256 threads per row, so that a decode-sized call (1-4 rows) is not one warp walking a
 // 13 824-wide row; 16 values per thread and step (two 16-byte loads, one 16-byte store).  The first pass finds amax
 // (max is exact in any order: warp shuffles, then the 8 warps through shared memory), the second reads the row again
-// (from L1 / L2) and stores q; thread 0 stores the scale.  Same arithmetic as lv_fp8_quant_row of kv_fp8_core.h.
+// (from L1 / L2) and stores q; thread 0 stores the scale.  Same arithmetic as lv_fp8_quant_row of fp8_core.h, in e4m3
+// or (E5M2, hybrid training's gradients) e5m2.
 // ---------------------------------------------------------------------------------------------
 constexpr int Q_THREADS = 256;
-
-// The two FP8 formats of the quantisers.  E5M2 (hybrid training's gradients) follows the rule of kv_fp8_core.h with
-// its own largest finite value: inv = 57344 / amax, q = e5m2_rn_satfinite(x * inv), scale = amax / 57344, a column or
-// row whose inv is not finite is zeros with scale 0.  The E4M3 members are exactly lv_kv8_inv / lv_kv8_scale /
-// lv_kv8_pack2, so the e4m3 instantiations compute what the e4m3-only kernels computed.
-constexpr float LV_E5M2_MAX = 57344.0f;
-
-template <bool E5M2>
-__device__ __forceinline__ float fp8_inv(float amax) {
-  return E5M2 ? __fdiv_rn(LV_E5M2_MAX, amax) : lv_kv8_inv(amax);
-}
-template <bool E5M2>
-__device__ __forceinline__ float fp8_scale(float amax) {
-  return E5M2 ? __fdiv_rn(amax, LV_E5M2_MAX) : lv_kv8_scale(amax);
-}
-template <bool E5M2>
-__device__ __forceinline__ uint16_t fp8_pack2(float lo, float hi) {
-  if constexpr (E5M2) {
-    uint16_t r;
-    asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-    return r;
-  } else {
-    return lv_kv8_pack2(lo, hi);
-  }
-}
 
 __device__ __forceinline__ void bf16x8(const uint4& v, float (&f)[8]) {
   const uint32_t w[4] = {v.x, v.y, v.z, v.w};
@@ -341,8 +317,8 @@ __global__ void __launch_bounds__(Q_THREADS)
   __syncthreads();
 #pragma unroll
   for (int w = 0; w < Q_THREADS / 32; ++w) amax = fmaxf(amax, warp_max[w]);
-  const float inv = fp8_inv<E5M2>(amax);
-  const bool zero = lv_kv8_zero_head(inv);
+  const float inv = lv_fp8_inv(E5M2, amax);
+  const bool zero = lv_fp8_zero_row(inv);
   for (int k = threadIdx.x * 16; k < K; k += Q_THREADS * 16) {
     uint32_t o[4] = {0u, 0u, 0u, 0u};
     if (!zero) {
@@ -352,13 +328,14 @@ __global__ void __launch_bounds__(Q_THREADS)
         bf16x8(*reinterpret_cast<const uint4*>(x + k + 8 * h), f);
 #pragma unroll
         for (int i = 0; i < 2; ++i)
-          o[2 * h + i] = (uint32_t)fp8_pack2<E5M2>(__fmul_rn(f[4 * i], inv), __fmul_rn(f[4 * i + 1], inv)) |
-                         ((uint32_t)fp8_pack2<E5M2>(__fmul_rn(f[4 * i + 2], inv), __fmul_rn(f[4 * i + 3], inv)) << 16);
+          o[2 * h + i] =
+              (uint32_t)lv_fp8_pack2(E5M2, __fmul_rn(f[4 * i], inv), __fmul_rn(f[4 * i + 1], inv)) |
+              ((uint32_t)lv_fp8_pack2(E5M2, __fmul_rn(f[4 * i + 2], inv), __fmul_rn(f[4 * i + 3], inv)) << 16);
       }
     }
     *reinterpret_cast<uint4*>(q + k) = make_uint4(o[0], o[1], o[2], o[3]);
   }
-  if (threadIdx.x == 0) S[row] = zero ? 0.f : fp8_scale<E5M2>(amax);
+  if (threadIdx.x == 0) S[row] = zero ? 0.f : lv_fp8_scale(E5M2, amax);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -417,12 +394,12 @@ __global__ void __launch_bounds__(CT_THREADS)
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
     const float amax = c + i < C ? __uint_as_float(amax_bits[c + i]) : 0.f;
-    inv[i] = fp8_inv<E5M2>(amax);
-    zero[i] = lv_kv8_zero_head(inv[i]);
+    inv[i] = lv_fp8_inv(E5M2, amax);
+    zero[i] = lv_fp8_zero_row(inv[i]);
   }
   if (blockIdx.x == 0 && threadIdx.x < CT_C && c0 + threadIdx.x < C) {
     const float amax = __uint_as_float(amax_bits[c0 + threadIdx.x]);
-    S[c0 + threadIdx.x] = lv_kv8_zero_head(fp8_inv<E5M2>(amax)) ? 0.f : fp8_scale<E5M2>(amax);
+    S[c0 + threadIdx.x] = lv_fp8_zero_row(lv_fp8_inv(E5M2, amax)) ? 0.f : lv_fp8_scale(E5M2, amax);
   }
 #pragma unroll
   for (int step = 0; step < CT_R / 32; ++step) {
@@ -433,7 +410,7 @@ __global__ void __launch_bounds__(CT_THREADS)
       bf16x8(*reinterpret_cast<const uint4*>(X + (long long)r * ldx + c), f);
 #pragma unroll
       for (int i = 0; i < 8; i += 2) {
-        const uint16_t p = fp8_pack2<E5M2>(__fmul_rn(f[i], inv[i]), __fmul_rn(f[i + 1], inv[i + 1]));
+        const uint16_t p = lv_fp8_pack2(E5M2, __fmul_rn(f[i], inv[i]), __fmul_rn(f[i + 1], inv[i + 1]));
         b[i] = zero[i] ? 0 : (uint8_t)(p & 0xFF);
         b[i + 1] = zero[i + 1] ? 0 : (uint8_t)(p >> 8);
       }
@@ -568,49 +545,19 @@ static int encode_fp8_operand(CUtensorMap* m, const void* p, int64_t rows, int64
   return encode_tmap_bf16(m, p, 2, dims, str, box, true);
 }
 
-static int launch_gemm_fp8(const void* A, const float* sa, const void* W, const float* sw, const void* bias, void* C,
-                           int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldw, int64_t ldc, int act,
-                           cudaStream_t s) {
-  CUtensorMap tmA, tmB, tmC;
-  int r = encode_fp8_operand(&tmA, A, M, K, lda, F_BM);
-  if (r) return r;
-  r = encode_fp8_operand(&tmB, W, N, K, ldw, F_BN);
-  if (r) return r;
-  const uint64_t dims[2] = {(uint64_t)(act == 3 ? N / 2 : N), (uint64_t)M};
-  const uint64_t str[2] = {2, (uint64_t)ldc * 2};
-  const uint32_t box[2] = {64, 64};
-  r = encode_tmap_bf16(&tmC, C, 2, dims, str, box, true);
-  if (r) return r;
-  static PerDeviceOnce attr_once;
-  int attr_dev;
-  if (attr_once.needed(&attr_dev)) {
-    LV_CHECK_CUDA(cudaFuncSetAttribute(gemm_fp8_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       F_SMEM));
-    attr_once.done(attr_dev);
-  }
-  const int64_t tiles = ((M + F_BM - 1) / F_BM) * ((N + F_BN - 1) / F_BN);
-  const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
-  // M-blocks per rasterisation group, as in gemm.cu: the group's A panel (gm x 128 rows x K bytes) takes ~16 MB of L2
-  int gm = (int)((16ll << 20) / (128 * K));
-  gm = gm < 8 ? 8 : (gm > 64 ? 64 : gm);
-  gemm_fp8_kernel<false, false><<<grid, F_THREADS, F_SMEM, s>>>(
-      tmA, tmB, tmC, sa, sw, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M, (int)N, (int)K, act, gm, nullptr, 0ll);
-  LV_CHECK_LAUNCH("gemm_fp8_kernel");
-  return LV_OK;
-}
-
-// The backward products (lv_gemm_fp8_grad): gemm_fp8_kernel without bias or activation, A e4m3 or e5m2, C bf16 or
-// (ACC) fp32 accumulated into.
+// gemm_fp8_kernel: A e4m3 or (A_E5M2, a gradient of the backward products) e5m2, B e4m3; C bf16 with bias and act,
+// or (ACC, lv_gemm_fp8_grad) fp32 accumulated into.
 template <bool A_E5M2, bool ACC>
-static int launch_gemm_fp8_grad(const void* A, const float* sa, const void* B, const float* sb, void* C, int64_t M,
-                                int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, cudaStream_t s) {
+static int launch_gemm_fp8(const void* A, const float* sa, const void* B, const float* sb, const void* bias, void* C,
+                           int64_t M, int64_t N, int64_t K, int64_t lda, int64_t ldb, int64_t ldc, int act,
+                           cudaStream_t s) {
   CUtensorMap tmA, tmB, tmC;
   int r = encode_fp8_operand(&tmA, A, M, K, lda, F_BM);
   if (r) return r;
   r = encode_fp8_operand(&tmB, B, N, K, ldb, F_BN);
   if (r) return r;
   if constexpr (!ACC) {
-    const uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
+    const uint64_t dims[2] = {(uint64_t)(act == 3 ? N / 2 : N), (uint64_t)M};
     const uint64_t str[2] = {2, (uint64_t)ldc * 2};
     const uint32_t box[2] = {64, 64};
     r = encode_tmap_bf16(&tmC, C, 2, dims, str, box, true);
@@ -627,10 +574,12 @@ static int launch_gemm_fp8_grad(const void* A, const float* sa, const void* B, c
   }
   const int64_t tiles = ((M + F_BM - 1) / F_BM) * ((N + F_BN - 1) / F_BN);
   const int grid = (int)(tiles < sm_count() ? tiles : sm_count());
+  // M-blocks per rasterisation group, as in gemm.cu: the group's A panel (gm x 128 rows x K bytes) takes ~16 MB of L2
   int gm = (int)((16ll << 20) / (128 * K));
   gm = gm < 8 ? 8 : (gm > 64 ? 64 : gm);
-  kernel<<<grid, F_THREADS, F_SMEM, s>>>(tmA, tmB, tmC, sa, sb, nullptr, (int)M, (int)N, (int)K, 0, gm,
-                                         ACC ? reinterpret_cast<float*>(C) : nullptr, ACC ? (long long)ldc : 0ll);
+  kernel<<<grid, F_THREADS, F_SMEM, s>>>(tmA, tmB, tmC, sa, sb, reinterpret_cast<const __nv_bfloat16*>(bias), (int)M,
+                                         (int)N, (int)K, act, gm, ACC ? reinterpret_cast<float*>(C) : nullptr,
+                                         ACC ? (long long)ldc : 0ll);
   LV_CHECK_LAUNCH("gemm_fp8_kernel");
   return LV_OK;
 }
@@ -661,20 +610,16 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 extern "C" {
 
-int lv_quant_rows_fp8(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, lv_stream_t stream) {
-  return lv_quant_rows_fp8_fmt(x, q, scale, M, K, ldx, 0, stream);
-}
-
 int lv_quant_rows_fp8_fmt(const void* x, void* q, float* scale, int64_t M, int64_t K, int64_t ldx, int32_t fmt,
                           lv_stream_t stream) {
-  LV_CHECK_ARG(x && q && scale, "lv_quant_rows_fp8: null pointer");
-  LV_CHECK_ARG(fmt == 0 || fmt == 1, "lv_quant_rows_fp8: format %d is not built (0 = e4m3, 1 = e5m2)", fmt);
+  LV_CHECK_ARG(x && q && scale, "lv_quant_rows_fp8_fmt: null pointer");
+  LV_CHECK_ARG(fmt == 0 || fmt == 1, "lv_quant_rows_fp8_fmt: format %d is not built (0 = e4m3, 1 = e5m2)", fmt);
   LV_CHECK_ARG(M >= 0 && K > 0 && K % 16 == 0 && M < (1ll << 31) && K < (1ll << 31),
-               "lv_quant_rows_fp8: bad shape M=%lld K=%lld (K must be a positive multiple of 16)", (long long)M,
+               "lv_quant_rows_fp8_fmt: bad shape M=%lld K=%lld (K must be a positive multiple of 16)", (long long)M,
                (long long)K);
-  LV_CHECK_ARG(ldx % 8 == 0 && ldx >= K, "lv_quant_rows_fp8: ldx=%lld must be a multiple of 8 and >= K=%lld",
+  LV_CHECK_ARG(ldx % 8 == 0 && ldx >= K, "lv_quant_rows_fp8_fmt: ldx=%lld must be a multiple of 8 and >= K=%lld",
                (long long)ldx, (long long)K);
-  LV_CHECK_ARG(aligned16(x) && aligned16(q), "lv_quant_rows_fp8: x and q must be 16-byte aligned");
+  LV_CHECK_ARG(aligned16(x) && aligned16(q), "lv_quant_rows_fp8_fmt: x and q must be 16-byte aligned");
   if (M == 0) return LV_OK;
   LV_BIND_DEVICE(x);
   auto* const kernel = fmt ? quant_rows_fp8_kernel<true> : quant_rows_fp8_kernel<false>;
@@ -736,7 +681,7 @@ int lv_gemm_fp8(const void* A, const float* a_scale, const void* W, const float*
   // the GEMV for decode-sized M, by the rule of lv_gemm_bias_act: unless a 256-column tiling already has a tile per SM
   if (M <= 4 && (N + 255) / 256 < sm_count())
     return launch_gemv_fp8(A, a_scale, W, w_scale, bias, C, M, N, K, lda, ldw, ldc, act, s);
-  return launch_gemm_fp8(A, a_scale, W, w_scale, bias, C, M, N, K, lda, ldw, ldc, act, s);
+  return launch_gemm_fp8<false, false>(A, a_scale, W, w_scale, bias, C, M, N, K, lda, ldw, ldc, act, s);
 }
 
 int lv_gemm_fp8_grad(const void* A, int32_t a_fmt, const float* a_scale, const void* B, const float* b_scale, void* C,
@@ -758,11 +703,9 @@ int lv_gemm_fp8_grad(const void* A, int32_t a_fmt, const float* a_scale, const v
   if (M == 0) return LV_OK;
   LV_BIND_DEVICE(A);
   const cudaStream_t s = (cudaStream_t)stream;
-  if (accumulate)
-    return a_fmt ? launch_gemm_fp8_grad<true, true>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s)
-                 : launch_gemm_fp8_grad<false, true>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s);
-  return a_fmt ? launch_gemm_fp8_grad<true, false>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s)
-               : launch_gemm_fp8_grad<false, false>(A, a_scale, B, b_scale, C, M, N, K, lda, ldb, ldc, s);
+  auto* const launch = accumulate ? (a_fmt ? launch_gemm_fp8<true, true> : launch_gemm_fp8<false, true>)
+                                  : (a_fmt ? launch_gemm_fp8<true, false> : launch_gemm_fp8<false, false>);
+  return launch(A, a_scale, B, b_scale, nullptr, C, M, N, K, lda, ldb, ldc, 0, s);
 }
 
 }  // extern "C"

@@ -429,56 +429,21 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: 
     lossy, opt-in), whole-tensor, row-chunked and streamed alike; its blocks are aligned to key row 0, so the span
     calls of the streamed layer still give exactly the rows of the whole call.  One new token (decode) and the cache
     contents stay bf16.  Packed rows (`cu_seqlens`) have no FP8 path: NotImplementedError, before anything runs."""
-    if check_attn_dtype(attn_dtype) == torch.float8_e4m3fn:
-        if cu_seqlens is not None:
-            raise NotImplementedError("packed samples (position ids restarting at 0) have no FP8 attention; use "
-                                      "attn_dtype=torch.bfloat16")
-        return _fp8_attention_step(cache, rows)
-    kw = ops.docs_kwargs(cu_seqlens)
+    fp8 = check_attn_dtype(attn_dtype) == torch.float8_e4m3fn
+    if fp8 and cu_seqlens is not None:
+        raise NotImplementedError("packed samples (position ids restarting at 0) have no FP8 attention; use "
+                                  "attn_dtype=torch.bfloat16")
+    docs = ops.docs_kwargs(cu_seqlens)
+
+    def prefill(q, k, v, **kw):
+        fwd = ops.attention_fwd_fp8 if fp8 else ops.attention_fwd
+        return fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True, **kw)
+
     if cache is None:
         def attend(li, q, k, v):
-            return ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True, **kw)
+            return prefill(q, k, v, **docs)
 
         attend.query_chunks = cu_seqlens is None
-        return attend
-
-    if isinstance(cache, OffloadedKVCache):
-        cache.check_rows(rows)
-
-        def attend(li, q, k, v):
-            n = q.shape[0]
-            if cache.on_host(li):
-                kh, length = cache.append_host(li, k, v, n)
-                if n == 1:
-                    return cache.decode_host(q[0], kh, length)
-                return ops.attention_fwd(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True)
-            kc, vc, length = cache.append(li, k, v, n)
-            if n == 1:
-                return ops.attention_decode(q[0], kc, vc, length)
-            return ops.attention_fwd(q.unsqueeze(0), kc[:length].unsqueeze(0), vc[:length].unsqueeze(0), causal=True)
-
-        attend.query_chunks = len(cache) == 0
-        return attend
-
-    def attend(li, q, k, v):
-        kc, vc, length = cache.append(li, k, v)
-        if q.shape[0] == 1:
-            return ops.attention_decode(q[0], kc, vc, length)
-        return ops.attention_fwd(q.unsqueeze(0), kc[:length].unsqueeze(0), vc[:length].unsqueeze(0), causal=True)
-
-    return attend
-
-
-def _fp8_attention_step(cache, rows: int):
-    """attention_step with FP8 prefill attention: the same steps, each multi-token call on ops.attention_fwd_fp8."""
-    def prefill(q, k, v):
-        return ops.attention_fwd_fp8(q.unsqueeze(0), k.unsqueeze(0), v.unsqueeze(0), causal=True)
-
-    if cache is None:
-        def attend(li, q, k, v):
-            return prefill(q, k, v)
-
-        attend.query_chunks = True
         return attend
 
     if isinstance(cache, OffloadedKVCache):

@@ -20,7 +20,7 @@ buffers above, the others one pinned host buffer each, read in place by the deco
 `make_cache` decides which, once, from the free device memory (`device_layers`).
 
 The host tier may be kept in FP8 (`host_dtype=torch.float8_e4m3fn`): e4m3 K|V rows with one fp32 scale per head
-(csrc/kv_fp8_core.h), 2112 instead of 4096 bytes per row at 8 kv heads, which halves both the pinned memory and the
+(csrc/fp8_core.h), 2112 instead of 4096 bytes per row at 8 kv heads, which halves both the pinned memory and the
 PCIe bytes a decode step reads.  It is lossy and opt-in; the default is bf16, and the device layers are bf16 either way.
 """
 from __future__ import annotations

@@ -546,7 +546,7 @@ def pinned_rows(rows: int, cols: int, dtype: torch.dtype = torch.bfloat16) -> to
 
 
 def kv_fp8_row_bytes(hkv: int, d: int) -> int:
-    """Bytes of one FP8 host row (csrc/kv_fp8_core.h): K and V of the hkv heads in e4m3, then the 2 hkv fp32 scales
+    """Bytes of one FP8 host row (csrc/fp8_core.h): K and V of the hkv heads in e4m3, then the 2 hkv fp32 scales
     padded to 16 bytes; 2112 at 8 kv heads of 128."""
     return 2 * hkv * d + (8 * hkv + 15) // 16 * 16
 
@@ -583,7 +583,7 @@ def kv_rows_to_host(k: torch.Tensor, v: torch.Tensor, dst: torch.Tensor) -> torc
 
 def kv_rows_to_host_fp8(k: torch.Tensor, v: torch.Tensor, dst: torch.Tensor) -> torch.Tensor:
     """kv_rows_to_host into FP8 host rows: dst uint8 [n, kv_fp8_row_bytes(hkv, d)] (pinned) receives the rows of k / v
-    [n, hkv, d] quantised per head (csrc/kv_fp8_core.h), in stream order, by a kernel that stores straight into the
+    [n, hkv, d] quantised per head (csrc/fp8_core.h), in stream order, by a kernel that stores straight into the
     mapped host rows (lv_rows_to_host_fp8; no device temporary).  d = 128.  Returns dst."""
     _need_cuda_bf16(k, v)
     n, hkv, d = k.shape
@@ -877,12 +877,11 @@ def linear(x: torch.Tensor, weight, bias: Optional[torch.Tensor] = None, act: Op
 
 
 # ------------------------------------------------------------------------------------------------
-# FP8 (e4m3) linears: per-row scales on both operands (csrc/kv_fp8_core.h), lv_gemm_fp8
+# FP8 (e4m3) linears: per-row scales on both operands (csrc/fp8_core.h), lv_gemm_fp8
 # ------------------------------------------------------------------------------------------------
 FP8 = torch.float8_e4m3fn
 FP8_E5M2 = torch.float8_e5m2
 _FP8_FMT = {FP8: 0, FP8_E5M2: 1}            # the `fmt` argument of the C entry points
-FP8_MAX = {FP8: 448.0, FP8_E5M2: 57344.0}   # largest finite value of each format
 
 
 def _fp8_fmt(op: str, dtype) -> int:
@@ -893,9 +892,9 @@ def _fp8_fmt(op: str, dtype) -> int:
 
 def quant_rows_fp8(x: torch.Tensor, dtype: torch.dtype = FP8) -> Tuple[torch.Tensor, torch.Tensor]:
     """x bf16 [M, K] (K contiguous, K a multiple of 16, row stride a multiple of 8) -> (q [M, K] of `dtype`, scale
-    fp32 [M]): one scale per row, amax / max, q = fp8(x * max / amax) saturating at max, where max is 448 for e4m3 (the
-    default) and 57 344 for e5m2; a row of zeros (or too small to scale) is zeros with scale 0
-    (lv_quant_rows_fp8_fmt).  x ~ q.float() * scale[:, None]."""
+    fp32 [M]): one scale per row, amax / max, q = fp8(x * max / amax) saturating at max, the largest finite value of
+    `dtype` (e4m3, the default, or e5m2); a row of zeros (or too small to scale) is zeros with scale 0
+    (lv_quant_rows_fp8_fmt, the rule of csrc/fp8_core.h).  x ~ q.float() * scale[:, None]."""
     _need_cuda_bf16(x)
     fmt = _fp8_fmt("quant_rows_fp8", dtype)
     if x.dim() != 2:
@@ -907,9 +906,7 @@ def quant_rows_fp8(x: torch.Tensor, dtype: torch.dtype = FP8) -> Tuple[torch.Ten
         x = x.contiguous()
     q = torch.empty((M, K), dtype=dtype, device=x.device)
     scale = torch.empty((M,), dtype=torch.float32, device=x.device)
-    if M and fmt == 0:
-        _call("lv_quant_rows_fp8", x.data_ptr(), q.data_ptr(), scale.data_ptr(), M, K, max(x.stride(0), K))
-    elif M:
+    if M:
         _call("lv_quant_rows_fp8_fmt", x.data_ptr(), q.data_ptr(), scale.data_ptr(), M, K, max(x.stride(0), K), fmt)
     return q, scale
 
@@ -1030,7 +1027,7 @@ def linear_fp8(x: torch.Tensor, weight: Fp8Weight, bias: Optional[torch.Tensor] 
     # per launch, so the FP8 call allocates once more than the bf16 one, not twice
     ws = torch.empty((M * K + 4 * M,), dtype=torch.uint8, device=x.device)
     xq, xs = ws.data_ptr(), ws.data_ptr() + M * K
-    _call("lv_quant_rows_fp8", x2.data_ptr(), xq, xs, M, K, max(x2.stride(0), K))
+    _call("lv_quant_rows_fp8_fmt", x2.data_ptr(), xq, xs, M, K, max(x2.stride(0), K), _FP8_FMT[FP8])
     ev0 = _TIMER.start() if _TIMER is not None else None
     ldc = out.stride(0) if M > 1 else -(-n_out // 8) * 8
     _call("lv_gemm_fp8", xq, xs, weight.data.data_ptr(), weight.scale.data_ptr(), _ptr(bias),

@@ -2,11 +2,8 @@
 (csrc/attn_fp8_core.h), a float64 reference, and the checker its GPU tests use.
 
 Rule (`quant_kv`, `quant_q`): K and V in 128-row blocks per (batch, kv head) aligned to key row 0, Q in 64-row groups
-per (batch, query head) aligned to query row 0; each block is one row of the rule of tests/test_kv_fp8_host.py
-(`quantise_heads`: amax / 448, zeros with scale 0 when 448 / amax is not finite; restated here as `quantise_blocks`
-with both divisions tensor by tensor, which CUDA rounds as IEEE divisions where a division by a Python scalar becomes a
-multiplication by its reciprocal).  V blocks are stored transposed with
-the key permutation `key_of`.
+per (batch, query head) aligned to query row 0; each block is one e4m3 row of the rule of csrc/fp8_core.h
+(tests/fp8_ref.quant_rows_ref).  V blocks are stored transposed with the key permutation `key_of`.
 
 Reference: `attention_fwd_ref` of tests/attn_fwd_ref.py over the DEQUANTISED operands (q8 s_q, k8 s_k, v8 s_v), so the
 quantisation of Q, K and V is part of the function being checked, not of its error.  What the kernel does beyond that
@@ -42,6 +39,7 @@ import math
 import torch
 
 from tests.attn_fwd_ref import _worst, attention_fwd_ref, ulp_bf16
+from tests.fp8_ref import quant_rows_ref
 
 FP8 = torch.float8_e4m3fn
 BLOCK = 128          # key rows per K / V scale
@@ -49,20 +47,6 @@ QROWS = 64           # query rows per Q scale
 ACC = 2.0 ** -11
 LSE_RATIO = 8.0
 Z_ROW = 3.0
-
-
-def quantise_blocks(x: torch.Tensor):
-    """x [..., n] bf16 -> (q [..., n] uint8 e4m3, scale [...] fp32): tests/test_kv_fp8_host.py's quantise_heads, with
-    amax / 448 also divided tensor by tensor (IEEE on every device)."""
-    xf = x.float()
-    amax = xf.abs().amax(-1, keepdim=True)
-    c448 = torch.full_like(amax, 448.0)
-    inv = c448 / amax
-    zero = torch.isinf(inv) | torch.isnan(inv)
-    q = (xf * inv).to(FP8).view(torch.uint8)
-    q = torch.where(zero, torch.zeros_like(q), q)
-    scale = torch.where(zero, torch.zeros_like(amax), amax / c448)[..., 0]
-    return q, scale
 
 
 def key_of(kappa):
@@ -87,8 +71,8 @@ def quant_kv(k, v):
     b, sk, hkv, d = k.shape
     kb, nt = _blocks(k, BLOCK)
     vb, _ = _blocks(v, BLOCK)
-    kq, ks = quantise_blocks(kb)               # zero padding rows never raise amax and quantise to zero bytes
-    vq, vs = quantise_blocks(vb)
+    kq, ks = quant_rows_ref(kb)                # zero padding rows never raise amax and quantise to zero bytes
+    vq, vs = quant_rows_ref(vb)
     k8 = kq.view(b, hkv, nt * BLOCK, d)
     vq = vq.view(b, hkv, nt, BLOCK, d)
     perm = key_of(torch.arange(BLOCK)).to(vq.device)
@@ -119,7 +103,7 @@ def quant_q(q, rows=None):
     ok = src < sq
     qg[:, ok] = q[:, src[ok]]
     qb, ng = _blocks(qg, QROWS)
-    qq, qs = quantise_blocks(qb)
+    qq, qs = quant_rows_ref(qb)
     qf = (qq.view(FP8).float() * qs[..., None]).view(b, hq, ng * QROWS, d).permute(0, 2, 1, 3)
     at = torch.searchsorted(groups, rows // QROWS) * QROWS + rows % QROWS
     return qf[:, at]

@@ -11,8 +11,6 @@
 """
 import contextlib
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
@@ -23,9 +21,9 @@ from long_vita_b200.config import LongVITAConfig
 from long_vita_b200.hf import modeling
 from long_vita_b200.weights import synthetic_state_dict
 from tests import attn_fp8_ref as R
+from tests.fp8_ref import E4M3, FP8_MAX, build_shim
 from tests.test_stream_layer_host import _constants, stream_oracle_ops
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FP8 = torch.float8_e4m3fn
 
 _SHIM = r"""
@@ -50,12 +48,7 @@ void quant_kv(const uint16_t* k, const uint16_t* v, int n, int hkv, int d, uint8
 
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    d = tmp_path_factory.mktemp("attn8_host")
-    src, so = d / "attn8_shim.c", str(d / "libattn8_host.so")
-    src.write_text(_SHIM)
-    subprocess.run(["gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", "-I",
-                    os.path.join(ROOT, "long-vita_b200", "csrc"), str(src), "-o", so, "-lm"], check=True)
-    lib = C.CDLL(so)
+    lib = build_shim(tmp_path_factory.mktemp("attn8_host"), _SHIM)
     lib.key_of.argtypes = [C.c_int]
     lib.quant_kv.argtypes = [C.c_void_p] * 2 + [C.c_int] * 3 + [C.c_void_p] * 6
     return lib
@@ -106,7 +99,8 @@ def test_header_matches_restatement(core, n):
             a, b = a.view(torch.int32), b.view(torch.int32)
         assert a.shape == b.shape and torch.equal(a, b), (name, n)
     if n > 256:
-        assert float(got[2][1, 1]) == 0.0 and float(got[3][2, 2]) == 0.0 and float(got[3][0, 1]) == float(torch.tensor(1000.0) / 448)
+        assert float(got[2][1, 1]) == 0.0 and float(got[3][2, 2]) == 0.0
+        assert float(got[3][0, 1]) == float(torch.tensor(1000.0) / FP8_MAX[E4M3])
         assert not got[0][1, 128:256].any()
     # padding rows / keys are zero bytes
     nt = -(-n // 128)
@@ -117,7 +111,7 @@ def test_header_matches_restatement(core, n):
     # the dequantised operands are the bf16 ones within the e4m3 rounding
     kf, vf = R.dequant_kv(*[t.unsqueeze(0) for t in got], n)
     for x, xf in ((k, kf[0]), (v, vf[0])):
-        tol = x.float().abs().amax(dim=(0, 2)).view(1, hkv, 1) / 448 * 2.0 ** -6   # below the e4m3 normals
+        tol = x.float().abs().amax(dim=(0, 2)).view(1, hkv, 1) / FP8_MAX[E4M3] * 2.0 ** -6   # below the e4m3 normals
         assert bool(((xf - x.float()).abs() <= 2.0 ** -4 * x.float().abs() + tol).all())
 
 

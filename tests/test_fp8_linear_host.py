@@ -1,9 +1,8 @@
 """CPU tests of the FP8 (e4m3) decoder linears (ops.Fp8Weight, ops.linear_fp8, DecoderLayer(linear_dtype=...)).
 
-* The row quantiser of csrc/kv_fp8_core.h (lv_fp8_quant_row, the text quant_rows_fp8_kernel compiles), built with
-  gcc: byte for byte the torch.float8_e4m3fn restatement (tests/test_kv_fp8_host.quantise_heads, one row per "head")
-  for every finite bf16 value under several amax, zero rows and rows with a bf16-subnormal amax, at row lengths 5120
-  and 13 824.
+* The row quantiser of csrc/fp8_core.h (lv_fp8_quant_row, the text quant_rows_fp8_kernel compiles), built with gcc:
+  byte for byte the torch restatement (tests/fp8_ref.quant_rows_ref) for every finite bf16 value under several amax,
+  zero rows and rows with a bf16-subnormal amax, at row lengths 5120 and 13 824.
 * The wrappers with the recording stub library of tests/test_ops_args_host.py: the C calls of quant_rows_fp8 and of
   linear with an Fp8Weight (a row slice included), and every refusal with nothing recorded.
 * Host logic on the CPU oracle, with the FP8 twins below: a tiny FP8 model gives torch.equal logits across the
@@ -14,11 +13,7 @@
 The GPU twin is tests/test_gpu_fp8_linear.py.
 """
 import contextlib
-import ctypes as C
-import os
-import subprocess
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -27,64 +22,34 @@ from long_vita_b200 import ops
 from long_vita_b200.config import LongVITAConfig
 from long_vita_b200.hf import modeling
 from long_vita_b200.weights import synthetic_state_dict
-from tests.test_kv_fp8_host import _finite_bf16, quantise_heads
+from tests.fp8_ref import build_rows_shim, check_rows, finite_bf16, quant_rows_ref
 from tests.test_ops_args_host import P, _bf16, lib  # noqa: F401  (lib is the recording-stub fixture)
 from tests.test_row_chunks_host import _inputs
 from tests.test_stream_layer_host import _equal, _three_plans
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FP8 = torch.float8_e4m3fn
 
 
 # ------------------------------------------------------------------------------------------------
 # the shared quantiser built with gcc, against the restatement
 # ------------------------------------------------------------------------------------------------
-_SHIM = r"""
-#include "kv_fp8_core.h"
-void fp8_rows(const uint16_t* x, uint8_t* q, float* scale, long long rows, long long n) {
-  for (long long r = 0; r < rows; ++r) scale[r] = lv_fp8_quant_row(x + r * n, q + r * n, n);
-}
-"""
-
-
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    d = tmp_path_factory.mktemp("fp8_rows_host")
-    src, so = d / "fp8_rows_shim.c", str(d / "libfp8_rows_host.so")
-    src.write_text(_SHIM)
-    subprocess.run(["gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", "-I",
-                    os.path.join(ROOT, "long-vita_b200", "csrc"), str(src), "-o", so, "-lm"], check=True)
-    lib = C.CDLL(so)
-    lib.fp8_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong]
-    return lib
-
-
-def _check(core, x):
-    x = x.contiguous()
-    rows, n = x.shape
-    q = np.zeros((rows, n), dtype=np.uint8)
-    scale = np.zeros(rows, dtype=np.float32)
-    core.fp8_rows(x.view(torch.int16).numpy().ctypes.data_as(C.c_void_p), q.ctypes.data_as(C.c_void_p),
-                  scale.ctypes.data_as(C.c_void_p), rows, n)
-    q, scale = torch.from_numpy(q), torch.from_numpy(scale)
-    q_ref, scale_ref = quantise_heads(x)
-    bad = (q != q_ref).any(-1) | (scale.view(torch.int32) != scale_ref.view(torch.int32))
-    assert not bool(bad.any()), (int(bad.sum()), q[bad][:2], q_ref[bad][:2])
-    return q, scale
+    return build_rows_shim(tmp_path_factory.mktemp("fp8_rows_host"))
 
 
 @pytest.mark.parametrize("n", [5120, 13824])
 def test_every_finite_bf16_value_against_several_amax(core, n):
     """The finite bf16 values sorted by magnitude fill rows of n - 1; the last element of each row is its amax: the
-    row's largest |x| times 1 (x = +-amax, q = +-448), 3 and 2^8, 2^16, 2^24 (e4m3 subnormals and underflow)."""
-    x = _finite_bf16()
+    row's largest |x| times 1 (x = +-amax, q = +-M), 3 and 2^8, 2^16, 2^24 (e4m3 subnormals and underflow)."""
+    x = finite_bf16()
     x = x[x.float().abs().argsort()]
     x = torch.cat([x, x[-1:].expand(-len(x) % (n - 1))]).view(-1, n - 1)
     top = x.float().abs().amax(1, keepdim=True)
     for f in (1.0, 3.0, 2.0 ** 8, 2.0 ** 16, 2.0 ** 24):
         amax = (top * f).to(torch.bfloat16)
         keep = (torch.isfinite(amax.float()) & (amax.float() >= top))[:, 0]
-        q, _ = _check(core, torch.cat([x, amax], 1)[keep])
+        q, _ = check_rows(core, torch.cat([x, amax], 1)[keep])
         if f == 1.0:
             assert bool((q[top[keep, 0] >= 1e-30, -1] == 0x7E).all())
 
@@ -94,11 +59,11 @@ def test_zero_rows_and_subnormal_amax(core, n):
     g = torch.Generator().manual_seed(n)
     x = torch.zeros(6, n, dtype=torch.bfloat16)
     x[1] = -0.0
-    x[2, 5] = torch.tensor([1], dtype=torch.int16).view(torch.bfloat16)           # amax 9.2e-41: 448 / amax overflows
+    x[2, 5] = torch.tensor([1], dtype=torch.int16).view(torch.bfloat16)           # amax 9.2e-41: M / amax overflows
     x[3, :4] = torch.tensor([0, 1, 0x8001, 0x7F], dtype=torch.int32).to(torch.int16).view(torch.bfloat16)
     x[4] = (torch.randn(n, generator=g) * 1e-36).to(torch.bfloat16)               # inv finite
     x[5] = (torch.randn(n, generator=g) * 30).to(torch.bfloat16)
-    q, scale = _check(core, x)
+    q, scale = check_rows(core, x)
     assert bool((q[:4] == 0).all()) and bool((scale[:4] == 0).all()) and scale[4] > 0 and scale[5] > 0
 
 
@@ -119,8 +84,8 @@ def test_quant_rows_calls(lib):  # noqa: F811
     wide = _bf16(5, 72)
     q2, s2 = ops.quant_rows_fp8(wide[:, 8:56])                                # a strided view is read in place
     assert q.dtype == FP8 and s.dtype == torch.float32 and q.shape == (5, 48) and s.shape == (5,)
-    assert lib.calls == [("lv_quant_rows_fp8", P(x), P(q), P(s), 5, 48, 48),
-                         ("lv_quant_rows_fp8", P(wide) + 16, P(q2), P(s2), 5, 48, 72)]
+    assert lib.calls == [("lv_quant_rows_fp8_fmt", P(x), P(q), P(s), 5, 48, 48, 0),
+                         ("lv_quant_rows_fp8_fmt", P(wide) + 16, P(q2), P(s2), 5, 48, 72, 0)]
 
 
 def test_linear_fp8_calls(lib):  # noqa: F811
@@ -128,8 +93,8 @@ def test_linear_fp8_calls(lib):  # noqa: F811
     x, b = _bf16(2, 3, 64), _bf16(96)
     y = ops.linear(x, w, b)
     assert y.shape == (2, 3, 96)
-    (n0, xp, xq, xs, M, K, ldx), g = lib.calls
-    assert (n0, xp, M, K, ldx) == ("lv_quant_rows_fp8", P(x), 6, 64, 64)
+    (n0, xp, xq, xs, M, K, ldx, fmt), g = lib.calls
+    assert (n0, xp, M, K, ldx, fmt) == ("lv_quant_rows_fp8_fmt", P(x), 6, 64, 64, 0)
     assert g == ("lv_gemm_fp8", xq, xs, P(w.data), P(w.scale), P(b), P(y), 6, 96, 64, 64, 64, 96, 0)
     # a row slice of the weight (the streamed plan's Q and K|V launches) into rows of a wider buffer, and SwiGLU
     lib.calls.clear()
@@ -188,8 +153,8 @@ def test_only_contiguous_row_slices():
 # host logic on the CPU oracle, with FP8 twins
 # ------------------------------------------------------------------------------------------------
 def _quant_rows_twin(x):
-    """quant_rows_fp8 restated: the rule of kv_fp8_core.h per row (quantise_heads)."""
-    q, s = quantise_heads(x.reshape(-1, x.shape[-1]).cpu())
+    """quant_rows_fp8 restated (tests/fp8_ref.quant_rows_ref)."""
+    q, s = quant_rows_ref(x.reshape(-1, x.shape[-1]).cpu())
     return q.view(FP8), s
 
 

@@ -1,6 +1,6 @@
 """CPU tests of FP8 training of the `--spec` decoder layer (config.fp8 = "e4m3" / "hybrid").
 
-* The restatements of tests/fp8_train_ref.py, whose bytes the GPU quantisers must reproduce: the e5m2 row quantiser
+* The restatements of tests/fp8_ref.py, whose bytes the GPU quantisers must reproduce: the e5m2 row quantiser
   and the cast-transpose in both formats, with padding columns, all-zero columns, saturation at both formats' largest
   values and strided inputs.
 * ops.linear_fp8_autograd on the CPU oracle forms of the FP8 operators: the output and every gradient (dX, dW, the
@@ -20,7 +20,8 @@ import torch
 from long_vita_b200 import ops
 from long_vita_b200.config import LongVITAConfig
 from long_vita_b200.megatron import checkpoint as CK
-from tests.fp8_train_ref import (E4M3, E5M2, FP8_MAX, dequant, oracle_fp8_ops, quant_cols_t_ref, quant_rows_ref)
+from tests.fp8_ref import E4M3, E5M2, FP8_MAX, dequant, quant_cols_t_ref, quant_rows_ref
+from tests.fp8_train_ref import oracle_fp8_ops
 
 bf16, f32 = torch.bfloat16, torch.float32
 

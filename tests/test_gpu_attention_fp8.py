@@ -22,6 +22,7 @@ import torch
 
 from tests import attn_fp8_ref as R
 from tests.attn_fwd_ref import _sample_rows, check_planted
+from tests.fp8_ref import E4M3, FP8_MAX
 from tests.test_gpu_attention_fwd_ref import D, HKV, HQ, _inputs, _plant_edge_rows, _randn, _tile_rows
 
 pytestmark = pytest.mark.gpu
@@ -86,7 +87,8 @@ def test_quantiser_bytes(L):
         assert a.shape == b.shape, (name, a.shape, b.shape)
         assert torch.equal(a, b), (name, int((a != b).sum()))
     for s in (got[2], got[3]):
-        assert float(s[0, 1, 3]) == 0.0 and float(s[0, 2, 5]) == 0.0 and float(s[0, 0, 7]) == float(torch.tensor(1000.0) / 448)
+        assert float(s[0, 1, 3]) == 0.0 and float(s[0, 2, 5]) == 0.0
+        assert float(s[0, 0, 7]) == float(torch.tensor(1000.0) / FP8_MAX[E4M3])
 
 
 # ------------------------------------------------------------------------------------------------ kernel

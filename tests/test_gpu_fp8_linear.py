@@ -1,7 +1,7 @@
-"""The FP8 (e4m3) linears on the H100 (lv_quant_rows_fp8, lv_gemm_fp8, ops.linear with an ops.Fp8Weight).
+"""The FP8 (e4m3) linears on the H100 (lv_quant_rows_fp8_fmt, lv_gemm_fp8, ops.linear with an ops.Fp8Weight).
 
-* Quantiser: the rows lv_quant_rows_fp8 writes are byte for byte the CPU restatement of the rule
-  (tests/test_kv_fp8_host.quantise_heads, one "head" per row), at K = 5120 and 13 824, with zero rows, rows too small
+* Quantiser: the rows lv_quant_rows_fp8_fmt writes are byte for byte the CPU restatement of the rule
+  (tests/fp8_ref.quant_rows_ref), at K = 5120 and 13 824, with zero rows, rows too small
   to scale, magnitudes from 1e-30 to 1e30 and a strided input.
 * GEMM and GEMV against float64 over the dequantised operands (tests/gemm_ref.py: r = (A_q s_a) (W_q s_w)^T + bias,
   in float64), per 64 x 64 output chunk and elementwise:
@@ -32,7 +32,7 @@ import pytest
 import torch
 
 from tests.gemm_ref import check_gemm, gemm_ref
-from tests.test_kv_fp8_host import quantise_heads
+from tests.fp8_ref import quant_rows_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -77,7 +77,7 @@ def test_quant_rows_is_the_restatement(L, K):
     for src in (x, wide[:, 8 : 8 + K]):                                           # contiguous, and a strided view
         q, s = L.quant_rows_fp8(src)
         torch.cuda.synchronize()
-        q_ref, s_ref = quantise_heads(x.cpu())
+        q_ref, s_ref = quant_rows_ref(x.cpu())
         assert q.dtype == torch.float8_e4m3fn and s.dtype == torch.float32
         assert torch.equal(q.view(torch.uint8).cpu(), q_ref) and torch.equal(s.cpu().view(torch.int32),
                                                                            s_ref.view(torch.int32))

@@ -2,7 +2,7 @@
 lv_gemm_fp8_grad; ops.linear_fp8_autograd; B200TransformerLayer with config.fp8).
 
 * Quantisers: the bytes and scales of quant_rows_fp8 (e5m2) and quant_cols_fp8_t (e4m3, e5m2) equal the CPU
-  restatement of tests/fp8_train_ref.py, with zero columns, columns too small to scale, magnitudes from 1e-30 to 1e30,
+  restatement of tests/fp8_ref.py, with zero columns, columns too small to scale, magnitudes from 1e-30 to 1e30,
   padded token counts and a strided input.
 * dgrad and wgrad against float64 over the dequantised operands (tests/gemm_ref.py), per 64 x 64 output chunk and
   elementwise, with e4m3 and e5m2 A operands, for the four 14B decoder linears at T = 18 432, 16 897 (wgrad's
@@ -24,7 +24,7 @@ The weights are synthetic, so training quality on a real run is not measured her
 import pytest
 import torch
 
-from tests.fp8_train_ref import E4M3, E5M2, dequant, quant_cols_t_ref, quant_rows_ref
+from tests.fp8_ref import E4M3, E5M2, dequant, quant_cols_t_ref, quant_rows_ref
 from tests.gemm_ref import check_gemm, gemm_ref
 
 pytestmark = pytest.mark.gpu

@@ -1,7 +1,7 @@
 """The FP8 (e4m3) host tier of the K/V cache on the H100 (lv_rows_to_host_fp8, lv_attn_decode_host_fp8).
 
 * Quantiser: the rows lv_rows_to_host_fp8 writes from a QKV-buffer view and from a K|V buffer are byte for byte the
-  CPU restatement (tests/test_kv_fp8_host.fp8_rows), for 8 kv heads (2112-byte rows) and 1 (272-byte rows, padded
+  CPU restatement (tests/fp8_ref.fp8_rows), for 8 kv heads (2112-byte rows) and 1 (272-byte rows, padded
   scales), with zero heads; rows outside the destination view are untouched.
 * Decode kernel: against float64 attention over the dequantised rows (tests/attn_fwd_ref.check_attn_fwd,
   merged=True) from 1 to 1 058 816 rows, for the split counts of the bf16 test and G = 5 and 8.  Host bytes at and
@@ -17,7 +17,7 @@ import torch
 from tests.attn_fwd_ref import attention_fwd_ref, check_attn_fwd
 from tests.test_gpu_attention_fwd_ref import _plant_decode, _randn
 from tests.test_gpu_offloaded_cache import _model, _need_host, _placed
-from tests.test_kv_fp8_host import dequantise_rows, fp8_rows
+from tests.fp8_ref import dequantise_rows, fp8_rows
 
 pytestmark = pytest.mark.gpu
 

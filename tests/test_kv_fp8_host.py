@@ -1,25 +1,21 @@
 """CPU tests of the FP8 (e4m3) host tier of the K/V cache (kv_cache.OffloadedKVCache(host_dtype=torch.float8_e4m3fn)).
 
-* The quantiser of csrc/kv_fp8_core.h, the text the kernels compile, built with gcc: byte for byte the
-  torch.float8_e4m3fn restatement below (`fp8_rows`) for every finite bf16 value x paired with several amax >= |x|
-  (x = +-amax, e4m3 subnormals and underflow to zero included), zero heads and heads too small to scale.
+* The row quantiser of csrc/fp8_core.h, the text the kernels compile, built with gcc: byte for byte the torch
+  restatement of tests/fp8_ref.py (`quant_rows_ref`) for every finite bf16 value x paired with several amax >= |x|
+  (x = +-amax, subnormals and underflow to zero included) in e4m3 and e5m2, zero heads and heads too small to scale.
 * The wrappers' argument checks with the recording stub library: what they pass to lv_rows_to_host_fp8 and
   lv_attn_decode_host_fp8, and that nothing reaches the library on bad input.
 * Placement: the device-layer count does not depend on the host format at the product lengths, and an FP8 host tier
   takes 2112 / 4096 of the pinned bytes of a bf16 one.
 * `kv_host_dtype` reaches the cache from forward, generate and B200GPTVLModel; any other value is a ValueError.
 * On the CPU oracle, generate() with an FP8 host tier runs the FP8 row copy and decode (restated with `fp8_rows` /
-  `dequantise_rows`) and its prefill logits equal the bf16 offloaded cache's.
+  `dequantise_rows` of tests/fp8_ref.py) and its prefill logits equal the bf16 offloaded cache's.
 
 The GPU twin is tests/test_gpu_kv_fp8_host.py.
 """
 import contextlib
-import ctypes as C
-import os
-import subprocess
 import types
 
-import numpy as np
 import pytest
 import torch
 
@@ -28,106 +24,31 @@ from long_vita_b200.config import LongVITAConfig
 from long_vita_b200.hf import modeling
 from long_vita_b200.kv_cache import KVCache, OffloadedKVCache
 from long_vita_b200.megatron import checkpoint as ck
+from tests.fp8_ref import E4M3, E5M2, FP8_MAX, build_rows_shim, check_rows, dequantise_rows, finite_bf16, fp8_rows
 from tests.test_offloaded_cache_host import _free_on_80gb, _offload, tiny  # noqa: F401  (tiny is a fixture)
 from tests.test_ops_args_host import P, _bf16, lib  # noqa: F401  (lib is the recording-stub fixture)
 from tests.test_row_chunks_host import _inputs
 from tests.test_stream_layer_host import _constants, stream_oracle_ops
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FP8 = torch.float8_e4m3fn
-
-
-# ------------------------------------------------------------------------------------------------
-# the torch restatement of the row format and the quantisation rule (csrc/kv_fp8_core.h)
-# ------------------------------------------------------------------------------------------------
-def quantise_heads(x: torch.Tensor):
-    """x [..., d] bf16 -> (q [..., d] uint8 e4m3, scale [...] fp32): amax = max|x|, inv = 448 / amax, q =
-    e4m3(x * inv) rounded to nearest even, scale = amax / 448; a head whose inv is not finite is zeros, scale 0."""
-    xf = x.float()
-    amax = xf.abs().amax(-1, keepdim=True)
-    inv = torch.full_like(amax, 448.0) / amax          # one IEEE division (a scalar / tensor is reciprocal * scalar)
-    zero = torch.isinf(inv) | torch.isnan(inv)
-    q = (xf * inv).to(FP8).view(torch.uint8)
-    q = torch.where(zero, torch.zeros_like(q), q)
-    scale = torch.where(zero, torch.zeros_like(amax), amax / 448.0)[..., 0]
-    return q, scale
-
-
-def fp8_rows(k: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
-    """k / v [n, hkv, d] bf16 -> the FP8 host rows uint8 [n, ops.kv_fp8_row_bytes(hkv, d)]: K heads, V heads, then
-    the 2 hkv fp32 scales, zero-padded to 16 bytes."""
-    n, hkv, d = k.shape
-    q, scale = quantise_heads(torch.cat([k, v], dim=1).cpu())
-    pad = ops.kv_fp8_row_bytes(hkv, d) - 2 * hkv * d - 8 * hkv
-    return torch.cat([q.reshape(n, -1), scale.contiguous().view(torch.uint8).reshape(n, -1),
-                      torch.zeros(n, pad, dtype=torch.uint8)], dim=1)
-
-
-def dequantise_rows(rows: torch.Tensor, hkv: int, d: int):
-    """FP8 host rows -> (K, V) [n, hkv, d] fp32: float(q) * scale."""
-    n = rows.shape[0]
-    q = rows[:, : 2 * hkv * d].contiguous().view(FP8).float().view(n, 2 * hkv, d)
-    scale = rows[:, 2 * hkv * d : 2 * hkv * d + 8 * hkv].contiguous().view(torch.float32).view(n, 2 * hkv, 1)
-    x = q * scale
-    return x[:, :hkv], x[:, hkv:]
 
 
 # ------------------------------------------------------------------------------------------------
 # the shared quantiser built with gcc, against the restatement
 # ------------------------------------------------------------------------------------------------
-_SHIM = r"""
-#include "kv_fp8_core.h"
-void kv8_heads(const uint16_t* x, uint8_t* q, float* scale, long long heads, int d) {
-  for (long long h = 0; h < heads; ++h) scale[h] = lv_kv8_quant_head(x + h * d, q + h * d, d);
-}
-long long kv8_row_bytes(long long hkv, long long d) { return lv_kv8_row_bytes(hkv, d); }
-"""
-
-
 @pytest.fixture(scope="module")
 def core(tmp_path_factory):
-    d = tmp_path_factory.mktemp("kv8_host")
-    src, so = d / "kv8_shim.c", str(d / "libkv8_host.so")
-    src.write_text(_SHIM)
-    subprocess.run(["gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", "-I",
-                    os.path.join(ROOT, "long-vita_b200", "csrc"), str(src), "-o", so, "-lm"], check=True)
-    lib = C.CDLL(so)
-    lib.kv8_heads.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int]
-    lib.kv8_row_bytes.restype = C.c_longlong
-    lib.kv8_row_bytes.argtypes = [C.c_longlong, C.c_longlong]
-    return lib
+    return build_rows_shim(tmp_path_factory.mktemp("kv8_host"))
 
 
-def _heads(core, x: torch.Tensor):
-    """The header's quantiser over the heads x [heads, d] bf16."""
-    x = x.contiguous()
-    heads, d = x.shape
-    q = np.zeros((heads, d), dtype=np.uint8)
-    scale = np.zeros(heads, dtype=np.float32)
-    xs = x.view(torch.int16).numpy()
-    core.kv8_heads(xs.ctypes.data_as(C.c_void_p), q.ctypes.data_as(C.c_void_p), scale.ctypes.data_as(C.c_void_p),
-                   heads, d)
-    return torch.from_numpy(q), torch.from_numpy(scale)
-
-
-def _check(core, x):
-    q, scale = _heads(core, x)
-    q_ref, scale_ref = quantise_heads(x)
-    bad = (q != q_ref).any(-1) | (scale.view(torch.int32) != scale_ref.view(torch.int32))
-    assert not bool(bad.any()), (int(bad.sum()), x[bad][:4], q[bad][:4], q_ref[bad][:4])
-    return q
-
-
-def _finite_bf16():
-    x = torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16).view(torch.bfloat16)
-    return x[torch.isfinite(x.float())]
-
-
-def test_every_finite_bf16_value_against_several_amax(core):
-    """Heads of two values [x, amax]: amax is the head's max, so x is quantised with inv = 448 / amax exactly as in a
-    128-wide head.  amax = |x| (the +-amax edge, q = +-448), the next bf16 above, 3|x|, and 2^8 .. 2^24 |x| (e4m3
-    subnormals and underflow to +-0)."""
-    x = _finite_bf16()
+@pytest.mark.parametrize("dtype", [E4M3, E5M2], ids=["e4m3", "e5m2"])
+def test_every_finite_bf16_value_against_several_amax(core, dtype):
+    """Heads of two values [x, amax]: amax is the head's max, so x is quantised with inv = M / amax exactly as in a
+    128-wide head.  amax = |x| (the +-amax edge, q = +-M), the next bf16 above, 3|x|, and 2^8 .. 2^24 |x| (subnormals
+    of the format and underflow to +-0)."""
+    mx = FP8_MAX[dtype]
+    top = {E4M3: 0x7E, E5M2: 0x7B}[dtype]                           # the code of M
+    x = finite_bf16()
     ax = x.float().abs()
     for f in (1.0, None, 3.0, 2.0 ** 8, 2.0 ** 16, 2.0 ** 20, 2.0 ** 24):
         if f is None:                                               # one bf16 step above |x|
@@ -136,15 +57,15 @@ def test_every_finite_bf16_value_against_several_amax(core):
             amax = (ax * f).to(torch.bfloat16)
         keep = torch.isfinite(amax.float()) & (amax.float() >= ax)
         heads = torch.stack([x[keep], amax[keep]], dim=1)
-        q = _check(core, heads)
+        q, _ = check_rows(core, heads, dtype)
         big = (heads[:, 1].float() >= 1e-30)                                              # inv finite
         if f == 1.0:
-            assert bool((q[big, 1] == 0x7E).all())                                         # amax -> 448
-            assert bool(((q[big, 0] & 0x7F) == 0x7E)[heads[big, 0].float() != 0].all())   # x = +-amax -> +-448
-    # amax = 448 (inv = 1): every e4m3 code is reached, subnormals included, and none is NaN
-    x = x[x.float().abs() <= 448]
-    q = _check(core, torch.stack([x, torch.full_like(x, 448.0)], dim=1))
-    assert set(q[:, 0].tolist()) == set(range(256)) - {0x7F, 0xFF}
+            assert bool((q[big, 1] == top).all())                                          # amax -> M
+            assert bool(((q[big, 0] & 0x7F) == top)[heads[big, 0].float() != 0].all())    # x = +-amax -> +-M
+    # amax = M (inv = 1): every finite code is reached, subnormals included, and none is NaN or inf
+    x = x[x.float().abs() <= mx]
+    q, _ = check_rows(core, torch.stack([x, torch.full_like(x, mx)], dim=1), dtype)
+    assert set(q[:, 0].tolist()) == {c for c in range(256) if c & 0x7F <= top}
 
 
 def test_zero_heads_and_heads_too_small_to_scale(core):
@@ -152,12 +73,11 @@ def test_zero_heads_and_heads_too_small_to_scale(core):
     tiny = torch.tensor([0, 1, 0x8001, 0x7F], dtype=torch.int32).to(torch.int16).view(torch.bfloat16)  # subnormals
     heads = torch.zeros(6, d, dtype=torch.bfloat16)
     heads[1] = -0.0
-    heads[2, 5] = tiny[1]                                           # amax 9.2e-41: 448 / amax overflows
+    heads[2, 5] = tiny[1]                                           # amax 9.2e-41: M / amax overflows
     heads[3, :4] = tiny
     heads[4] = torch.randn(d).to(torch.bfloat16) * 1e-36            # amax ~ 3e-36: inv finite
-    heads[5, 7] = 2.0 ** -119                                       # just above 448 / FLT_MAX: inv = 448 * 2^119
-    q = _check(core, heads)
-    _, scale = _heads(core, heads)
+    heads[5, 7] = 2.0 ** -119                                       # just above M / FLT_MAX: inv = M * 2^119
+    q, scale = check_rows(core, heads)
     assert bool((q[:4] == 0).all()) and bool((scale[:4] == 0).all())
     assert scale[4] > 0 and scale[5] > 0 and q[5, 7] == 0x7E
 
@@ -166,7 +86,7 @@ def test_random_heads_and_rows(core):
     g = torch.Generator().manual_seed(5)
     x = (torch.randn(4096, 128, generator=g) * torch.logspace(-20, 20, 4096).unsqueeze(1)).to(torch.bfloat16)
     x[::7, :3] = 0
-    _check(core, x)
+    check_rows(core, x)
     assert core.kv8_row_bytes(8, 128) == ops.kv_fp8_row_bytes(8, 128) == 2112
     for hkv in (1, 2, 3, 4, 16):
         assert core.kv8_row_bytes(hkv, 128) == ops.kv_fp8_row_bytes(hkv, 128)
