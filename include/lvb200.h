@@ -385,6 +385,14 @@ int lv_attn_decode_host_fp8(const void* q, const void* kv_host, void* o_part, fl
                             int64_t capacity, int64_t hq, int64_t hkv, int64_t d, int64_t n_splits, float scale,
                             lv_stream_t stream);
 
+/* lv_kv_rows_dequant_fp8: FP8 host rows staged in device memory, src uint8 [rows, row bytes] (the format above, copied
+ * as they are), -> bf16 K|V rows dst [rows, 2 * hkv * d] (K of the hkv heads, then V), by the decode rule of
+ * csrc/fp8_core.h: each value becomes bf16_rn(float(q) * scale) with its head's scale, one fp32 multiply rounded to
+ * nearest.  The attention over host rows for several query tokens copies each chunk of rows to the device and runs
+ * lv_attn_fwd over it; this makes an FP8 chunk that call's bf16 operands.  HBM-bound.  d = 128, hkv divides 16, src
+ * and dst 16-byte aligned device memory. */
+int lv_kv_rows_dequant_fp8(const void* src, void* dst, int64_t rows, int64_t hkv, int64_t d, lv_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Dense linears (tensor-core roofline).  C[M,N] = act(A[M,K] . W[N,K]^T + bias[N]), bf16 in,
  * fp32 accumulate, bf16 out.  Replaces torch.matmul / te.Linear at layers.py:270,409, the ViT

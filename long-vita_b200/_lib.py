@@ -123,6 +123,7 @@ SIGNATURES = {
     "lv_rows_to_host_fp8": (c_i32, [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_ptr]),
     "lv_attn_decode_host_fp8": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_f32,
                                         c_ptr]),
+    "lv_kv_rows_dequant_fp8": (c_i32, [c_ptr, c_ptr, c_i64, c_i64, c_i64, c_ptr]),
     "lv_gemm_bias_act": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_ptr]),
     "lv_gemm_ex": (c_i32, [c_ptr, c_ptr, c_ptr, c_ptr, c_i64, c_i64, c_i64, c_i64, c_i64, c_i64, c_i32, c_i32, c_i32,
                            c_ptr]),

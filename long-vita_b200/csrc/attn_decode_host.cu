@@ -15,6 +15,10 @@
 // The FP8 host tier (opt-in, lossy) halves the bytes per row: e4m3 K | V with one fp32 scale per head and row, the
 // format and quantisation rule of fp8_core.h (2112 B per row at 8 kv heads).  rows_to_host_fp8_kernel quantises
 // device rows straight into the mapped host rows; attn_decode_host_fp8_kernel is the flash-decoding above over them.
+//
+// Several query tokens (a question about a prefilled context) do not read host rows in place: the rows are copied to
+// the device chunk by chunk (ops.attention_host_rows) and attended by lv_attn_fwd.  kv_rows_dequant_fp8_kernel decodes
+// an FP8 chunk, once it is in HBM, into the bf16 K|V rows that call reads.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -388,6 +392,57 @@ void launch_fp8(const __nv_bfloat16* q, const uint8_t* kv, __nv_bfloat16* o, flo
                                                                               scale_log2);
 }
 
+constexpr int kDequantThreads = 256;
+constexpr int kDequantUnroll = 4;      // rows in flight per lane
+
+// FP8 host rows staged in device memory -> bf16 K|V rows [rows, 2 hkv 128], by the decode rule of fp8_core.h.  Each
+// lane owns 16 e4m3 bytes of a row (one 16-byte load) and writes their 16 bf16 values (two 16-byte stores); the 8
+// lanes of a head read its scale (a 4-byte load the L1 serves once for them).  The 16 hkv lanes of a row are consecutive, so a CTA
+// covers 256 / (16 hkv) whole rows per step, and each lane issues the loads of kDequantUnroll rows before it converts
+// any of them.  HBM-bound: 2112 bytes read and 4096 written per row at 8 kv heads.
+__global__ void __launch_bounds__(kDequantThreads) kv_rows_dequant_fp8_kernel(const uint8_t* __restrict__ src,
+                                                                             __nv_bfloat16* __restrict__ dst,
+                                                                             int64_t rows, int hkv) {
+  const int vecs = 2 * hkv * kD / 16;
+  const int rows_per_step = kDequantThreads / vecs;
+  const int c = threadIdx.x % vecs, head = c / (kD / 16);   // head in [0, 2 hkv): K heads, then V heads
+  const int64_t row_bytes = lv_kv8_row_bytes(hkv, kD);
+  const int64_t row_elems = 2ll * hkv * kD;
+  const int64_t step = (int64_t)gridDim.x * rows_per_step;
+  for (int64_t base = (int64_t)blockIdx.x * rows_per_step + threadIdx.x / vecs; base < rows;
+       base += step * kDequantUnroll) {
+    uint4 x[kDequantUnroll];
+    float s[kDequantUnroll];
+#pragma unroll
+    for (int u = 0; u < kDequantUnroll; ++u) {
+      const int64_t row = base + u * step;
+      if (row < rows) {
+        const uint8_t* p = src + row * row_bytes;
+        x[u] = *reinterpret_cast<const uint4*>(p + 16 * c);
+        s[u] = *reinterpret_cast<const float*>(p + row_elems + 4 * head);
+      } else {
+        x[u] = make_uint4(0u, 0u, 0u, 0u);
+        s[u] = 0.f;
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kDequantUnroll; ++u) {
+      const int64_t row = base + u * step;
+      if (row < rows) {
+        float f[16];
+        e4m3x16_to_f32(x[u], f);
+        uint32_t w[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i)
+          w[i] = (uint32_t)lv_kv8_decode(f[2 * i], s[u]) | (uint32_t)lv_kv8_decode(f[2 * i + 1], s[u]) << 16;
+        uint4* o = reinterpret_cast<uint4*>(dst + row * row_elems + 16 * c);
+        o[0] = make_uint4(w[0], w[1], w[2], w[3]);
+        o[1] = make_uint4(w[4], w[5], w[6], w[7]);
+      }
+    }
+  }
+}
+
 // cudaPointerGetAttributes on `p`: LV_OK when it is pinned host memory, else an error naming `what`.
 int check_pinned_host(const void* p, const char* what) {
   cudaPointerAttributes a;
@@ -535,6 +590,23 @@ int lv_rows_to_host_fp8(void* host_dst, const void* src, int64_t rows, int64_t h
   rows_to_host_fp8_kernel<<<(unsigned)blocks, kQuantThreads, 0, (cudaStream_t)stream>>>(
       static_cast<const __nv_bfloat16*>(src), src_pitch / 2, static_cast<uint8_t*>(dst_dev), rows, (int)hkv);
   LV_CHECK_LAUNCH("rows_to_host_fp8_kernel");
+  return LV_OK;
+}
+
+int lv_kv_rows_dequant_fp8(const void* src, void* dst, int64_t rows, int64_t hkv, int64_t d, lv_stream_t stream) {
+  LV_CHECK_ARG(src && dst, "lv_kv_rows_dequant_fp8: null pointer");
+  LV_CHECK_ARG(d == kD, "lv_kv_rows_dequant_fp8: head_dim %lld not supported (128 only)", (long long)d);
+  LV_CHECK_ARG(hkv > 0 && kHalfWarps % hkv == 0, "lv_kv_rows_dequant_fp8: hkv %lld must divide 16", (long long)hkv);
+  LV_CHECK_ARG(rows > 0 && rows < (1ll << 40), "lv_kv_rows_dequant_fp8: bad rows %lld", (long long)rows);
+  LV_CHECK_ARG((uintptr_t)src % 16 == 0 && (uintptr_t)dst % 16 == 0,
+               "lv_kv_rows_dequant_fp8: source and destination must be 16-byte aligned");
+  LV_BIND_DEVICE(dst);
+  const int rows_per_step = kDequantThreads / (2 * (int)hkv * kD / 16);
+  const int64_t need = (rows + rows_per_step * kDequantUnroll - 1) / (rows_per_step * kDequantUnroll);
+  const int64_t cap = 8ll * lv::sm_count();
+  kv_rows_dequant_fp8_kernel<<<(unsigned)(need < cap ? need : cap), kDequantThreads, 0, (cudaStream_t)stream>>>(
+      static_cast<const uint8_t*>(src), static_cast<__nv_bfloat16*>(dst), rows, (int)hkv);
+  LV_CHECK_LAUNCH("kv_rows_dequant_fp8_kernel");
   return LV_OK;
 }
 

@@ -68,6 +68,33 @@ LV_FP8_HD float lv_fp8_scale(int fmt, float amax) {
 // A row stored as zeros: M / amax is not finite (amax = 0, or a subnormal amax).
 LV_FP8_HD int lv_fp8_zero_row(float inv) { return !(inv <= 3.40282347e38f); }
 
+// The decode rule of an FP8 K/V host row, for attention that runs over the rows in bf16: element x (the exact value of
+// its e4m3 byte) of a head whose scale is s becomes bf16_rn(x * s), one fp32 multiply rounded to nearest, then one
+// rounding to bf16, nearest even.  Returns the bf16 bits.
+#ifndef __CUDA_ARCH__
+// float -> bf16 bits, nearest even; a NaN becomes 0x7FC0 (the row format holds none: the quantiser saturates).
+LV_FP8_HD uint16_t lv_f32_to_bf16(float f) {
+  union {
+    float f;
+    uint32_t u;
+  } c;
+  c.f = f;
+  if (f != f) return 0x7FC0;
+  return (uint16_t)((c.u + 0x7FFFu + ((c.u >> 16) & 1u)) >> 16);
+}
+#endif
+
+LV_FP8_HD uint16_t lv_kv8_decode(float x, float s) {
+#ifdef __CUDA_ARCH__
+  uint16_t r;
+  asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(__fmul_rn(x, s)));
+  return r;
+#else
+  volatile float p = x * s;
+  return lv_f32_to_bf16(p);
+#endif
+}
+
 #ifdef __CUDACC__
 // Two products x * inv -> two bytes of the format (lo in the low byte): PTX cvt.rn.satfinite.{e4m3x2,e5m2x2}.f32, which
 // for the products of the rule (|v| <= M rounded up by the two divisions) gives exactly lv_fp8_encode.
@@ -105,6 +132,13 @@ static inline uint8_t lv_fp8_encode(int fmt, float f) {
   frexpf(a, &e);                                  // a = m * 2^e, m in [0.5, 1): 2^(e-1) <= a < 2^e
   const int q = (int)rintf(ldexpf(a, mbits + 1 - e));   // in [2^mbits, 2^(mbits+1)], exact scaling; the top carries
   return sign | (uint8_t)(((e - emin) << mbits) + (q - (1 << mbits)));
+}
+
+// e4m3 bits -> float, exact (0x7F and 0xFF are NaN).  The kernels convert with PTX cvt.rn.f16x2.e4m3x2, also exact.
+static inline float lv_e4m3_to_f32(uint8_t b) {
+  const int e = (b >> 3) & 15, m = b & 7;
+  const float a = (e == 15 && m == 7) ? NAN : e == 0 ? ldexpf((float)m, -9) : ldexpf((float)(8 + m), e - 10);
+  return (b & 0x80) ? -a : a;
 }
 
 // Quantise one row: x [n] bf16 bits -> q [n] in the format, returns the scale.  The kernels split a row over lanes,

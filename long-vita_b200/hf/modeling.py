@@ -25,7 +25,7 @@ import torch
 
 from .. import kv_cache, ops
 from ..config import LongVITAConfig
-from ..kv_cache import KVCache, OffloadedKVCache
+from ..kv_cache import ContextCache, ContextSession, KVCache, OffloadedKVCache
 
 
 @dataclass
@@ -428,12 +428,18 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: 
     `attn_dtype=torch.float8_e4m3fn` runs every call of several new tokens on the FP8 kernel (ops.attention_fwd_fp8:
     lossy, opt-in), whole-tensor, row-chunked and streamed alike; its blocks are aligned to key row 0, so the span
     calls of the streamed layer still give exactly the rows of the whole call.  One new token (decode) and the cache
-    contents stay bf16.  Packed rows (`cu_seqlens`) have no FP8 path: NotImplementedError, before anything runs."""
+    contents stay bf16.  Packed rows (`cu_seqlens`) have no FP8 path: NotImplementedError, before anything runs.
+
+    With a kv_cache.ContextSession (a question about a prefilled context) see context_step."""
     fp8 = check_attn_dtype(attn_dtype) == torch.float8_e4m3fn
     if fp8 and cu_seqlens is not None:
         raise NotImplementedError("packed samples (position ids restarting at 0) have no FP8 attention; use "
                                   "attn_dtype=torch.bfloat16")
     docs = ops.docs_kwargs(cu_seqlens)
+    if isinstance(cache, ContextSession):
+        if cu_seqlens is not None:
+            raise NotImplementedError(PACKED_WITH_CACHE)
+        return context_step(cache, rows)
 
     def prefill(q, k, v, **kw):
         fwd = ops.attention_fwd_fp8 if fp8 else ops.attention_fwd
@@ -469,6 +475,44 @@ def attention_step(cache=None, cu_seqlens: Optional[torch.Tensor] = None, rows: 
         if q.shape[0] == 1:
             return ops.attention_decode(q[0], kc, vc, length)
         return prefill(q, kc[:length], vc[:length])
+
+    return attend
+
+
+def context_step(session: ContextSession, rows: int):
+    """The attention step of a question about a prefilled context: each layer appends its new K/V rows to the session's
+    suffix, then attends its new rows over the context's P rows and over the suffix, each part with its log-sum-exp,
+    and merges the two parts (ops.merge_attention).
+
+    The context part is unmasked: on a device layer ops.attention_fwd over K[:P] (ops.attention_decode for one row),
+    on a host layer ops.attention_host_rows (ops.attention_decode_host or _fp8 for one row).  The suffix part is causal
+    attention over the suffix rows, aligned to the last key (ops.attention_decode for one row).  A question runs bf16
+    attention whatever the model's attn_dtype, as decode steps do.  A question that overflows the suffix raises before
+    anything is launched."""
+    session.check_rows(rows)
+    ctx, P = session.context.cache, session.prefix_len
+
+    def attend(li, q, k, v):
+        n, hq, d = q.shape
+        kc, vc, length = session.suffix.append(li, k, v)
+        if isinstance(ctx, OffloadedKVCache) and ctx.on_host(li):
+            host = ctx.host[li - ctx.n_dev]
+            if n == 1:
+                o1, l1 = ctx.decode_host(q[0], host, P, return_lse=True)
+            else:
+                o1, l1 = ops.attention_host_rows(q, host, P, return_lse=True)
+        elif n == 1:
+            o1, l1 = ops.attention_decode(q[0], ctx.k[li], ctx.v[li], P, return_lse=True)
+        else:
+            o1, l1 = ops.attention_fwd(q.unsqueeze(0), ctx.k[li][:P].unsqueeze(0), ctx.v[li][:P].unsqueeze(0),
+                                       causal=False, return_lse=True)
+        if n == 1:
+            o2, l2 = ops.attention_decode(q[0], kc, vc, length, return_lse=True)
+        else:
+            o2, l2 = ops.attention_fwd(q.unsqueeze(0), kc[:length].unsqueeze(0), vc[:length].unsqueeze(0), causal=True,
+                                       return_lse=True)
+        return ops.merge_attention(torch.stack([o1.view(n, hq, d), o2.view(n, hq, d)]),
+                                   torch.stack([l1.view(hq, n), l2.view(hq, n)]))
 
     return attend
 
@@ -619,7 +663,11 @@ class LongVITAModel(_WeightHolderModule):
         cfg = self.config
         if (input_ids is None) ^ (inputs_embeds is not None):
             raise ValueError("You must specify exactly one of input_ids or inputs_embeds")
-        if past_key_values is not None and not isinstance(past_key_values, (KVCache, OffloadedKVCache)):
+        if isinstance(past_key_values, ContextCache):
+            raise TypeError("a ContextCache is read-only: pass past_key_values=context.session(max_new_rows), a "
+                            "session with room for the question's and the answer's rows")
+        if past_key_values is not None and not isinstance(past_key_values, (KVCache, OffloadedKVCache,
+                                                                            ContextSession)):
             if len(past_key_values) != 0:
                 raise NotImplementedError("past_key_values must be the KVCache returned by a use_cache=True call")
             past_key_values = None
@@ -880,15 +928,41 @@ class LongVITAForCausalLM(_WeightHolderModule):
         return out if (return_dict is None or return_dict) else out.to_tuple()
 
     @torch.no_grad()
+    def prefill_context(self, input_ids: torch.Tensor, images: Optional[torch.Tensor] = None,
+                        image_indices: Optional[torch.Tensor] = None, *,
+                        kv_host_dtype=torch.bfloat16) -> ContextCache:
+        """Prefill a prompt (a long video) once, for several questions about it: the prefill of
+        `forward(use_cache=True, num_logits_to_keep=1, max_cache_len=s)` - the same placement of the cache, device or
+        partly in pinned host memory (`kv_host_dtype` for its host tier), the same streaming and the same logits - with
+        no spare rows, returned as a read-only kv_cache.ContextCache.  Ask with `generate(question, context=ctx)` or
+        `forward(input_ids=question, past_key_values=ctx.session(n), use_cache=True)`."""
+        dev = self.device
+        s = input_ids.shape[1]
+        if images is not None:
+            images = images.to(dev, dtype=torch.bfloat16)
+        if image_indices is not None:
+            image_indices = image_indices.to(dev)
+        out = self.forward(input_ids=input_ids.to(dev), images=images, image_indices=image_indices, use_cache=True,
+                           num_logits_to_keep=1, max_cache_len=s, kv_host_dtype=kv_host_dtype)
+        cfg = self.config
+        return ContextCache(out.past_key_values, out.logits, cfg.num_key_value_heads, cfg.head_dim)
+
+    @torch.no_grad()
     def generate(self, inputs: Optional[torch.Tensor] = None, images: Optional[torch.Tensor] = None,
                  image_indices: Optional[torch.Tensor] = None, generation_config=None, input_ids: Optional[torch.Tensor] = None,
                  max_new_tokens: Optional[int] = None, eos_token_id=None, do_sample: Optional[bool] = None,
-                 kv_host_dtype=torch.bfloat16, **kwargs):
+                 kv_host_dtype=torch.bfloat16, context: Optional[ContextCache] = None, **kwargs):
         """`model.generate(inputs=, images=, image_indices=)` as tools/inference_long_vita.py:868 calls it: greedy
         decoding (the script sets do_sample = False) with the K/V cache; stops at `eos_token_id` (int or list) or after
         `max_new_tokens`; returns prompt + generated ids [1, s + n] like transformers' GenerationMixin.  Inputs on the
         host are moved to the model's device (the script leaves them on the CPU under device_map="auto").
-        `kv_host_dtype=torch.float8_e4m3fn` keeps the host tier of a cache that does not fit in HBM in FP8 (lossy)."""
+        `kv_host_dtype=torch.float8_e4m3fn` keeps the host tier of a cache that does not fit in HBM in FP8 (lossy).
+
+        With `context` (a ContextCache from prefill_context), `inputs` is a question about the context's prompt: it
+        runs in a new session of the context (ContextCache.session), which the context outlives unchanged, and the
+        result is question + answer ids.  The images belong to the context's prompt, so none are taken here."""
+        if context is not None and images is not None:
+            raise ValueError("generate(context=): the images belong to the context's prompt (prefill_context)")
         gc = generation_config if generation_config is not None else self.generation_config
         ids = inputs if inputs is not None else input_ids
         if ids is None:
@@ -905,24 +979,29 @@ class LongVITAForCausalLM(_WeightHolderModule):
             images = images.to(dev, dtype=torch.bfloat16)
         if image_indices is not None:
             image_indices = image_indices.to(dev)
+        cache = None if context is None else context.session(ids.shape[1] + int(n_new))
         new = self.generate_greedy(ids, images, image_indices, max_new_tokens=int(n_new), eos_token_ids=eos,
-                                   kv_host_dtype=kv_host_dtype)
+                                   kv_host_dtype=kv_host_dtype, cache=cache)
         return torch.cat([ids, new], dim=1)
 
     @torch.no_grad()
     def generate_greedy(self, input_ids: torch.Tensor, images: Optional[torch.Tensor] = None,
                         image_indices: Optional[torch.Tensor] = None, max_new_tokens: int = 16,
                         eos_token_id: Optional[int] = None, eos_token_ids=None,
-                        kv_host_dtype=torch.bfloat16) -> torch.Tensor:
+                        kv_host_dtype=torch.bfloat16, cache=None) -> torch.Tensor:
         """Greedy decoding with the K/V cache: one prefill, then one forward per token over a single new
         row (the reference's Megatron loop feeds the whole sequence again for every token,
-        generation.py:127-135).  Returns the generated ids [1, n]."""
+        generation.py:127-135).  With `cache` (a kv_cache.ContextSession) the prefill is that of the input rows
+        after the cache's.  Returns the generated ids [1, n]."""
         s = input_ids.shape[1]
         stop = set(eos_token_ids or ())
         if eos_token_id is not None:
             stop.add(int(eos_token_id))
-        out = self.forward(input_ids=input_ids, images=images, image_indices=image_indices, use_cache=True,
-                           num_logits_to_keep=1, max_cache_len=s + max_new_tokens, kv_host_dtype=kv_host_dtype)
+        if cache is None:
+            out = self.forward(input_ids=input_ids, images=images, image_indices=image_indices, use_cache=True,
+                               num_logits_to_keep=1, max_cache_len=s + max_new_tokens, kv_host_dtype=kv_host_dtype)
+        else:
+            out = self.forward(input_ids=input_ids, past_key_values=cache, use_cache=True, num_logits_to_keep=1)
         cache = out.past_key_values
         new = []
         tok = out.logits[0, -1].float().argmax().view(1, 1)

@@ -22,6 +22,10 @@ buffers above, the others one pinned host buffer each, read in place by the deco
 The host tier may be kept in FP8 (`host_dtype=torch.float8_e4m3fn`): e4m3 K|V rows with one fp32 scale per head
 (csrc/fp8_core.h), 2112 instead of 4096 bytes per row at 8 kv heads, which halves both the pinned memory and the
 PCIe bytes a decode step reads.  It is lossy and opt-in; the default is bf16, and the device layers are bf16 either way.
+
+Several questions about one prompt (a long video) share its cache as a `ContextCache`: the filled cache of the
+prompt, never written again.  Each question runs in a `ContextSession`, the context plus a private device `KVCache`
+suffix for the question's and the answer's rows, so that a question costs a prefill of its own tokens only.
 """
 from __future__ import annotations
 
@@ -212,11 +216,11 @@ class OffloadedKVCache:
         to_host(k[kr - n :], v[kr - n :], host[r0:end])
         return host, end
 
-    def decode_host(self, q: torch.Tensor, host: torch.Tensor, length: int) -> torch.Tensor:
+    def decode_host(self, q: torch.Tensor, host: torch.Tensor, length: int, return_lse: bool = False):
         """One new token's attention over rows [0, length) of a host layer, in its format."""
         if self.host_dtype == torch.float8_e4m3fn:
-            return ops.attention_decode_host_fp8(q, host, length)
-        return ops.attention_decode_host(q, host, length)
+            return ops.attention_decode_host_fp8(q, host, length, return_lse=return_lse)
+        return ops.attention_decode_host(q, host, length, return_lse=return_lse)
 
     def commit(self) -> None:
         self._len += self._pending
@@ -232,3 +236,63 @@ class OffloadedKVCache:
     def host_bytes(self) -> int:
         """Pinned host bytes of the cache."""
         return sum(t.numel() * t.element_size() for t in self.host)
+
+
+class ContextCache:
+    """The read-only K/V cache of a prefilled prompt (LongVITAForCausalLM.prefill_context): `cache` (a filled KVCache
+    or OffloadedKVCache of len(cache) = P rows) and `logits`, those of the prompt's last token.  It has no append:
+    questions about the prompt run in sessions of their own (session()), and the context's rows stay as they are."""
+
+    def __init__(self, cache, logits: torch.Tensor, num_kv_heads: int, head_dim: int):
+        if len(cache) == 0:
+            raise ValueError("ContextCache: the cache holds no prompt")
+        self.cache = cache
+        self.logits = logits
+        self.num_kv_heads = int(num_kv_heads)
+        self.head_dim = int(head_dim)
+        self.num_layers = len(cache.k) + len(getattr(cache, "host", ()))
+
+    def __len__(self) -> int:
+        return len(self.cache)
+
+    def get_seq_length(self, layer_idx: int = 0) -> int:
+        return len(self.cache)
+
+    def session(self, max_new_rows: int) -> "ContextSession":
+        """A new ContextSession with room for `max_new_rows` rows of question and answer."""
+        return ContextSession(self, max_new_rows)
+
+
+class ContextSession:
+    """One question about a ContextCache: the context's P rows, read only, and a private device KVCache `suffix` of
+    `max_new_rows` rows per layer for the question's and the answer's rows.  Used as `past_key_values`, it takes the
+    cache's part: len() is P + the committed suffix rows, so positions continue at P + len(suffix), and commit /
+    commit_to advance the suffix.  The attention step (hf.modeling.attention_step) attends each new row over the
+    context and over the suffix, and merges the two."""
+
+    def __init__(self, context: ContextCache, max_new_rows: int):
+        if int(max_new_rows) <= 0:
+            raise ValueError(f"ContextSession: max_new_rows must be positive, got {max_new_rows}")
+        self.context = context
+        self.prefix_len = len(context)
+        self.suffix = KVCache(context.num_layers, int(max_new_rows), context.num_kv_heads, context.head_dim,
+                              context.logits.device)
+
+    def __len__(self) -> int:
+        return self.prefix_len + len(self.suffix)
+
+    def get_seq_length(self, layer_idx: int = 0) -> int:
+        return len(self)
+
+    def check_rows(self, rows: int) -> None:
+        """Refuses, before anything is launched, a forward of `rows` new tokens that overflows the suffix (the error
+        KVCache.append raises)."""
+        end = len(self.suffix) + rows
+        if end > self.suffix.capacity:
+            raise RuntimeError(f"KV cache overflow: {end} tokens > capacity {self.suffix.capacity}")
+
+    def commit(self) -> None:
+        self.suffix.commit()
+
+    def commit_to(self, offset: int) -> None:
+        self.suffix.commit_to(int(offset) - self.prefix_len)

@@ -650,6 +650,141 @@ def attention_decode_host_fp8(q: torch.Tensor, kv_host: torch.Tensor, length: in
     return decode_merge(o, lse, return_lse=return_lse)
 
 
+def merge_attention(o_part: torch.Tensor, lse_part: torch.Tensor, return_lse: bool = False):
+    """The attention of M query rows over the union of n disjoint key sets, from its n parts: o_part [n, M, hq, d] bf16
+    and lse_part [n, hq, M] fp32 (natural log; attention_fwd's lse without the batch) -> out [M, hq, d] (and lse
+    [hq, M]).  lv_attn_decode_merge with the M hq rows as the query heads of one kv head (G = M hq, hkv = 1), so
+    M hq < 2^20."""
+    n, M, hq, d = o_part.shape
+    if M * hq >= 1 << 20:
+        raise ValueError(f"merge_attention: {M} query rows of {hq} heads exceed the merge's 2^20 rows")
+    out, lse = decode_merge(o_part.reshape(n, M * hq, 1, d), lse_part.transpose(1, 2).reshape(n, 1, M * hq),
+                            return_lse=True)
+    out = out.view(M, hq, d)
+    return (out, lse.view(M, hq).t().contiguous()) if return_lse else out
+
+
+def kv_rows_dequant_fp8(src: torch.Tensor, hkv: int, d: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """FP8 host rows copied to the device, src uint8 [n, kv_fp8_row_bytes(hkv, d)], -> bf16 K|V rows [n, 2 hkv d]
+    (written to `out` if given), each value bf16_rn(float(q) * scale) (csrc/fp8_core.h; lv_kv_rows_dequant_fp8)."""
+    _need_cuda(src, torch.uint8)
+    if src.dim() != 2 or src.shape[1] != kv_fp8_row_bytes(hkv, d) or not src.is_contiguous():
+        raise ValueError(f"kv_rows_dequant_fp8: src must be contiguous FP8 rows [n, {kv_fp8_row_bytes(hkv, d)}], got "
+                         f"{tuple(src.shape)}")
+    n = src.shape[0]
+    if out is None:
+        out = torch.empty((n, 2 * hkv * d), dtype=torch.bfloat16, device=src.device)
+    _need_cuda_bf16(out)
+    if tuple(out.shape) != (n, 2 * hkv * d) or not out.is_contiguous():
+        raise ValueError(f"kv_rows_dequant_fp8: out must be a contiguous [{n}, {2 * hkv * d}], got {tuple(out.shape)}")
+    _call("lv_kv_rows_dequant_fp8", src.data_ptr(), out.data_ptr(), n, hkv, d)
+    return out
+
+
+def _copy_to_device(dst: torch.Tensor, src: torch.Tensor) -> None:
+    """dst.copy_(src) from pinned host rows, asynchronously on the current stream (the copy engine)."""
+    dst.copy_(src, non_blocking=True)
+
+
+HOST_ROWS_CHUNK = 65536
+HOST_ROWS_PARTS_BYTES = 1 << 30       # chunk results held at once by attention_host_rows before a merge
+
+
+def attention_host_rows(q: torch.Tensor, kv_host: torch.Tensor, length: int, *, chunk_rows: int = HOST_ROWS_CHUNK,
+                        return_lse: bool = False):
+    """M >= 1 query rows q [M, hq, d] (device) attend, unmasked, to the rows [0, length) of a host layer of the K/V
+    cache: kv_host pinned, bf16 [capacity, 2 hkv d] or FP8 uint8 [capacity, kv_fp8_row_bytes(hkv, d)].  Returns out
+    [M, hq, d] (and lse [hq, M] fp32, natural log).
+
+    The rows are not read in place: the copy engine stages them, `chunk_rows` at a time, into a ring of two device
+    buffers on a side stream, while the current stream runs the previous chunk; an FP8 chunk is copied as FP8 and
+    decoded to bf16 in HBM (kv_rows_dequant_fp8).  Each chunk is one attention_fwd over K / V views of the staged rows,
+    the ragged last one a shorter call, and the chunk results are merged by merge_attention.  So every host row
+    crosses PCIe once, whatever M is.  Stream order: the side stream first waits for the work enqueued before the
+    call (the rows may have just been written to the host), a buffer is refilled only after the call that read it, and
+    the current stream waits for each copy before it reads the buffer.  Refused with ValueError before anything is
+    launched: rows that are not pinned or not of the layer's width, length outside [1, capacity], a chunk_rows that is
+    not a positive multiple of 128, M hq >= 2^20.
+
+    The chunk results are held until they are merged: when all n of them would take more than HOST_ROWS_PARTS_BYTES
+    (many small chunks for many query rows), they are merged in groups of about sqrt(n) and the group results once
+    more, so that at most ~2 sqrt(n) of them exist at a time."""
+    _need_cuda_bf16(q)
+    op = "attention_host_rows"
+    if q.dim() != 3:
+        raise ValueError(f"{op}: q must be [M, hq, d], got {tuple(q.shape)}")
+    M, hq, d = q.shape
+    fp8 = kv_host.dtype == torch.uint8
+    _host_rows(op, "kv_host", kv_host, dtype=torch.uint8 if fp8 else torch.bfloat16)
+    cap, cols = kv_host.shape
+    hkv = cols // (2 * d + 8) if fp8 else cols // (2 * d)
+    if hkv == 0 or cols != (kv_fp8_row_bytes(hkv, d) if fp8 else 2 * hkv * d) or hq % hkv:
+        raise ValueError(f"{op}: kv_host rows of {cols} {'bytes' if fp8 else 'values'} are not "
+                         f"{'FP8 ' if fp8 else ''}K|V rows of kv heads of {d} for {hq} query heads")
+    if not 0 < length <= cap:
+        raise ValueError(f"{op}: length {length} outside the cache (capacity {cap})")
+    if chunk_rows <= 0 or chunk_rows % 128:
+        raise ValueError(f"{op}: chunk_rows {chunk_rows} is not a positive multiple of 128")
+    if M * hq >= 1 << 20:
+        raise ValueError(f"{op}: {M} query rows of {hq} heads exceed the merge's 2^20 rows")
+    n = -(-length // chunk_rows)
+    rows = min(chunk_rows, length)
+    group = n if n * M * hq * d * 2 <= HOST_ROWS_PARTS_BYTES else math.isqrt(n - 1) + 1
+    dev = q.device
+    cur = torch.cuda.current_stream(dev)
+    side = torch.cuda.Stream(device=dev)
+    stage = [torch.empty((rows, cols), dtype=kv_host.dtype, device=dev) for _ in range(2)]
+    kv = torch.empty((rows, 2 * hkv * d), dtype=torch.bfloat16, device=dev) if fp8 else None
+    o_part = torch.empty((group, M, hq, d), dtype=torch.bfloat16, device=dev)
+    lse_part = torch.empty((group, hq, M), dtype=torch.float32, device=dev)
+    groups = -(-n // group)
+    o_grp = torch.empty((groups, M, hq, d), dtype=torch.bfloat16, device=dev) if groups > 1 else None
+    lse_grp = torch.empty((groups, hq, M), dtype=torch.float32, device=dev) if groups > 1 else None
+    q4 = q.unsqueeze(0)
+
+    def after(stream):
+        ev = torch.cuda.Event()
+        ev.record(stream)
+        return ev
+
+    side.wait_event(after(cur))
+    ready, free = [None, None], [None, None]
+
+    def fill(i):
+        b, r0 = i % 2, i * chunk_rows
+        r1 = min(r0 + chunk_rows, length)
+        if free[b] is not None:
+            side.wait_event(free[b])
+        with torch.cuda.stream(side):
+            _copy_to_device(stage[b][: r1 - r0], kv_host[r0:r1])
+        ready[b] = after(side)
+
+    fill(0)
+    for i in range(n):
+        if i + 1 < n:
+            fill(i + 1)
+        b, r = i % 2, min(chunk_rows, length - i * chunk_rows)
+        cur.wait_event(ready[b])
+        rows_i = stage[b][:r]
+        if fp8:
+            rows_i = kv_rows_dequant_fp8(rows_i, hkv, d, out=kv[:r])
+            free[b] = after(cur)
+        k = rows_i[:, : hkv * d].view(r, hkv, d).unsqueeze(0)
+        v = rows_i[:, hkv * d :].view(r, hkv, d).unsqueeze(0)
+        j = i % group
+        _, lse = attention_fwd(q4, k, v, causal=False, return_lse=True, out=o_part[j : j + 1])
+        lse_part[j].copy_(lse[0])
+        if not fp8:
+            free[b] = after(cur)
+        if groups > 1 and (j == group - 1 or i == n - 1):
+            o, lse = merge_attention(o_part[: j + 1], lse_part[: j + 1], return_lse=True)
+            o_grp[i // group].copy_(o)
+            lse_grp[i // group].copy_(lse)
+    if groups > 1:
+        return merge_attention(o_grp, lse_grp, return_lse=return_lse)
+    return merge_attention(o_part, lse_part, return_lse=return_lse)
+
+
 # ------------------------------------------------------------------------------------------------
 # token-wise operators
 # ------------------------------------------------------------------------------------------------
