@@ -9,9 +9,20 @@
   the last query tile - the diagonal tiles and the ragged last tile - make a one-key mask error O(1).
 * Streamed spans q[r0:r1] over k[:r1] (sq < sk, r0 a multiple of 128) are torch.equal to those rows of the whole call,
   output and LSE; a repeated call is bit-identical (static schedule) and return_lse=False changes no bit.
+* The calls a filled K/V cache makes, against the same reference with every row planted (sq <= 300; beyond, the
+  first, middle and last query tiles), each also bit-identical on a second call and without the LSE:
+  `test_cache_offsets` (sq < sk, sk - sq = 1, 63, 64, 65, 72, 87, 127 mod 128 and two aligned controls: every offset
+  of the diagonal inside a key tile and a 64-row Q group, a partial last Q tile, a grid smaller than the SM count),
+  `test_short_prompts` (sq = sk from 1 to 1000 around 64 and 128), `test_abi_edges` (GQA 8:8, 64:8 and 5:1; batch 2
+  and 3 with distinct plants per entry; scales 0.02 and 0.5 on inputs x4; QKV column views with out= a column view
+  of a wider buffer; zero Q groups on a diagonal tile and in the ragged last Q tile, the FLT_MIN substitute for
+  their zero scale; a 1000x row setting its group's scale).  A negative control: the kernel's output on a planted
+  cache call fails against a reference whose query positions are shifted by one key either way.
 * A 4-layer model of the 14B geometry at 18 432 tokens: FP8 against bf16 attention (relative Frobenius difference of
   the prefill logits, greedy agreement over 16 teacher-forced steps), and the whole-tensor, row-chunked and streamed
-  plans give torch.equal logits with FP8 attention.
+  plans give torch.equal logits with FP8 attention.  `test_kv_cache_turns`: a prefill of 18 432 tokens into a device
+  KVCache, forwards of 3, 37 and 300 tokens on it and a decode step; every FP8 call of the three forwards (12, sk =
+  18 435, 18 472, 18 772) against float64, and each step's logits against the bf16 model.
 
 The figures are printed (`pytest -s`); DESIGN.md lists them against the limits.
 """
@@ -21,7 +32,7 @@ import pytest
 import torch
 
 from tests import attn_fp8_ref as R
-from tests.attn_fwd_ref import _sample_rows, check_planted
+from tests.attn_fwd_ref import _sample_rows, attention_fwd_ref, check_planted, plant_keys
 from tests.fp8_ref import E4M3, FP8_MAX
 from tests.test_gpu_attention_fwd_ref import D, HKV, HQ, _inputs, _plant_edge_rows, _randn, _tile_rows
 
@@ -41,8 +52,8 @@ def L(lib_built):
           f"peak extra device memory {(torch.cuda.max_memory_allocated() - base) / 2**30:.1f} GiB")
 
 
-def _check(out, lse, q, k, v, *, rows=None, label):
-    ref = R.reference(q, k, v, q_rows=rows)
+def _check(out, lse, q, k, v, *, rows=None, scale=None, label):
+    ref = R.reference(q, k, v, q_rows=rows, scale=scale)
     if rows is not None:
         r = rows.to(out.device)
         out, lse = out[:, r], lse[:, :, r]
@@ -53,11 +64,13 @@ def _check(out, lse, q, k, v, *, rows=None, label):
     return ref
 
 
-def _check_plants(ref, rows, q, k, v, planted):
+def _check_plants(ref, rows, q, k, v, planted, entry=None):
     """A plant must still dominate (or stay hidden) after quantisation: judged on the reference over the dequantised
-    V, whose rows the kernel output is held to."""
+    V, whose rows the kernel output is held to.  `entry`: the plants of that batch entry alone."""
     k8, vt8, ks, vs = R.quant_kv(k, v)
     _, vf = R.dequant_kv(k8, vt8, ks, vs, k.shape[1])
+    if entry is not None:
+        ref, vf = {"out": ref["out"][entry:entry + 1]}, vf[entry:entry + 1]
     rh, th, rv, tv = planted
     if rh.numel():
         check_planted(ref, vf, torch.searchsorted(rows, rh), th, visible=False)
@@ -155,6 +168,142 @@ def test_argument_errors(L):
         L.attention_fwd_fp8(q64, k64, v64, causal=True)
 
 
+# ------------------------------------------------------------------------------------------------ cache calls and edges
+def _plant(q, k, rows=None, skip=None, scale=None):
+    """Plant `rows` (None = all; minus `skip`) of every batch entry at their bottom-right aligned positions: rows
+    alternately want their first hidden key and their diagonal key (plant_keys at `scale`), the alternation of entry
+    e shifted by e so that the entries' plants differ.  Returns (hidden rows, targets, visible rows, targets) per
+    entry."""
+    sq, sk = q.shape[1], k.shape[1]
+    rows = torch.arange(sq) if rows is None else rows
+    if skip is not None:
+        rows = rows[~torch.isin(rows, skip)]
+    pos = rows + (sk - sq)
+    planted = []
+    for e in range(q.shape[0]):
+        hid = ((torch.arange(rows.numel()) + e) % 2 == 0) & (pos + 1 < sk)
+        plant_keys(q[e:e + 1], k[e:e + 1], torch.cat([rows[hid], rows[~hid]]), torch.cat([pos[hid] + 1, pos[~hid]]),
+                   scale=scale)
+        planted.append((rows[hid], pos[hid] + 1, rows[~hid], pos[~hid]))
+    return planted
+
+
+def _run(L, q, k, v, *, label, planted=(), scale=None, rows=None, out=None):
+    """One call against the float64 reference on `rows` (None = all) - lse, elementwise, per-row Z, exact zeros - and
+    each entry's plants; return_lse=False gives the same bits and a second call is bit-identical."""
+    o, lse = L.attention_fwd_fp8(q, k, v, causal=True, return_lse=True, scale=scale, out=out)
+    ref = _check(o, lse, q, k, v, rows=rows, scale=scale, label=label)
+    checked = torch.arange(q.shape[1]) if rows is None else rows
+    for e, p in enumerate(planted):
+        _check_plants(ref, checked, q, k, v, p, entry=e)
+    del ref
+    assert torch.equal(L.attention_fwd_fp8(q, k, v, causal=True, scale=scale), o)
+    o2, lse2 = L.attention_fwd_fp8(q, k, v, causal=True, return_lse=True, scale=scale)
+    assert torch.equal(o2, o) and torch.equal(lse2, lse)
+    return o, lse
+
+
+def _plant_rows(sq):
+    """Every row up to 300 rows; beyond, the first, middle and last query tiles."""
+    n_t = -(-sq // 128)
+    return None if sq <= 300 else _tile_rows([0, n_t // 2, n_t - 1], sq)
+
+
+# (sq, sk) of a forward over a filled cache: sk - sq = 1, 1, 127, 72, 1, 63, 64, 65, 127, 87 (mod 128), then two
+# aligned controls (0 mod 128; 16 897 has a one-key last tile)
+CACHE_CALLS = [(1, 2), (1, 130), (2, 129), (3, 203), (37, 18470), (63, 18558), (64, 18560), (65, 18562),
+               (200, 18759), (300, 18435), (4096, 22528), (129, 16897)]
+
+
+@pytest.mark.parametrize("sq,sk", CACHE_CALLS)
+def test_cache_offsets(L, sq, sk):
+    """q = the new rows, k / v = the cache's first sk rows, as hf/modeling.attention_step calls the kernel on a filled
+    KVCache: the diagonal crosses a key tile at every kind of offset inside it and inside a 64-row Q group (each
+    consumer warpgroup's first masked tile, `j_mask`, differs from its neighbour's), the last Q tile is partial (TMA
+    zero fill in the Q amax) and for sq <= 128 the grid (40 items) is smaller than the SM count."""
+    q, k, v = _inputs(1, sq, sk, HQ, HKV, D, seed=sq * 31 + sk)
+    planted = _plant(q, k, _plant_rows(sq))
+    _run(L, q, k, v, planted=planted, label=f"fp8 cache {sq}x{sk}")
+
+
+@pytest.mark.parametrize("s", [1, 2, 63, 64, 65, 127, 128, 129, 191, 255, 257, 1000])
+def test_short_prompts(L, s):
+    """sq = sk below, at and above one 64-row Q group and one 128-row tile: a single partial work item, an empty
+    second consumer half (s <= 64), ragged first and last key tiles."""
+    q, k, v = _inputs(1, s, s, HQ, HKV, D, seed=s + 4)
+    planted = _plant(q, k, _plant_rows(s))
+    _run(L, q, k, v, planted=planted, label=f"fp8 short {s}")
+
+
+ABI_EDGES = ["gqa_8_8", "gqa_64_8", "gqa_5_1", "batch_2", "batch_3", "scale_0.02", "scale_0.5_x4", "qkv_views",
+             "zero_q_groups", "outlier_row"]
+
+
+@pytest.mark.parametrize("case", ABI_EDGES)
+def test_abi_edges(L, case):
+    """300 new rows over 1000 keys (sk - sq = 700 = 60 mod 128), 40:8 unless stated.  GQA ratios 1, 8 and 5 with one
+    kv head; batch 2 and 3 (`row_base` of the K8 / Vt8 maps, the per-entry scales), each entry with its own data and
+    plants; an explicit scale, and scale 0.5 on inputs x4 (logits of a few hundred, near one-hot rows, not planted);
+    q / k / v as column views of one QKV buffer [T, (hq + 2 hkv) 128] with out= a column view of a wider buffer (sq =
+    sk = 1000, as the prefill passes them); an all-zero Q group across a diagonal tile and one in the ragged last Q
+    tile (scale 0: the FLT_MIN substitute keeps the masked logits -inf); a Q group whose scale one 1000x row sets."""
+    b, sq, sk, hq, hkv = 1, 300, 1000, HQ, HKV
+    hq, hkv = {"gqa_8_8": (8, 8), "gqa_64_8": (64, 8), "gqa_5_1": (5, 1)}.get(case, (hq, hkv))
+    b = {"batch_2": 2, "batch_3": 3}.get(case, b)
+    scale = {"scale_0.02": 0.02, "scale_0.5_x4": 0.5}.get(case)
+    seed = 1000 + ABI_EDGES.index(case)
+    out = None
+    if case == "qkv_views":
+        sq = sk = 1000
+        g = torch.Generator(device="cuda").manual_seed(seed)
+        qkv = _randn((1, sk, (hq + 2 * hkv) * D), g)
+        q = qkv[..., :hq * D].unflatten(-1, (hq, D))
+        k = qkv[..., hq * D:(hq + hkv) * D].unflatten(-1, (hkv, D))
+        v = qkv[..., (hq + hkv) * D:].unflatten(-1, (hkv, D))
+        buf = torch.full((1, sq, (hq + 8) * D), 7.0, dtype=torch.bfloat16, device="cuda")
+        out = buf[..., 4 * D:(hq + 4) * D].unflatten(-1, (hq, D))
+        assert not any(t.is_contiguous() for t in (q, k, v, out))
+    else:
+        q, k, v = _inputs(b, sq, sk, hq, hkv, D, seed=seed)
+    skip = {"zero_q_groups": torch.cat([torch.arange(64, 128), torch.arange(256, 300)]),
+            "outlier_row": torch.arange(64, 128)}.get(case)
+    if case == "scale_0.5_x4":
+        q, k, v = ((t.float() * 4).to(torch.bfloat16) for t in (q, k, v))
+        planted = []
+    else:
+        planted = _plant(q, k, _plant_rows(sq), skip, scale)
+    if case == "zero_q_groups":
+        q[0, 64:128, 7] = 0                           # the second half of the first Q tile: a diagonal tile
+        q[0, 256:300, 12] = 0                         # the last Q tile's only group, 44 rows + zero fill
+    elif case == "outlier_row":
+        q[0, 70, 5] = (q[0, 70, 5].float() * 1000).to(torch.bfloat16)
+    o, _ = _run(L, q, k, v, planted=planted, scale=scale, out=out, label=f"fp8 abi {case}")
+    if case == "qkv_views":
+        assert o.data_ptr() == out.data_ptr()
+        assert torch.equal(out, L.attention_fwd_fp8(q.contiguous(), k.contiguous(), v.contiguous(), causal=True))
+        rest = torch.ones(buf.shape, dtype=torch.bool, device="cuda")
+        rest[..., 4 * D:(hq + 4) * D] = False
+        assert bool((buf[rest] == 7.0).all())
+
+
+def test_negative_control_shifted_positions(L):
+    """The kernel's result on a planted cache call (37 rows over 18 470 keys) passes against the reference and fails
+    against one whose query positions are shifted by one either way: on GPU data the plants make a one-key mask
+    error visible."""
+    sq, sk = 37, 18470
+    q, k, v = _inputs(1, sq, sk, HQ, HKV, D, seed=77)
+    _plant(q, k)
+    out, lse = L.attention_fwd_fp8(q, k, v, causal=True, return_lse=True)
+    R.check(out, lse, R.reference(q, k, v), label="control")
+    kf, vf = R.dequant_kv(*R.quant_kv(k, v), sk)
+    qf = R.quant_q(q)
+    for shift in (-1, 1):
+        ref = R.reference(q, k, v)
+        ref.update(attention_fwd_ref(qf, kf, vf, causal=True, q_pos=torch.arange(sq) + (sk - sq) + shift))
+        with pytest.raises(AssertionError):
+            R.check(out, lse, ref, label=f"positions shifted by {shift}")
+
+
 # ------------------------------------------------------------------------------------------------ model
 @pytest.fixture(scope="module")
 def M(lib_built):
@@ -216,3 +365,64 @@ def test_model_plans_bit_identical(M, monkeypatch):
             logits[name] = models[torch.float8_e4m3fn](input_ids=ids, num_logits_to_keep=64).logits
     assert torch.isfinite(logits["whole"]).all()
     assert torch.equal(logits["whole"], logits["chunked"]) and torch.equal(logits["whole"], logits["streamed"])
+
+
+# Limit from the measurement on an H100 80GB HBM3 at 700 W (DESIGN.md §8): relative logit difference of each step of
+# test_kv_cache_turns at most 0.042 (the prefill's last token; the forwards of 3, 37 and 300 tokens 0.035 - 0.037, the
+# decode step 0.011), limit about 2x.
+TURN_REL_LIMIT = 0.08
+
+
+def test_kv_cache_turns(M, monkeypatch):
+    """A prefill of 18 432 tokens into a device KVCache, forwards of 3, 37 and 300 tokens on the filled cache, then
+    one decode step, with FP8 attention.  Every FP8 call is recorded (ops.attention_fwd_fp8 wrapped; modeling looks it
+    up at call time): the shapes are sk = 18 432 + the rows so far, and each of the 12 turn calls is checked against
+    the float64 reference on all rows (the prefill of layer 0 on sampled rows).  Each step's logits against the bf16
+    model on the same ids (relative Frobenius difference)."""
+    from long_vita_b200.kv_cache import KVCache
+
+    cfg, models, modeling = M
+    T, turns = 18432, (3, 37, 300)
+    ids = _ids(cfg, T + sum(turns) + 1, seed=13)
+    real = modeling.ops.attention_fwd_fp8
+    shapes, kept = [], []
+
+    def recorded(q, k, v, causal=True, return_lse=False, **kw):
+        out, lse = real(q, k, v, causal=causal, return_lse=True, **kw)
+        shapes.append((q.shape[1], k.shape[1]))
+        if len(shapes) == 1 or q.shape[1] < k.shape[1]:          # the prefill of layer 0, and every turn call
+            kept.append(tuple(t.clone() for t in (q, k, v, out, lse)))
+        return (out, lse) if return_lse else out
+
+    monkeypatch.setattr(modeling.ops, "attention_fwd_fp8", recorded)
+    ends = [T]
+    for n in turns + (1,):
+        ends.append(ends[-1] + n)
+    logits = {}
+    for dt, model in models.items():
+        cache = KVCache(cfg.num_hidden_layers, ids.shape[1], cfg.num_key_value_heads, cfg.head_dim, "cuda")
+        steps = []
+        with torch.no_grad():
+            for a, e in zip([0] + ends[:-1], ends):
+                out = model(input_ids=ids[:, a:e], past_key_values=cache, use_cache=True,
+                            num_logits_to_keep=1 if a == 0 else e - a)
+                steps.append(out.logits[0].float())
+        assert len(cache) == ids.shape[1]
+        logits[dt] = steps
+    n_layers = cfg.num_hidden_layers
+    want = [(T, T)] * n_layers
+    for a, e in zip(ends[:-2], ends[1:-1]):
+        want += [(e - a, e)] * n_layers
+    assert shapes == want, shapes
+    q, k, v, out, lse = kept[0]
+    rows = torch.unique(torch.cat([_sample_rows(96, T, seed=13), torch.arange(T - 128, T)]))
+    _check(out, lse, q, k, v, rows=rows, label="fp8 turns: prefill layer 0 sampled")
+    for i, (q, k, v, out, lse) in enumerate(kept[1:]):
+        _check(out, lse, q, k, v, label=f"fp8 turns: {q.shape[1]}x{k.shape[1]} layer {i % n_layers}")
+    print(f"[attn_fp8 turns] {len(kept) - 1} turn calls checked")
+    assert len(kept) - 1 == len(turns) * n_layers
+    for name, lb, l8 in zip(("prefill", "turn 3", "turn 37", "turn 300", "decode"), logits[torch.bfloat16],
+                            logits[torch.float8_e4m3fn]):
+        rel = float((l8 - lb).norm() / lb.norm())
+        print(f"[attn_fp8 turns] {name}: logits rel Frobenius {rel:.4g}")
+        assert torch.isfinite(l8).all() and rel < TURN_REL_LIMIT, (name, rel)
